@@ -1,6 +1,6 @@
 """bench.py — vectors quantized / second at dim=256, codebook=1024 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload cfg2|cfg5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload cfg2|cfg5] [--dump-outputs DIR]
 
 Workload (N=1 and per GPU for N>1): BASELINE.json configs[1] — VectorQuantize(dim=256, codebook_size=1024),
 x = (64, 4096, 256) bf16, training-mode forward with the EMA codebook update.  A "step" is one such
@@ -10,7 +10,10 @@ Under torchrun every rank runs the same per-GPU batch (weak scaling) with sync_c
 statistics are summed over the ranks inside the EMA kernels (NVLink peer loads from symmetric memory after one
 barrier kernel; ONE NCCL all-reduce if symmetric memory is unavailable); the time is the max over ranks.
 
-`--impl reference` times the UNMODIFIED reference package (baseline/_ref) on the host cores — its own
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (quantized, indices, loss) as DIR/<name>.npy
+(float32; indices float64) after the timed steps: the inputs are seeded, so two builds can be compared output for output.
+
+`--impl reference` times the UNMODIFIED reference package (oracle/_ref, see oracle/ref_loader.py) on the host cores — its own
 VectorQuantize(dim=256, codebook_size=1024) training-mode forward on the full 262144-vector batch — and falls back
 to the torch-CPU oracle port (oracle/vq_oracle_torch.py, the same ATen op sequence) only if the package cannot be
 imported, saying so in `cpu_baseline.kind`.
@@ -38,7 +41,7 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback (NVIDIA H100 SXM data sheet: dense bf16, 700 W)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -53,7 +56,7 @@ CPU_FULL_BATCH = (B, T)          # the reference arm runs the WHOLE config-2 bat
 def cpu_reference_step_factory(threads=None):
     """One training-mode forward of the reference on the host cores, on the full BASELINE config-2 batch.
 
-    Preferred: the UNMODIFIED reference package (`baseline/_ref`, pip-installed from /root/reference; `oracle/ref_loader.py`)
+    Preferred: the UNMODIFIED reference package (`oracle/_ref` or $VQB_REFERENCE_ROOT; `oracle/ref_loader.py`)
     through its own public API — `VectorQuantize(dim=256, codebook_size=1024)(x)` — kind "reference".  If it cannot be
     imported on this box: the torch-CPU oracle port (the same ATen op sequence, bit-identical on the goldens), kind "port"."""
     import torch
@@ -110,7 +113,7 @@ def time_cpu(steps, warmup):
 
 
 def cpu_baseline_block(value):
-    what = ("the UNMODIFIED reference package (baseline/_ref), VectorQuantize(dim=256, codebook_size=1024) training-mode forward on CPU"
+    what = ("the UNMODIFIED reference package, VectorQuantize(dim=256, codebook_size=1024) training-mode forward on CPU"
             if CPU_KIND[0] == "reference" else
             "oracle/vq_oracle_torch.py (the reference's ATen op sequence: N x K fp32 distances, one-hot, 3 sgemm)")
     return {"value": value, "unit": "vectors/s", "cores": CPU_THREADS[0] or os.cpu_count(), "host_cores": os.cpu_count(),
@@ -141,31 +144,34 @@ def run_reference_arm(args):
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md "clocks line")
+# clocks sampler
 # ------------------------------------------------------------------------------------------------
 
-NCU_SUMMARY = "r2_assign_benched_summary.txt"   # ncu --set full of the search launch as benched (scripts/r2_profile.sh)
+DUMP_ROWS = 16384   # rows of `quantized` / `indices` kept by --dump-outputs (a fixed, seeded sample: <= 64 MB in all)
 
 
-def ncu_dram_bytes():
-    """dram read + write bytes of one vq_assign_kernel launch, from the committed ncu summary (None if it is missing)."""
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", NCU_SUMMARY)
-    mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    total, seen = 0.0, 0
-    try:
-        for line in open(path):
-            if "dram__bytes_read.sum =" in line or "dram__bytes_write.sum =" in line:
-                val, unit = line.split("=")[1].split()[:2]
-                total += float(val) * mult[unit]
-                seen += 1
-    except Exception:
-        return None
-    return total if seen == 2 else None
+def dump_outputs(out_dir, outputs):
+    """Write the arrays a caller of the timed path received (device tensors) as float32 / float64 .npy files.  Leading
+    dimensions are flattened to rows (indices: the first two, one row per vector); larger outputs keep the same seeded
+    sample of DUMP_ROWS rows."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    rows = None
+    for name, t in outputs.items():
+        a = t.detach().cpu()
+        a = a.float().numpy() if a.is_floating_point() else a.double().numpy()
+        if name != "loss" and a.ndim >= 2:
+            a = a.reshape(-1, a.shape[-1]) if name == "quantized" else a.reshape(a.shape[0] * a.shape[1], -1)
+            if a.shape[0] > DUMP_ROWS:
+                if rows is None:
+                    rows = np.sort(np.random.default_rng(0).choice(a.shape[0], DUMP_ROWS, replace=False))
+                a = a[rows]
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a))
 
 
 def pin_to_gpu_numa_node(local):
     """Bind this rank (and its pinned host buffers, by first touch) to the NUMA node its GPU hangs off: with 8 ranks
-    pushing 270 MB per step each through host memory, remote-node traffic halves the e2e rate (round-1 SCALE: 0.57)."""
+    pushing 270 MB per step each through host memory, remote-node traffic can halve the e2e rate."""
     try:
         import torch
         pr = torch.cuda.get_device_properties(local)
@@ -339,6 +345,8 @@ def run_gpu_arm(args):
     t_end = time.time()
     launches = ops.LAUNCHES
     clocks = sampler.stop(t_start, t_end)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"quantized": q, "indices": ind, "loss": loss})
     ms_dev = max_over_ranks(e0.elapsed_time(e1) / args.steps)
     host_ms = (t_host - t_start) * 1e3 / args.steps   # CPU time to enqueue one step (must stay below ms_dev)
 
@@ -380,7 +388,7 @@ def run_gpu_arm(args):
     # looped for >= 2 s shows what the part sustains (clocks / power recorded), once replaying the step's graph (ms per step)
     # and once with the event pair around the search kernel (its duration under sustained clocks).
     sustained = None
-    if not args.no_sustained and world == 1:
+    if args.sustained and not args.no_sustained and world == 1:
         s_ms, _, s_steps, s_clk = timed_loop(seconds=args.sustained_seconds)
         _, s_kms, _, s_clk2 = timed_loop(seconds=args.sustained_seconds, events=True)
         sustained = {"seconds": args.sustained_seconds, "steps": s_steps, "ms_per_step": s_ms,
@@ -430,19 +438,17 @@ def run_gpu_arm(args):
     d_stage = D // 2 if cfg5 else D
     flops = 2.0 * n_vec * K * d_stage  # algorithmic, per search launch: one pass of the N x K x D contraction (SURVEY 8d)
     # The kernel was timed alone between two events inside a step of a few-millisecond region at boost clocks: the
-    # BURST peak is the honest denominator (B200_PROFILING.md); the sustained block carries its own fraction.
+    # BURST peak is the honest denominator; the sustained block carries its own fraction.
     peak_tf = peaks["bf16_tflops"]
     ach = flops / (assign_ms * 1e-3) / 1e12 if assign_ms else None
-    roof = {"bound": "tensor", "kernel": "vq_assign_kernel (tcgen05 distance MMA + fused arg-max)",
+    roof = {"bound": "tensor", "kernel": "vq_assign_kernel (wgmma distance MMA + fused arg-max)",
             "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf if ach else None,
             "peak_source": peak_src + " bf16_tflops (burst: kernel event-timed inside a short region at boost clocks)",
             "kernel_ms": assign_ms, "kernel_share_of_step": assign_ms * stages / ms_dev_events if assign_ms else None,
             "measured": "CUDA event pair on the launching stream around every vq_assign_kernel launch, over the same K "
                         "steps repeated right after the headline region (events split the step's CUDA graph)",
             "ms_per_step_with_events": ms_dev_events,
-            "algorithmic_flops_per_launch": flops, "executed_mma_passes": 3 if cfg5 else 2, "traffic": ncu_dram_bytes(),
-            "traffic_unit": "bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum of the launch AS BENCHED, fused tail on; "
-                            "profiles/r2_assign_benched_summary.txt)"}
+            "algorithmic_flops_per_launch": flops, "executed_mma_passes": 3 if cfg5 else 2}
     if sustained and sustained["kernel_ms"]:
         pk = peaks.get("bf16_tflops_sustained", peak_tf)
         sustained["kernel_tflops"] = flops / (sustained["kernel_ms"] * 1e-3) / 1e12
@@ -457,7 +463,7 @@ def run_gpu_arm(args):
         "vs_baseline": None, "dtype": "f32" if cfg5 else "bf16", "data": "synthetic",
         "config": {"workload": workload, "per_gpu_vectors": n_vec, "global_vectors": world * n_vec,
                    "parallelism": f"dp{world}: batch sharded, packed EMA statistics summed over the ranks once per step" if world > 1 else "single GPU",
-                   "l2": "input (134 MB) + output (134 MB) per step exceed the 126 MB L2; no extra flush",
+                   "l2": "input (134 MB) + output (134 MB) per step exceed the 50 MB L2; no extra flush",
                    "index_mismatch_policy": "bit-exact vs the reference fixtures outside fp32 near-ties (tests/test_big_golden.py)"},
         "e2e": e2e,
         "gpu_launches": launches,
@@ -482,7 +488,11 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="cfg2", choices=["cfg2", "cfg5"],
                     help="cfg2 = BASELINE.json configs[1] (the headline, default); cfg5 = configs[4], GroupedResidualVQ, strong scaling")
-    ap.add_argument("--no-sustained", action="store_true", help="skip the >= 2 s sustained-clock block")
+    ap.add_argument("--sustained", action="store_true",
+                    help="add a block that loops the step for --sustained-seconds (a time, not --steps) to show sustained clocks")
+    ap.add_argument("--no-sustained", action="store_true", help="skip the sustained-clock block (the default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last timed step as DIR/<name>.npy")
     ap.add_argument("--sustained-seconds", type=float, default=2.0)
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)

@@ -1,4 +1,4 @@
-/* vqb200 — C ABI of the B200 (sm_100a) vector-quantization hot path.
+/* vqb200 — C ABI of the H100 (sm_90a) vector-quantization hot path.
  *
  * The reference (lucidrains/vector-quantize-pytorch v1.31.0) is pure Python and has NO FFI for this
  * path; its boundary is `Codebook.forward` (vector_quantize_pytorch/vector_quantize_pytorch.py:674-791)
@@ -36,7 +36,7 @@ extern "C" {
 #define VQB_E_INVALID -1     /* null pointer / non-positive size / bad enum */
 #define VQB_E_UNSUPPORTED -2 /* shape outside what the kernels support (see vqb_assign) */
 #define VQB_E_ALIGN -3       /* pointer not 16-byte aligned */
-#define VQB_E_NO_DEVICE -4   /* no CUDA device, or device is not sm_100 */
+#define VQB_E_NO_DEVICE -4   /* no CUDA device, or device is not sm_90 */
 #define VQB_E_DRIVER -5      /* cuTensorMapEncodeTiled unavailable / failed */
 #define VQB_E_WORKSPACE -6   /* workspace too small */
 
@@ -87,7 +87,7 @@ int vqb_padded_codes(int K);
  *   cmax    f32  [4]          : [0] max_k ||c||, [1] max_k ||c - fp16 plane||, [2] max_k ||c - hi - lo||, [3] max_k ||lo||: the
  *                               exact residual norms that size the certification band of each pass scheme
  * Replaces nothing in the reference (it searches the fp32 rows directly, :710-712, :743); this is
- * the layout change that lets the search run on tcgen05.  Also done by vqb_ema_apply. */
+ * the layout change that lets the search run on the tensor cores.  Also done by vqb_ema_apply. */
 int vqb_codebook_prepare(const float* embed, int K, int D, int metric, void* planes, void* bext, float* bias,
                          float* cnorm2, float* cmax, void* stream);
 
@@ -100,16 +100,15 @@ int vqb_input_prepare(const void* x, int dtype, int64_t N, int D, int metric, vo
                       int n_planes, void* stream);
 
 /* Nearest-code search: replaces cdist/einsum + argmax (:58-62, :741-747, :130-145) without ever
- * materialising the (N x K) distance matrix.  tcgen05 MMA over TMA-staged tiles, fp32 accumulate in
- * TMEM, fused running arg-max.  Scores are x.c - 0.5||c||^2 (euclid) or x.c (cosine).
+ * materialising the (N x K) distance matrix.  wgmma over TMA-staged tiles, fp32 accumulate in
+ * registers, fused running arg-max.  Scores are x.c - 0.5||c||^2 (euclid) or x.c (cosine).
  *   a_planes  n_a = 1: bf16 rows [N][D] (the input itself, read in place); n_a = 2: bf16 hi/lo planes [2][N][D] of an fp32
  *             input (vqb_input_prepare).
  *   n_passes  n_a + 1 : the "split" scheme, bf16 hi / lo codebook planes into ONE fp32 accumulator:
  *                       (x,c_hi)+(x,c_lo) for bf16 rows, +(x_lo,c_hi) for fp32 rows;
  *             0       : automatic (= n_a + 1);
- *             1       : diagnostics only (n_a == 1): hi plane alone, band widened by max||c_lo|| (DESIGN.md 8, x4).
- *             Anything else returns VQB_E_UNSUPPORTED.  (A single pass on the fp16 plane was built, measured slower per
- *             step and removed: tcgen05 kind::f16 rejects bf16 x fp16 operands in one instruction.)
+ *             1       : diagnostics only (n_a == 1): hi plane alone, band widened by max||c_lo||.
+ *             Anything else returns VQB_E_UNSUPPORTED.
  *   b_planes/bext/cmax           from vqb_codebook_prepare / vqb_ema_apply
  *   margin_rel                   m, the tensor-core accumulation share of the certification band
  *                                W = 2(||x|| cres + ||x_lo|| caux + m ||x|| cmax + 2^-21 cmax^2) + tag slack + sqrt-collapse
@@ -119,7 +118,7 @@ int vqb_input_prepare(const void* x, int dtype, int64_t N, int D, int metric, vo
  *   flagged   [N] entries, flag_count i32[2] (caller zeroes both): [0] rows with 2 / 3 candidates, appended from the
  *             front; [1] rows with more (whole-row exact re-scan), appended from the back (flagged[N-1], [N-2], ...)  -> vqb_fix_flagged
  *   dbg_best  f32 [N] or NULL    best score per row (tests)
- * Supported: D % 8 == 0, 8 <= D <= 1024, 1 <= K, N >= 1, sm_100 device.  When n_a * ceil(D/64) > 8 (fp32 split input with
+ * Supported: D % 8 == 0, 8 <= D <= 1024, 1 <= K, N >= 1, sm_90 device.  When n_a * ceil(D/64) > 8 (fp32 split input with
  * D > 256) the A tile does not stay resident in shared memory: its k-blocks are streamed with the codebook's. */
 int vqb_assign(const void* a_planes, int n_a, int64_t N, int D, const void* b_planes, const void* bext,
                const float* cmax, int K, float margin_rel, int n_passes, int32_t* idx, vqb_flag_entry* flagged,
@@ -136,7 +135,7 @@ int vqb_assign_ex(const void* a_planes, int n_a, int64_t N, int D, const void* b
 /* Diagnostics: i64 [grid][16] per-role cycle counters written by subsequent vqb_assign calls (NULL disables). */
 int vqb_debug_set_profile_buffer(void* device_buffer);
 int vqb_debug_active(void);
-int vqb_debug_set_mode(int mode); /* bit0: skip the epilogue's TMEM sweep (timing experiments only; results invalid) */
+int vqb_debug_set_mode(int mode); /* nonzero: diagnostics mode (the forward chains are enqueued one by one, never graph-captured) */
 /* How vqb_vq_forward's CUDA-graph cache served the calls so far: out4 = {replayed, patched (cudaGraphExecUpdate),
  * instantiated, enqueued launch by launch after a capture / instantiate failure} (host array of 4 int64). */
 int vqb_debug_graph_stats(long long* out4);

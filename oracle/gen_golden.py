@@ -1,6 +1,6 @@
 """Generate tests/golden/*.npz by running the UNMODIFIED reference  (TEST INFRASTRUCTURE ONLY).
 
-Run in the build container (needs /root/reference):   python oracle/gen_golden.py
+Needs the reference (oracle/ref_loader.py):   python oracle/gen_golden.py [--state-dicts]
 
 Each fixture stores, for a seeded case, everything needed to replay it without the reference:
   x                      input values as float32 (bf16 cases: bf16-representable values)
@@ -408,5 +408,34 @@ def main():
                                                shared_codebook=True))
 
 
+# The constructions of tests/test_abi.py::test_reference_state_dict_loads: state_dict keys (in order) and the initial
+# buffers under torch.manual_seed(0), so that the test compares against the reference without importing it.
+STATE_DICT_BUILDS = [
+    lambda mod: mod.VectorQuantize(dim=64, codebook_size=32, use_cosine_sim=True),
+    lambda mod: mod.ResidualVQ(dim=32, num_quantizers=3, codebook_size=16),
+    lambda mod: mod.VectorQuantize(dim=64, codebook_size=32, heads=4, codebook_dim=16),
+    lambda mod: mod.VectorQuantize(dim=48, codebook_size=32, heads=2, separate_codebook_per_head=True),
+    lambda mod: mod.SimVQ(dim=32, codebook_size=40),
+    lambda mod: mod.GroupedResidualVQ(dim=64, groups=2, num_quantizers=2, codebook_size=16, shared_codebook=True),
+]
+
+
+def state_dict_cases():
+    ref = load_reference()
+    store, keys = {}, []
+    for i, build in enumerate(STATE_DICT_BUILDS):
+        torch.manual_seed(0)
+        sd = build(ref).state_dict()
+        keys.append(list(sd))
+        for j, v in enumerate(sd.values()):
+            store[f"m{i}_{j}"] = v.numpy()
+    store["keys"] = np.frombuffer(json.dumps(keys).encode(), np.uint8)
+    os.makedirs(os.path.join(OUT, "state_dict"), exist_ok=True)
+    np.savez_compressed(os.path.join(OUT, "state_dict", "reference_init.npz"), **store)
+
+
 if __name__ == "__main__":
-    main()
+    if "--state-dicts" in sys.argv:
+        state_dict_cases()
+    else:
+        main()

@@ -90,23 +90,20 @@ def test_state_dict_layout_matches_reference():
 
 
 def test_reference_state_dict_loads(tmp_path):
-    """If the reference is importable here, its state_dict must load into ours key-for-key."""
-    from oracle.ref_loader import reference_available, load_reference
-    if not reference_available():
-        pytest.skip("reference tree not present on this machine")
-    ref = load_reference()
+    """The reference's state_dict (keys and initial buffers under seed 0, tests/golden/state_dict/reference_init.npz, written by
+    `oracle/gen_golden.py --state-dicts`) must equal ours key-for-key and load into ours."""
+    import json
+    import numpy as np
+    from oracle.gen_golden import STATE_DICT_BUILDS
     import vector_quantize_pytorch_b200 as m
-    for build in (lambda mod: mod.VectorQuantize(dim=64, codebook_size=32, use_cosine_sim=True),
-                  lambda mod: mod.ResidualVQ(dim=32, num_quantizers=3, codebook_size=16),
-                  lambda mod: mod.VectorQuantize(dim=64, codebook_size=32, heads=4, codebook_dim=16),
-                  lambda mod: mod.VectorQuantize(dim=48, codebook_size=32, heads=2, separate_codebook_per_head=True),
-                  lambda mod: mod.SimVQ(dim=32, codebook_size=40),
-                  lambda mod: mod.GroupedResidualVQ(dim=64, groups=2, num_quantizers=2, codebook_size=16, shared_codebook=True)):
-        torch.manual_seed(0)
-        a = build(ref)
+    z = np.load(os.path.join(ROOT, "tests", "golden", "state_dict", "reference_init.npz"))
+    keys = json.loads(z["keys"].tobytes().decode())
+    assert len(keys) == len(STATE_DICT_BUILDS)
+    for i, build in enumerate(STATE_DICT_BUILDS):
+        sa = {k: torch.from_numpy(z[f"m{i}_{j}"]) for j, k in enumerate(keys[i])}
         torch.manual_seed(0)
         b = build(m)
-        sa, sb = a.state_dict(), b.state_dict()
+        sb = b.state_dict()
         assert list(sa) == list(sb)
         for k in sa:  # same RNG consumption at construction -> identical initial codebooks
             assert torch.equal(sa[k], sb[k]), k

@@ -1,9 +1,10 @@
 """CPU model of the search kernel's epilogue arithmetic (csrc/epilogue.cuh: ScanReg, RowState::insert, merge_slices).
 
-Per row slice the CUDA epilogue keeps the exact running maximum t1 and a skip threshold thr = max(own, partner) - W.  A
-16-column group whose maximum beats thr is a potential candidate: if it beats t1 by more than W it REPLACES the live group
-(and empties the queue), otherwise it is queued next to it (a near tie; at most CAP groups, overflow -> exact re-scan).  At
-the end of the row sweep the exact tagged top-3 (4 low mantissa bits = 15 - column inside the group; compare-exchange minima
+Each row is split over the four threads of a quad; per row slice the CUDA epilogue keeps the exact running maximum t1 and
+a skip threshold thr = (maximum over the row's four slices) - W.  A 16-score group (the values one thread holds for the
+row across eight 8-column wgmma blocks: columns base + 8 (e / 2) + (e % 2)) whose maximum beats thr is a potential
+candidate: if it beats t1 by more than W it REPLACES the live group (and empties the queue), otherwise it is queued next to it (a near tie; at most CAP groups, overflow -> exact re-scan).  At
+the end of the row sweep the exact tagged top-3 (4 low mantissa bits = 15 - position inside the group; compare-exchange minima
 recovered with min = a + b - max) is rebuilt from the live groups only, and the column slices are merged into up to three
 candidates.  This file restates that arithmetic bit for bit in numpy and checks the CERTIFICATE the parity argument rests
 on (DESIGN.md 4.1) against brute force on adversarial score matrices:
@@ -13,7 +14,7 @@ on (DESIGN.md 4.1) against brute force on adversarial score matrices:
   * reported indices are valid and distinct; the exact winning score (`best`, feeds the loss) is the true maximum.
 
 It is a model of the algorithm (test infrastructure), not of the GPU: the CUDA code itself is checked on the device by
-tests/test_parity_gpu.py and scripts/epi_bench.cu.
+tests/test_parity_gpu.py.
 """
 import numpy as np
 import pytest
@@ -73,8 +74,16 @@ class RowState:
             setattr(self, name, np.where(act, new, getattr(self, name)))
 
 
+def group_col(e):
+    """Column offset of element e of a group (epilogue.cuh: group_col)."""
+    return ((e >> 1) << 3) | (e & 1)
+
+
+GROUP_COLS = group_col(np.arange(16))
+
+
 def col(t, j):
-    return j + 15 - (f2u(t) & np.uint32(15)).astype(np.int64)
+    return j + group_col(15 - (f2u(t) & np.uint32(15)).astype(np.int64))
 
 
 class Scan:
@@ -130,9 +139,9 @@ class Scan:
         return st
 
 
-def merge(a, b):
-    """(i0, i1, i2, n, best) per row (epilogue.cuh: merge_slices, Top3::offer)."""
-    R = a.t1.shape[0]
+def merge(slices):
+    """(i0, i1, i2, n, best) per row (epilogue.cuh: merge_slices, Top3::offer); slices[0] is the merging thread's."""
+    R = slices[0].t1.shape[0]
     v = np.full((R, 3), NEG, np.float32)
     ix = np.zeros((R, 3), np.int64)
 
@@ -146,29 +155,36 @@ def merge(a, b):
             elif x > v[r, 2] or (x == v[r, 2] and i < ix[r, 2]):
                 v[r, 2], ix[r, 2] = x, i
 
-    for s in (a, b):
+    for s in slices:
         offer(s.t1, col(s.t1, s.j1)); offer(s.t2, col(s.t2, s.j2)); offer(s.t3, col(s.t3, s.j3))
-    best = np.maximum(a.bexact, b.bexact)
-    tb = np.maximum(a.t1, b.t1)
-    band = (tb - a.W).astype(np.float32)
-    n = sum((t > band).astype(np.int64) for t in (a.t1, a.t2, a.t3, a.t4, b.t1, b.t2, b.t3, b.t4))
+    best = np.maximum.reduce([s.bexact for s in slices])
+    tb = np.maximum.reduce([s.t1 for s in slices])
+    band = (tb - slices[0].W).astype(np.float32)
+    n = sum((t > band).astype(np.int64) for s in slices for t in (s.t1, s.t2, s.t3, s.t4))
     return ix[:, 0], ix[:, 1], ix[:, 2], n, best
 
 
-def epilogue(V, W, BN=256, share=True):
-    """(i0, i1, i2, n, best) per row, as the kernel produces them.  V: (R, Kpad) float32, Kpad % BN == 0."""
+WN = 128   # codes per MMA step of the search kernel
+
+
+def epilogue(V, W, share=True):
+    """(i0, i1, i2, n, best) per row, as the kernel produces them.  V: (R, Kpad) float32; columns past Kpad score -3e38
+    (the kernel seeds them so), up to a whole number of 128-code steps."""
     R, Kpad = V.shape
-    halves = [Scan(W), Scan(W)]
-    for ct in range(Kpad // BN):
-        if share and ct > 0:                               # partner's running maximum, one code tile stale
-            a1, b1 = halves[0].t1.copy(), halves[1].t1.copy()
-            halves[0].raise_(b1)
-            halves[1].raise_(a1)
-        for p in range(BN // 16):
-            h = (p % 4) // 2                               # pieces 4q + 2*half + {0, 1} belong to column half `half`
-            c0 = ct * BN + p * 16
-            halves[h].scan16(V[:, c0:c0 + 16], c0)
-    return merge(halves[0].finish(), halves[1].finish())
+    steps = -(-Kpad // WN)
+    Vp = np.full((R, steps * WN), np.float32(-3e38), np.float32)
+    Vp[:, :Kpad] = V
+    quad = [Scan(W) for _ in range(4)]                     # slice q: columns 2q, 2q + 1 of every 8-column block
+    for ct in range(steps):
+        if share and ct > 0:                               # the row's running maximum over the quad (two shuffles)
+            m = np.maximum.reduce([s.t1 for s in quad])
+            for s in quad:
+                s.raise_(m)
+        for q in range(4):
+            for g in range(2):                             # group g: 8-column blocks 8g .. 8g + 7 of the step
+                c0 = ct * WN + 64 * g + 2 * q
+                quad[q].scan16(Vp[:, c0 + GROUP_COLS], c0)
+    return merge([s.finish() for s in quad])
 
 
 def make_scores(kind, R, K, rng):
@@ -208,7 +224,7 @@ def test_epilogue_certificate(kind, K, BN, w_rel):
     vmax_abs = np.abs(V).max(axis=1)
     slack = (np.float32(2.0 ** -18) * vmax_abs).astype(np.float32)        # 2 * (16 ulp <= 2^-19 |score|)
     W = (np.float32(w_rel) * vmax_abs + slack + np.float32(1e-30)).astype(np.float32)
-    i0, i1, i2, n, best = epilogue(Vp, W, BN)
+    i0, i1, i2, n, best = epilogue(Vp, W)
 
     exact_best = V.max(axis=1)
     assert np.array_equal(best, exact_best), "bexact must be the exact row maximum"
@@ -242,5 +258,5 @@ def test_epilogue_certificate(kind, K, BN, w_rel):
 def test_constant_rows_go_to_the_whole_row_rescan():
     V = np.full((8, 256), np.float32(1.5), np.float32)
     W = np.full(8, np.float32(1e-6), np.float32)
-    _, _, _, n, best = epilogue(V, W, 256)
+    _, _, _, n, best = epilogue(V, W)
     assert (n > 3).all() and (best == np.float32(1.5)).all()

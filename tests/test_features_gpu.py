@@ -1,4 +1,4 @@
-"""GPU tests of the EMA options and adjacent paths of SURVEY §8 (a8, a10, f1) — `pytest -m gpu` on the B200 box.
+"""GPU tests of the EMA options and adjacent paths of SURVEY §8 (a8, a10, f1) — `pytest -m gpu` on an H100.
 
   * `ema_update_weight` (tensor / callable) and `accum_ema_update`: the reference's own tests
     (tests/test_readme.py:434-465, :467-492 of the reference) restated, plus the post-state against the oracle;

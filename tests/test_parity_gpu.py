@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: `pytest -m gpu`).
+"""GPU parity tests (run on an H100: `pytest -m gpu`).
 
 The CUDA path (through the C ABI) is compared with
   * the committed golden fixtures generated from the real reference (tests/golden/*.npz),

@@ -1,8 +1,8 @@
-"""B200-native (sm_100a) nearest-code search / gather / EMA kernels behind the vector-quantize-pytorch API.
+"""H100-native (sm_90a) nearest-code search / gather / EMA kernels behind the vector-quantize-pytorch API.
 
 Drop-in for ONE path of lucidrains/vector-quantize-pytorch: `VectorQuantize`, `ResidualVQ`,
 `GroupedResidualVQ` forward (`(quantized, indices, commit_loss)`), the `Codebook` surface, and `SimVQ`'s search.
-The hot path is hand-written CUDA (tcgen05 / TMA / TMEM) in `csrc/`, bound through the C ABI in
+The hot path is hand-written CUDA (wgmma / TMA / mbarrier) in `csrc/`, bound through the C ABI in
 `include/vqb200.h`.  No Triton, no CPU fallback.
 """
 from .codebook import Codebook, EuclideanCodebook, CosineSimCodebook  # noqa: E402

@@ -1,4 +1,4 @@
-"""Builds libvqb200.so IN-TREE with nvcc for sm_100a (no torch headers: the library has a pure C ABI).
+"""Builds libvqb200.so IN-TREE with nvcc for sm_90a (H100) (no torch headers: the library has a pure C ABI).
 
     python -m vector_quantize_pytorch_b200.build          # build if stale
     python -m vector_quantize_pytorch_b200.build --force
@@ -15,7 +15,7 @@ SOURCES = ["vq_assign.cu", "vq_aux.cu", "vq_ema.cu", "vq_forward.cu", "vq_peer.c
 HEADERS = ["ptx.cuh", "vqb_common.cuh", "code_operands.cuh", "gather_row.cuh", "epilogue.cuh", os.path.join("..", "..", "include", "vqb200.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
     "-cudart", "static",
@@ -57,7 +57,7 @@ def _build_locked(verbose):
     nvcc = find_nvcc()
     if nvcc is None:
         raise RuntimeError("vqb200: nvcc not found and libvqb200.so is missing/stale; cannot build the CUDA library")
-    extra = ["-DVQB_PROFILE"] if os.environ.get("VQB_PROFILE") else []  # per-role cycle counters (scripts/gpu_roles.py)
+    extra = ["-DVQB_PROFILE"] if os.environ.get("VQB_PROFILE") else []  # per-role cycle counters (vqb_debug_set_profile_buffer)
     extra += os.environ.get("VQB_NVCC_EXTRA", "").split()  # A/B experiments, e.g. -DVQB_EPI_SIMPLE
     tmp = LIB + ".tmp%d" % os.getpid()
     cmd = [nvcc] + NVCC_FLAGS + extra + ["-o", tmp] + [os.path.join(CSRC, s) for s in SOURCES]

@@ -2,7 +2,7 @@
 
 Same constructor arguments, same persistent buffers (`initted`, `cluster_size`, `embed_avg`, `embed`
 with a leading num_codebooks=1 dim, vqp:415-423) so reference checkpoints load unchanged.  The
-arithmetic of `forward` runs in the sm_100a kernels (`ops.py`); anything that is not on the hot
+arithmetic of `forward` runs in the sm_90a kernels (`ops.py`); anything that is not on the hot
 path (SURVEY.md §8) raises NotImplementedError instead of silently taking a slow path.
 """
 from __future__ import annotations
@@ -136,7 +136,7 @@ class Codebook(nn.Module):
         anything other than our own EMA kernel (load_state_dict, `.codebook = ...`, `.to(device)`)."""
         embed = self.embed
         if not embed.is_cuda:
-            raise RuntimeError("vqb200 has no CPU path: move the module to a CUDA (B200) device")
+            raise RuntimeError("vqb200 has no CPU path: move the module to a CUDA (H100) device")
         if embed.dtype != torch.float32 or not embed.is_contiguous():
             raise RuntimeError("vqb200: the `embed` buffer must be contiguous float32")
         key = (embed.data_ptr(), embed._version, embed.device)
@@ -173,7 +173,7 @@ class Codebook(nn.Module):
 
     def sync_stats(self, stats: torch.Tensor) -> torch.Tensor:
         """The reference all-reduces cluster_size and embed_sum separately (vqp:603, :607); the packed
-        buffer needs ONE all-reduce (NCCL over NVLink on B200)."""
+        buffer needs ONE all-reduce (NCCL over NVLink)."""
         if self.use_ddp:
             allreduce_packed(stats)
         return stats

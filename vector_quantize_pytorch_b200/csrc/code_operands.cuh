@@ -14,8 +14,7 @@ namespace vqb {
 //   [1] bf16 lo = bf16(c - hi)   B operand of the (x, c_lo) pass of the bf16 schemes (hi + lo carries 16 mantissa bits)
 //   [2] fp16(c)                  B operand of the MIXED scheme (bf16 rows x fp16 codes, products exact in fp32): 11 instead of 8
 //                                mantissa bits at the same tensor-core rate, i.e. a residual of 2^-12 ||c|| that certifies ~97 %
-//                                of the rows at K ~ 1e3 with ONE pass per A plane.  The tensor core honours fp16 subnormals
-//                                (scripts/gpu_flush_probe.py: exact down to 2^-24); values beyond +-65504 are clamped.
+//                                of the rows at K ~ 1e3 with ONE pass per A plane; values beyond +-65504 are clamped.
 //                                cmax[1] = max_k ||c - fp16 plane|| is the exact norm of everything the plane leaves out
 //                                (clamp included) and sizes the certification band of that scheme (vq_assign.cu).
 // cmax[2] = max_k ||c - hi - lo|| and cmax[3] = max_k ||lo|| do the same for the bf16 split schemes: the band is a

@@ -1,31 +1,26 @@
-// Row-wise arg-max with a certificate, as run by the epilogue warps of the search kernel (vq_assign.cu) on the
-// fp32 score tiles they read back from TMEM (one thread = one row slice).  Replaces the reference's
+// Row-wise arg-max with a certificate, as run by the consumer warpgroups of the search kernel (vq_assign.cu) on the
+// fp32 score tiles the tensor cores leave in their registers (one thread = one row slice).  Replaces the reference's
 // `dist.argmax(dim=-1)` over the materialised (N x K) matrix (vector_quantize_pytorch.py:130-145).
 //
 // Two layers:
-//   ScanState  the HOT loop.  Per group of G columns: a 3-input max tree (FMNMX3) and one compare against the row's
+//   ScanState  the HOT loop.  Per group of G columns: a max tree and one compare against the row's
 //              running threshold thr = (best so far) - W.  Only a group whose maximum beats thr can hold a candidate; it
 //              is copied, raw, to a tiny per-thread queue of LIVE groups.  A group that beats the running maximum by
 //              more than W kills every older group (queue reset), so the queue almost always holds ONE group.
-//   RowState   the exact tagged top-3 (scores carry their column in 4 low mantissa bits).  In round 1 it was applied
-//              to every element (7.5 instructions per element, alu-pipe bound: 4550 clk per 128x256 tile); now it is
-//              rebuilt once per row sweep from the live groups only.
-// Measured (scripts/epi_bench.cu, B200): see DESIGN.md section 8.
+//   RowState   the exact tagged top-3 (scores carry their column in 4 low mantissa bits), rebuilt once per row sweep
+//              from the live groups only.
+//
+// A group is the 16 accumulator values one thread holds for one row across eight consecutive 8-column blocks of a
+// wgmma tile: element e sits at column  base + group_col(e) = base + 8 (e / 2) + (e % 2).  Columns grow with e, so the
+// tag order (first column wins among equal truncated values) is the column order.
 #pragma once
 #include <stdint.h>
 
 namespace vqb {
 
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-__device__ __forceinline__ float fmin3(float a, float b, float c) {
-  float d;
-  asm("min.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+__host__ __device__ __forceinline__ int group_col(int e) { return ((e >> 1) << 3) | (e & 1); }
+
+__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 template <int G>
 __device__ __forceinline__ float max_group(const uint32_t* r) {
   static_assert(G == 4 || G == 8 || G == 16, "group size");
@@ -95,7 +90,7 @@ struct RowState {
   __device__ __forceinline__ void piece(const uint32_t (&r)[16], int cbase, uint32_t tagmask, uint32_t mul1, uint32_t mulm1) {
     insert<16>(r, cbase, tagmask, mul1, mulm1);
   }
-  static __device__ __forceinline__ int col(float t, int j) { return j + 15 - static_cast<int>(__float_as_uint(t) & 15u); }
+  static __device__ __forceinline__ int col(float t, int j) { return j + group_col(15 - static_cast<int>(__float_as_uint(t) & 15u)); }
 };
 
 struct MergeSlot { float t1, t2, t3, t4, bexact; int i0, i1, i2; };

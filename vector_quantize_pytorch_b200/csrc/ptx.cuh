@@ -1,11 +1,10 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / fences).
+// Thin inline-PTX wrappers for the sm_90a features the search kernel uses:
+// mbarrier, TMA (cp.async.bulk.tensor) and warpgroup MMA (wgmma.mma_async).
 // Raw PTX on purpose: no CUTLASS/CuTe dependency, the .so has a plain C ABI.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 namespace vqb {
 
@@ -19,9 +18,6 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
@@ -43,8 +39,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   return ok != 0;
 }
 
-// Bounded wait: a protocol bug must surface as a CUDA error, never as a hung GPU box.
-// ~4 s at 2 GHz is far beyond any legitimate wait in these kernels.
+// Bounded wait: a protocol bug must surface as a CUDA error (illegal instruction), never as a hung GPU.
+// ~4 s at 2 GHz is far beyond any legitimate wait in these kernels.  No printf here: a function call anywhere in a
+// kernel that uses wgmma makes ptxas serialise all of its wgmmas.
 #ifndef VQB_WAIT_TIMEOUT_CYCLES
 #define VQB_WAIT_TIMEOUT_CYCLES (8000000000ll)
 #endif
@@ -52,50 +49,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > VQB_WAIT_TIMEOUT_CYCLES) {
-      printf("vqb200: mbarrier wait timeout (block %d thread %d bar 0x%x parity %u)\n", blockIdx.x, threadIdx.x, bar,
-             parity);
-      __trap();
-    }
+    if (clock64() - t0 > VQB_WAIT_TIMEOUT_CYCLES) __trap();
   }
-}
-
-// Wait with cluster-scope acquire: pairs with a peer CTA's mbar_arrive_cluster (release.cluster).
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  const long long t0 = clock64();
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (clock64() - t0 > VQB_WAIT_TIMEOUT_CYCLES) {
-      printf("vqb200: mbarrier wait timeout (block %d thread %d bar 0x%x parity %u)\n", blockIdx.x, threadIdx.x, bar,
-             parity);
-      __trap();
-    }
-  }
-}
-
-// One lane of a CONVERGED warp (the others get false).  Issuing tcgen05 / TMA instructions under this predicate from
-// warp-uniform control flow lets ptxas keep their operands in uniform registers; under an `if (lane == 0)` region it
-// wraps every such instruction in an ELECT / BRA.U.ANY loop instead (measured: ~60 SM clocks more per MMA issue).
-__device__ __forceinline__ bool elect_one_sync() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred P;\n"
-      "elect.sync _|P, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, P;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ---------------------------------------------------------------- TMA
@@ -110,167 +65,53 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 x bf16 -> fp32, issued by ONE thread for the CTA.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed.
-// (Implies tcgen05.fence::before_thread_sync.)
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive 32-bit columns (thread t <- lane base+t).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- CTA-pair (cta_group::2) variants
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address -> the same offset in CTA `rank` of the cluster (shared::cluster address)
-__device__ __forceinline__ uint32_t mapa_cluster(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// Relaxed form: no memory ordering (and therefore no fence in front of it — the release form costs ~1 us).  Enough
-// when the only thing handed over is "my tcgen05.ld's have completed" (tcgen05.wait::ld precedes it).
-__device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load issued by either CTA of a pair; the byte count is credited to the barrier at the same offset in
-// the LEADER CTA (rank 0) — pass a barrier address with the peer bit cleared (see kPeerBitMask).
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_3d_2sm(uint32_t dst, const CUtensorMap* m, uint32_t leader_bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 rows: 128 per CTA] * B[N codes: N/2 per CTA]^T ; issued by the leader CTA only.
-__device__ __forceinline__ void umma_bf16_ss_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Lean issue form for the hot loop: the descriptors arrive as (lo, hi) words so that advancing along K is one 32-bit
-// add on `lo` (address field, units of 16 B), and the accumulate predicate is a compile-time constant.  The issuing
-// thread is latency-bound on the uniform datapath: every instruction removed here raises the MMA issue rate.
-__device__ __forceinline__ void umma_bf16_ss_2sm_acc(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                                     uint32_t b_hi, uint32_t idesc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      ".reg .b64 da, db;\n"
-      "mov.b64 da, {%1, %2};\n"
-      "mov.b64 db, {%3, %4};\n"
-      "setp.eq.u32 p, 1, 1;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc)
-      : "memory");
-}
-// Arrive (once every prior MMA of this thread retired) on the barrier at this offset in every CTA of `mask`.
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(mask) : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor for a K-major bf16 operand tile stored as rows of 128 B with the
-// 128-byte swizzle (what a TMA box of 64 bf16 x R rows with CU_TENSOR_MAP_SWIZZLE_128B produces):
-// 8-row groups are 1024 B apart (SBO), the tile base is 1024 B aligned (base_offset 0).
-// Field layout: cute/arch/mma_sm100_desc.hpp `SmemDescriptor` (library header, format reference only).
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t saddr) {
+// ---------------------------------------------------------------- wgmma
+// Shared-memory matrix descriptor for a K-major bf16 operand tile stored as rows of 128 B with the 128-byte swizzle
+// (what a TMA box of 64 bf16 x R rows with CU_TENSOR_MAP_SWIZZLE_128B produces): 8-row groups are 1024 B apart (SBO),
+// the tile base is 1024 B aligned (base offset 0).  Stepping 16 elements (32 B) along K adds 2 to the low word.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);        // [0,14)  start address >> 4
-  d |= static_cast<uint64_t>(1) << 16;                       // [16,30) leading byte offset >> 4 (unused for SW128 K-major)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;               // [32,46) stride byte offset >> 4
-  d |= static_cast<uint64_t>(1) << 46;                       // [46,48) descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                       // [61,64) layout: SWIZZLE_128B
+  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);   // [0,14)  start address >> 4
+  d |= static_cast<uint64_t>(1) << 16;                  // [16,30) leading byte offset >> 4 (unused for SW128 K-major)
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;          // [32,46) stride byte offset >> 4
+  d |= static_cast<uint64_t>(1) << 62;                  // [62,64) layout: 1 = SWIZZLE_128B
   return d;
 }
-// Instruction descriptor, kind::f16: D=f32, A=B=bf16, both K-major, dense, no negate.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N) {
-  return (1u << 4)          // [4,6)   D format  : 1 = F32
-         | (1u << 7)        // [7,10)  A format  : 1 = BF16
-         | (1u << 10)       // [10,13) B format  : 1 = BF16
-         | ((N >> 3) << 17) // [17,23) N >> 3
-         | ((M >> 4) << 24);// [24,29) M >> 4
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// Keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs.
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Same, A = B = fp16 (format code 0).  (kind::f16 rejects bf16 x fp16 in one instruction: measured, illegal instruction.)
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t M, uint32_t N) {
-  return (1u << 4)          // D = F32
-         | (0u << 7)        // A = F16
-         | (0u << 10)       // B = F16
-         | ((N >> 3) << 17)
-         | ((M >> 4) << 24);
+// D[64 x 128] += A[64 x 16] * B[128 x 16]^T, bf16 x bf16 -> fp32, both operands K-major in shared memory, issued by the
+// whole warpgroup.  Thread t of the warpgroup holds rows 16 (t/32) + (t%32)/4 (+8) and columns 8 j + 2 (t%4) (+1):
+// d[4j + 0/1] = (row, cols), d[4j + 2/3] = (row + 8, cols).
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, 1, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc));
 }
 
 }  // namespace vqb

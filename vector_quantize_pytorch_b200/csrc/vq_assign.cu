@@ -1,30 +1,19 @@
-// Nearest-code search on the 5th-gen tensor cores (sm_100a).
+// Nearest-code search on the Hopper tensor cores (sm_90a: TMA, mbarrier, wgmma).
 //
 // Replaces the reference's   dist = -cdist(x, embed) | einsum(x, embed) ; ind = dist.argmax(-1)
 // (vector_quantize_pytorch.py:58-62, :741-747, :130-145) without materialising the (N x K) matrix.
 //
-// Persistent CTA PAIRS (cluster of 2, tcgen05 cta_group::2): the two CTAs of a pair quantize two adjacent
-// 128-row tiles against the same codebook sweep.  Each CTA stages only HALF of every codebook tile
-// (BN/2 codes) — the M=256 MMA reads both halves — which halves the L2->SM operand traffic that bounded
-// the single-CTA version (measured: 53 B/clk/SM of B-tile ingest at 2 passes).
-// Per CTA, warp-specialised (14 warps).  The warp scheduler favours the HIGHER warp id of a scheduler partition when
-// several warps are ready, and the epilogue warps are always ready (alu-pipe bound) — so the two warps whose issue
-// latency gates everything else (MMA issuer, TMA producer) get the highest ids of their partitions:
-//   warps 0..7  epilogue     : tcgen05.ld (lane == row).  Warps w and w+4 share a TMEM lane group and split
-//                              the columns; a thread keeps a branch-free running top-3 of its row slice (RowState),
-//                              the two slices are merged once per row tile.
-//   warps 8..11 store        : row norms ||x||^2 of the next tile from the A tile in smem; fused gather tail
-//                              (quantized rows, int64 indices) of the tile just certified
-//   warp 12     TMA producer : x tile (A: 128 rows, stationary in smem for the whole code sweep, refilled
-//                              k-block by k-block as the last sweep of the previous tile releases it),
-//                              codebook tiles (B: BN codes x 64 dims per stage) and the per-tile bias
-//                              block (Bext: BN codes x 16) -> swizzled smem
-//   warp 13     MMA issuer   : (leader CTA only) tcgen05.mma.cta_group::2.kind::f16, M=256 (128 rows per CTA),
-//                              bf16 x bf16 -> fp32 into the TMEM of both CTAs.
-//                              Per code tile: one K=16 MMA  [1 1 1 0..] x [-b1 -b2 -b3 0..]^T  that seeds
-//                              the accumulator with -0.5||c||^2 (three bf16 terms = exact fp32), then the
-//                              split-precision passes (a0,c_hi)+(a0,c_lo)[+(a1,c_hi)] accumulate on top.
-//                              Two accumulator stages (2 x 256 TMEM columns).
+// Persistent CTAs, one 128-row tile of x at a time, three warpgroups (384 threads):
+//   warp 0          TMA producer : x tile (A: 128 rows, stationary in smem for the whole code sweep, refilled k-block by
+//                                  k-block as the last code step of the previous tile releases it) and codebook tiles
+//                                  (B: 128 codes x 64 dims per ring stage) -> 128-byte-swizzled smem
+//   warps 1..3      store warps  : fused gather tail (quantized rows, int64 indices, residuals) of the tile just certified
+//   warpgroups 1, 2 consumers    : rows 0..63 / 64..127 of the tile.  Per step of 128 codes the accumulator registers are
+//                                  seeded with -0.5||c||^2 (the three bf16 terms of bext summed in fp32: the exact value),
+//                                  then wgmma m64n128k16 accumulates the split-precision passes (a0,c_hi)+(a0,c_lo)
+//                                  [+(a1,c_hi)] on top (bf16 x bf16 -> fp32), and the certified arg-max scan
+//                                  (epilogue.cuh) reads the scores straight from the registers.  The two consumer
+//                                  warpgroups share the tensor cores: one scans while the other's MMAs run.
 //
 // Exactness: the tensor-core score of a (row, code) pair differs from the exact fp32 value by at most
 // tau = margin_rel * ||x|| * max||c||, and the epilogue's 4-bit column tag perturbs it by < 16 ulp.  A row is
@@ -35,10 +24,8 @@
 #include "vqb_common.cuh"
 #include "gather_row.cuh"
 #include "epilogue.cuh"
-#include <type_traits>
 
-// Per-role cycle accounting (scripts/gpu_roles.py): compile with -DVQB_PROFILE.  Off by default: the counters cost
-// registers in a kernel that runs at the 128-register cap.
+// Per-role cycle accounting (vqb_debug_set_profile_buffer): compile with -DVQB_PROFILE.  Off by default.
 #ifdef VQB_PROFILE
 #define PROF_CLOCK() clock64()
 #else
@@ -47,35 +34,33 @@
 
 namespace vqb {
 
-constexpr int BM = 128;         // rows of x per tile (UMMA M, one TMEM lane per row)
+constexpr int BM = 128;         // rows of x per tile
+constexpr int WM = 64;          // rows per consumer warpgroup (wgmma M)
+constexpr int WN = 128;         // codes per MMA step (wgmma N)
 constexpr int BK = 64;          // bf16 elements per 128-byte swizzle row
-constexpr int UMMA_K = 16;      // K of one tcgen05.mma for 16-bit inputs
 constexpr int A_SUB_BYTES = BM * BK * 2;  // 16 KiB: one (plane, k-block) sub-tile of A
+constexpr int B_SUB_BYTES = WN * BK * 2;  // 16 KiB: one (plane, k-block) sub-tile of a code step
 constexpr int MAX_A_SUB = 8;    // n_a * ceil(D/64) <= 8  -> A <= 128 KiB
 constexpr int MAX_STAGES = 8;
-constexpr int TMEM_COLS = 512;
-constexpr int NUM_EPI_WARPS = 8;
-constexpr int NUM_STORE_WARPS = 4;  // fused gather / loss / residual tail of the certified rows
-constexpr int NUM_THREADS = (2 + NUM_EPI_WARPS + NUM_STORE_WARPS) * 32;
-constexpr int MMA_GROUP = 4;      // k-blocks issued per elected region of the MMA warp
-constexpr int WARP_PROD = NUM_EPI_WARPS + NUM_STORE_WARPS;      // 12
-constexpr int WARP_MMA = NUM_EPI_WARPS + NUM_STORE_WARPS + 1;   // 13
-constexpr int AEXT_BYTES = BM * 32;       // [128 rows][16 bf16], 32-byte swizzle
-constexpr int SMEM_CTRL_BYTES = 14336;    // barriers + tmem ptr + row norms + merge area + threshold exchange
-constexpr int SMEM_LIMIT = 232448;        // 227 KiB opt-in maximum per CTA
+constexpr int NUM_CONSUMER_WARPS = 8;   // two warpgroups
+constexpr int NUM_STORE_WARPS = 3;      // warps 1..3 (warp 0 is the TMA producer)
+constexpr int NUM_THREADS = 128 + NUM_CONSUMER_WARPS * 32;
+constexpr int SMEM_CTRL_BYTES = 14336;  // barriers + winner hand-off + merge area
+constexpr int SMEM_LIMIT = 232448;      // 227 KiB opt-in maximum per CTA
 
 struct AssignParams {
   int64_t N;
-  int D, K, Kpad, BN;
+  int D, K, Kpad;
   int n_a, n_passes;   // pass 0 (a0,c_hi), 1 (a0,c_lo), 2 (a1,c_hi): bf16 operands, fp32 accumulation
   int KB;              // ceil(D / 64)
-  int n_stages, n_xstages;
+  int n_stages;
   int stream_a;        // A does not fit in smem next to a useful B ring (fp32 split input with D > 256): its k-blocks travel
-                       // through the ring together with the codebook k-blocks (re-read from L2 for every code tile)
-  const uint16_t* a_global;   // [n_a][N][D] bf16: the A planes in global memory (row norms in stream_a mode)
-  int num_row_tiles, num_code_tiles;
+                       // through the ring together with the codebook k-blocks (re-read from L2 for every code step)
+  const uint16_t* a_global;   // [n_a][N][D] bf16: the A planes in global memory (row norms)
+  const uint16_t* bext;       // [Kpad][16] bf16: -0.5||c||^2 as three bf16 terms (code_operands.cuh)
+  int num_row_tiles, num_code_steps;
   float margin_rel;
-  const float* cmax;   // [1]
+  const float* cmax;   // [4]
   int32_t* idx;
   int32_t* idx_prov;   // optional: idx with -1 for flagged rows
   int32_t* hist;       // optional [slabs][K]: histogram of the certified winners per slab of (128 << hist_shift) rows — the
@@ -88,48 +73,20 @@ struct AssignParams {
   FusedOut fo;         // optional fused gather tail (fo.enabled)
   int copy_mode;       // tail = pure row copy q <- codebook row (+ loss from the scores); no x re-read
   int resid_mode;      // tail = residual only: r <- x - codebook row (+ loss from the scores): a ResidualVQ stage (rvq:524)
-  int score_loss;      // copy_mode || resid_mode: the epilogue accumulates the loss from the exact winning scores
   int metric;
   const uint16_t* b_hi;     // bf16 hi plane [Kpad][D]: bf16(c) == the quantized row for bf16 inputs
   const float* cnorm2;      // [K] (cosine loss term)
-  uint32_t tagmask, mul1, mulm1;  // 0xFFFFFFF0, 1, -1: constants the compiler must not fold (RowState::piece)
-  int dbg_mode;        // diagnostics: bit0 = epilogue skips the TMEM sweep, bit1 = skip B loads+MMAs except bias
+  uint32_t tagmask, mul1, mulm1;  // 0xFFFFFFF0, 1, -1: constants the compiler must not fold (RowState::insert)
 };
 
 struct Ctrl {  // lives at the start of dynamic smem
   uint64_t a_full[MAX_A_SUB], a_empty[MAX_A_SUB];
-  uint64_t a_read;                       // store warps finished reading A (row norms)
-  uint64_t a_ready;                      // follower CTA: its A tile has landed (forwarded by the leader's store warp 0)
-  uint64_t n_full[2];                    // row norms of a tile are in xn2[tile parity]
   uint64_t b_full[MAX_STAGES], b_empty[MAX_STAGES];
-  uint64_t x_full[2], x_empty[2];        // bias blocks
-  uint64_t t_full[2], t_empty[2];        // TMEM accumulator stages
   uint64_t g_full[2], g_empty[2];        // winners of a row tile handed to the store warps
-  uint32_t tmem_base;
-  uint32_t pad;
-  float xn2[2][BM];                      // row norms, double buffered by row-tile parity
-  MergeSlot merge[2][BM];                // slice states of the upper column-half warps, double buffered
   int gidx[2][BM];                       // certified winner per row (-1: flagged / out of range)
-  float xlo[2][BM];                      // ||x_lo|| of the row (fp32 inputs: the x-side residual terms of the band); 0 for bf16 inputs
-  float share[2][2][BM];                 // [row-tile parity][column half][row]: running maximum of each slice, read by the
-                                         // partner warp to raise its skip threshold (stale values are merely conservative)
+  MergeSlot merge[BM][3];                // slices 1..3 of each row, published for the quad's lane 0
 };
 static_assert(sizeof(Ctrl) <= SMEM_CTRL_BYTES, "control block too large");
-
-// 32-byte-swizzle K-major descriptor (the [rows][16 bf16] bias operands): 8-row groups are 256 B apart.
-__device__ __forceinline__ uint64_t umma_smem_desc_sw32(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(256 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(6) << 61;  // SWIZZLE_32B
-  return d;
-}
-
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 
 // Generic fused tail of one batch of rows (needs x again: residual / running sum / fused statistics).  Kept out of
 // line so that its register appetite does not set the allocation of the whole persistent kernel.
@@ -143,573 +100,99 @@ __device__ __forceinline__ float tail_rows(const FusedOut& fo, const int64_t (&r
 // budget): 0 = none / generic (x re-read: running sum, fused statistics, cosine residual), 1 = copy mode, 2 = resid mode.
 template <int TAIL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmX, const AssignParams p) {
+vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const AssignParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   Ctrl* ctrl = reinterpret_cast<Ctrl*>(smem);
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t a_base = (smem_base + SMEM_CTRL_BYTES + 1023u) & ~1023u;    // swizzled tiles need 1024 B alignment
-  const uint8_t* a_gen = smem + (a_base - smem_base);                         // same place, generic address
   const int n_sub = p.stream_a ? 0 : p.n_a * p.KB;                            // stationary A sub-tiles
-  const uint32_t aext_base = a_base + n_sub * A_SUB_BYTES;                    // 4 KiB
-  const uint32_t b_stage_bytes = (p.BN / 2) * BK * 2;   // this CTA's half of a codebook tile
-  const uint32_t x_stage_bytes = (p.BN / 2) * 32;
-  const uint32_t xb_base = aext_base + AEXT_BYTES;                            // n_xstages * BN*32
-  const uint32_t b_base = (xb_base + p.n_xstages * x_stage_bytes + 1023u) & ~1023u;
-  // ring stage = [A k-block (stream_a only) | this CTA's half of the codebook k-block]
+  const uint32_t b_base = a_base + n_sub * A_SUB_BYTES;
+  // ring stage = [A k-block (stream_a only) | codebook k-block of the code step]
   const uint32_t a_stage_bytes = p.stream_a ? A_SUB_BYTES : 0;
-  const uint32_t stage_stride = a_stage_bytes + b_stage_bytes;
+  const uint32_t stage_stride = a_stage_bytes + B_SUB_BYTES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int my_tiles = (p.num_row_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
 
   // ------------------------------------------------------------------ one-time setup
-  if (warp == WARP_PROD && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmX);
     for (int s = 0; s < n_sub; ++s) {
       mbar_init(smem_u32(&ctrl->a_full[s]), 1);
-      mbar_init(smem_u32(&ctrl->a_empty[s]), 1);
+      mbar_init(smem_u32(&ctrl->a_empty[s]), NUM_CONSUMER_WARPS);
     }
-    mbar_init(smem_u32(&ctrl->a_read), NUM_STORE_WARPS);
-    mbar_init(smem_u32(&ctrl->a_ready), 1);
-    mbar_init(smem_u32(&ctrl->n_full[0]), NUM_STORE_WARPS);
-    mbar_init(smem_u32(&ctrl->n_full[1]), NUM_STORE_WARPS);
     for (int s = 0; s < p.n_stages; ++s) {
       mbar_init(smem_u32(&ctrl->b_full[s]), 1);
-      mbar_init(smem_u32(&ctrl->b_empty[s]), 1);
+      mbar_init(smem_u32(&ctrl->b_empty[s]), NUM_CONSUMER_WARPS);
     }
     for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&ctrl->x_full[s]), 1);
-      mbar_init(smem_u32(&ctrl->x_empty[s]), 1);
-      mbar_init(smem_u32(&ctrl->t_full[s]), 1);
-      mbar_init(smem_u32(&ctrl->t_empty[s]), 2 * NUM_EPI_WARPS);  // the epilogue warps of BOTH CTAs (the follower's arrive remotely)
-      mbar_init(smem_u32(&ctrl->g_full[s]), NUM_EPI_WARPS / 2);
+      mbar_init(smem_u32(&ctrl->g_full[s]), NUM_CONSUMER_WARPS);
       mbar_init(smem_u32(&ctrl->g_empty[s]), NUM_STORE_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == WARP_MMA) {
-    tmem_alloc_2sm(smem_u32(&ctrl->tmem_base), TMEM_COLS);
-    tmem_relinquish_2sm();
-  }
-  if (threadIdx.x < BM) {
-    ctrl->share[0][0][threadIdx.x] = -3.4e38f; ctrl->share[0][1][threadIdx.x] = -3.4e38f;
-    // constant A-side bias operand: row r = [1 1 1 0 ... 0] (16 bf16 = two 16-byte chunks), 32-byte swizzle:
-    // chunk j of row r lives at r*32 + ((j ^ ((r >> 2) & 1)) << 4)
-    const int r = threadIdx.x;
-    uint8_t* row = const_cast<uint8_t*>(a_gen) + (aext_base - a_base) + r * 32;
-    const int sw = (r >> 2) & 1;
-    *reinterpret_cast<uint4*>(row + ((0 ^ sw) << 4)) = make_uint4(0x3F803F80u, 0x00003F80u, 0u, 0u);
-    *reinterpret_cast<uint4*>(row + ((1 ^ sw) << 4)) = make_uint4(0u, 0u, 0u, 0u);
-  }
-  fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();        // the peer's barriers are initialised before anything signals them remotely
-  tc_fence_after();
-  const uint32_t tmem_base = ctrl->tmem_base;
 
-  const uint32_t rank = cluster_ctarank();          // 0 = leader (issues the MMAs)
-  const bool leader = rank == 0;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-  const int num_pairs = (p.num_row_tiles + 1) >> 1;  // a pair of CTAs quantizes two adjacent row tiles
-  const int my_tiles = (num_pairs - cluster_id + num_clusters - 1) / num_clusters;
-  // Plane of pass ps (no tables: indexing the kernel parameters dynamically sends them to local memory, and a local load
-  // per item in the MMA issue loop cost 19 % of the kernel).  split: A plane = (ps == 2), codebook plane = (ps == 1).
-  const int last_pass_a0 = p.n_passes >= 2 ? 1 : 0;  // last pass of a k-block that reads A plane 0
-
-  if (warp == WARP_PROD) {
+  if (warp == 0) {
     // ================================================================ TMA producer
     if (lane == 0) {
-      long long prof_acc[2] = {0, 0};
+      long long w_empty = 0;
       const long long pstart = PROF_CLOCK();
       int stage = 0;
       uint32_t ph = 0;
-      uint32_t it = 0;
-      const int code_half = static_cast<int>(rank) * (p.BN / 2);
       for (int t = 0; t < my_tiles; ++t) {
-        const int tile = (cluster_id + t * num_clusters) * 2 + static_cast<int>(rank);
-        const int row0 = tile * BM;  // may lie beyond N for the odd last pair: TMA zero-fills, nothing is written back
-        if (t > 0 && !p.stream_a) mbar_wait(smem_u32(&ctrl->a_read), (t - 1) & 1);  // norms of the previous tile were read
-        for (int ct = 0; ct < p.num_code_tiles; ++ct, ++it) {
-          {  // bias block of this code tile (this CTA's half of the codes)
-            const uint32_t xs = p.n_xstages == 2 ? (it & 1) : 0;
-            const uint32_t xph = p.n_xstages == 2 ? ((it >> 1) & 1) : (it & 1);
-            mbar_wait(smem_u32(&ctrl->x_empty[xs]), xph ^ 1);
-            if (leader) mbar_arrive_expect_tx(smem_u32(&ctrl->x_full[xs]), 2 * x_stage_bytes);
-            tma_load_3d_2sm(xb_base + xs * x_stage_bytes, &tmX, smem_u32(&ctrl->x_full[xs]) & kPeerBitMask, 0,
-                            ct * p.BN + code_half, 0);
-          }
-          // k-block-major: all passes of a k-block back to back, so that in the LAST code tile of a row tile an A sub-tile
-          // is released (and refilled for the next row tile) a whole code tile ahead of its next use instead of 3 k-blocks
+        const int row0 = (static_cast<int>(blockIdx.x) + t * static_cast<int>(gridDim.x)) * BM;
+        for (int ct = 0; ct < p.num_code_steps; ++ct) {
+          // k-block-major: all passes of a k-block back to back, so that in the LAST code step of a row tile an A sub-tile
+          // is released (and refilled for the next row tile) as early as possible
           for (int kb = 0; kb < p.KB; ++kb) {
             for (int ps = 0; ps < p.n_passes; ++ps) {
               const int bplane = (ps == 1) ? 1 : 0;
               const int aplane = (ps == 2) ? 1 : 0;
-              const bool first_use = !p.stream_a && (ct == 0) && (ps == 0 || ps == 2);
-              if (first_use) {  // refill this A sub-tile as soon as the previous row tile released it
+              if (!p.stream_a && ct == 0 && (ps == 0 || ps == 2)) {  // refill this A sub-tile once the previous row tile released it
                 const int sub = aplane * p.KB + kb;
                 mbar_wait(smem_u32(&ctrl->a_empty[sub]), (t & 1) ^ 1);
-                if (leader) mbar_arrive_expect_tx(smem_u32(&ctrl->a_full[sub]), 2 * A_SUB_BYTES);
-                tma_load_3d_2sm(a_base + sub * A_SUB_BYTES, &tmA, smem_u32(&ctrl->a_full[sub]) & kPeerBitMask, kb * BK, row0,
-                                aplane);
+                mbar_arrive_expect_tx(smem_u32(&ctrl->a_full[sub]), A_SUB_BYTES);
+                tma_load_3d(a_base + sub * A_SUB_BYTES, &tmA, smem_u32(&ctrl->a_full[sub]), kb * BK, row0, aplane);
               }
-              { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_empty[stage]), ph ^ 1); prof_acc[0] += PROF_CLOCK() - c0; }
-              if (p.dbg_mode & 4) {  // timing experiment: no codebook traffic, the MMAs run on stale smem
-                if (leader) mbar_arrive(smem_u32(&ctrl->b_full[stage]));
-              } else {
-                if (leader) mbar_arrive_expect_tx(smem_u32(&ctrl->b_full[stage]), 2 * stage_stride);
-                if (p.stream_a)
-                  tma_load_3d_2sm(b_base + stage * stage_stride, &tmA, smem_u32(&ctrl->b_full[stage]) & kPeerBitMask, kb * BK, row0,
-                                  aplane);
-                tma_load_3d_2sm(b_base + stage * stage_stride + a_stage_bytes, &tmB, smem_u32(&ctrl->b_full[stage]) & kPeerBitMask,
-                                kb * BK, ct * p.BN + code_half, bplane);
-              }
+              { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_empty[stage]), ph ^ 1); w_empty += PROF_CLOCK() - c0; }
+              mbar_arrive_expect_tx(smem_u32(&ctrl->b_full[stage]), stage_stride);
+              if (p.stream_a)
+                tma_load_3d(b_base + stage * stage_stride, &tmA, smem_u32(&ctrl->b_full[stage]), kb * BK, row0, aplane);
+              tma_load_3d(b_base + stage * stage_stride + a_stage_bytes, &tmB, smem_u32(&ctrl->b_full[stage]), kb * BK,
+                          ct * WN, bplane);
               if (++stage == p.n_stages) { stage = 0; ph ^= 1; }
             }
           }
         }
       }
-      if (p.prof) { p.prof[blockIdx.x * 16 + 0] = prof_acc[0]; p.prof[blockIdx.x * 16 + 1] = PROF_CLOCK() - pstart; }
+      if (p.prof) { p.prof[blockIdx.x * 16 + 0] = w_empty; p.prof[blockIdx.x * 16 + 1] = PROF_CLOCK() - pstart; }
     }
-  } else if (warp == WARP_MMA) {
-    // ================================================================ MMA issuer
-    if (leader) {  // the whole warp runs the loop (warp-uniform); one elected lane issues
-      const uint32_t idesc = umma_idesc_bf16(2 * BM, p.BN);                 // bias MMA: bf16 x bf16
-      // the passes multiply fp16 operands (same tensor-core rate, 3 more mantissa bits per operand than bf16)
-      // timing experiment (results invalid): issue the pass MMAs with half the N extent
-      // the passes: A is always bf16; B is a bf16 plane or the fp16 plane (mixed bf16 x fp16: products exact in fp32)
-      const uint32_t n_pass = (p.dbg_mode & 8) ? p.BN / 2 : p.BN;
-      const uint32_t idesc_pass = umma_idesc_bf16(2 * BM, n_pass);
-      constexpr uint16_t kBoth = 0x3;
-      long long w_tempty = 0, w_bfull = 0, w_xfull = 0, w_afull = 0;
-      const long long mstart = PROF_CLOCK();
-      const uint64_t aext_desc = umma_smem_desc_sw32(aext_base);
-      // K-major SW128 descriptors: constant high word, the low word is (address >> 4) | LBO; stepping 32 B along K or
-      // one sub-tile / stage further is an add on the low word
-      const uint64_t d0 = umma_smem_desc_sw128(a_base);
-      const uint32_t desc_hi = static_cast<uint32_t>(d0 >> 32);
-      const uint32_t a_desc_lo0 = static_cast<uint32_t>(d0);
-      const uint32_t b_desc_lo0 = static_cast<uint32_t>(umma_smem_desc_sw128(b_base + a_stage_bytes));
-      const uint32_t as_desc_lo0 = static_cast<uint32_t>(umma_smem_desc_sw128(b_base));   // stream_a: A block of stage 0
-      const uint32_t b_stage_units = stage_stride >> 4;
-      const bool full_k = (p.D & (BK - 1)) == 0;
-      const int ksteps_last = full_k ? 4 : ((p.D & (BK - 1)) + UMMA_K - 1) / UMMA_K;
-      // a group never spans more than half of the B ring (the producer must be able to run ahead of it)
-      const int mma_group = p.n_stages >= 2 * MMA_GROUP ? MMA_GROUP : (p.n_stages >= 4 ? 2 : 1);
-      int stage = 0;
-      uint32_t ph = 0;
-      uint32_t it = 0;  // accumulator iteration counter (across row tiles)
-      for (int t = 0; t < my_tiles; ++t) {
-        for (int ct = 0; ct < p.num_code_tiles; ++ct, ++it) {
-          const uint32_t as = it & 1;
-          { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->t_empty[as]), ((it >> 1) & 1) ^ 1); w_tempty += PROF_CLOCK() - c0; }
-          const uint32_t d_tmem = tmem_base + as * 256;
-          {  // seed the accumulator with -bias
-            const uint32_t xs = p.n_xstages == 2 ? (it & 1) : 0;
-            const uint32_t xph = p.n_xstages == 2 ? ((it >> 1) & 1) : (it & 1);
-            { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->x_full[xs]), xph); w_xfull += PROF_CLOCK() - c0; }
-            tc_fence_after();
-            if (elect_one_sync()) {
-              umma_bf16_ss_2sm(d_tmem, aext_desc, umma_smem_desc_sw32(xb_base + xs * x_stage_bytes), idesc, 0u);
-              umma_commit_2sm(smem_u32(&ctrl->x_empty[xs]), kBoth);
-            }
-            __syncwarp();
-          }
-          // Items of a code tile in k-block-major order (kb, ps) — the order the producer stages them in.  Groups of up to
-          // MMA_GROUP items: wait for all their operands, then ONE elected region issues their MMAs back to back.  The
-          // issuing warp shares its scheduler with two always-ready epilogue warps; every instruction it does not
-          // execute (loop control, waits, elect, fences per item) is issue latency the tensor pipe does not see.
-          const int n_items = p.KB * p.n_passes;
-          const bool last_ct = ct == p.num_code_tiles - 1;
-          int kb_w = 0, ps_w = 0;   // (kb, ps) of the next item to wait for / issue
-          for (int i0 = 0; i0 < n_items; i0 += mma_group) {
-            const int cnt = min(mma_group, n_items - i0);
-            int st_w = stage;
-            uint32_t ph_w = ph;
-            int kb_g = kb_w, ps_g = ps_w;
-#pragma unroll
-            for (int g = 0; g < MMA_GROUP; ++g) {
-              if (g < cnt) {
-                if (ct == 0 && !p.stream_a) { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->a_full[(ps_g == 2 ? p.KB : 0) + kb_g]), t & 1); w_afull += PROF_CLOCK() - c0; }
-                { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_full[st_w]), ph_w); w_bfull += PROF_CLOCK() - c0; }
-                if (++st_w == p.n_stages) { st_w = 0; ph_w ^= 1; }
-                if (++ps_g == p.n_passes) { ps_g = 0; ++kb_g; }
-              }
-            }
-            tc_fence_after();
-            if (elect_one_sync()) {
-              int st_i = stage;
-              int kb = kb_w, ps = ps_w;
-#pragma unroll
-              for (int g = 0; g < MMA_GROUP; ++g) {
-                if (g < cnt) {
-                  const int aplane = (ps == 2) ? 1 : 0;
-                  const int sub = aplane * p.KB + kb;
-                  const bool last_use = last_ct && (aplane == 1 ? ps == 2 : ps == last_pass_a0);
-                  const uint32_t a_lo = p.stream_a ? as_desc_lo0 + static_cast<uint32_t>(st_i) * b_stage_units
-                                                   : a_desc_lo0 + static_cast<uint32_t>(sub) * (A_SUB_BYTES >> 4);
-                  const uint32_t b_lo = b_desc_lo0 + static_cast<uint32_t>(st_i) * b_stage_units;
-                  if (full_k || kb + 1 < p.KB) {  // full k-block: four K=16 steps, descriptors advance by 32 B
-                    umma_bf16_ss_2sm_acc(d_tmem, a_lo, desc_hi, b_lo, desc_hi, idesc_pass);
-                    umma_bf16_ss_2sm_acc(d_tmem, a_lo + 2, desc_hi, b_lo + 2, desc_hi, idesc_pass);
-                    umma_bf16_ss_2sm_acc(d_tmem, a_lo + 4, desc_hi, b_lo + 4, desc_hi, idesc_pass);
-                    umma_bf16_ss_2sm_acc(d_tmem, a_lo + 6, desc_hi, b_lo + 6, desc_hi, idesc_pass);
-                  } else {  // ragged last k-block (D % 64 != 0): only the K steps that hold data (the rest is TMA zero fill)
-                    for (int k = 0; k < ksteps_last; ++k)
-                      umma_bf16_ss_2sm_acc(d_tmem, a_lo + 2 * k, desc_hi, b_lo + 2 * k, desc_hi, idesc_pass);
-                  }
-                  umma_commit_2sm(smem_u32(&ctrl->b_empty[st_i]), kBoth);              // ring stage reusable once these MMAs retire
-                  if (last_use && !p.stream_a) umma_commit_2sm(smem_u32(&ctrl->a_empty[sub]), kBoth); // ... and this A sub-tile too
-                  if (++st_i == p.n_stages) st_i = 0;
-                  if (++ps == p.n_passes) { ps = 0; ++kb; }
-                }
-              }
-            }
-            __syncwarp();
-            stage = st_w;
-            ph = ph_w;
-            kb_w = kb_g;
-            ps_w = ps_g;
-          }
-          if (elect_one_sync()) umma_commit_2sm(smem_u32(&ctrl->t_full[as]), kBoth);  // accumulator complete -> both epilogues
-          __syncwarp();
-        }
-      }
-      if (p.prof && lane == 0) {
-        long long* o = p.prof + blockIdx.x * 16;
-        o[2] = w_tempty; o[3] = w_bfull; o[4] = w_xfull; o[5] = w_afull; o[6] = PROF_CLOCK() - mstart;
-      }
-    }
-  } else if (warp < NUM_EPI_WARPS) {
-    // ================================================================ epilogue (warps 0..7)
-    const int ew = warp;                     // 0..7
-    const int lg = warp & 3;                 // TMEM lane group this warp may access
-    const int half = ew >> 2;                // column half: chunk parity handled by this warp
-    const int row_in_tile = lg * 32 + lane;  // TMEM lane == row of the tile
-    const int pair_bar = 1 + lg;             // named barrier shared by the two warps of a lane group
-    const float cmax = __ldg(p.cmax);
-    // Exact norms of what the pass scheme leaves out of the codebook operand (code_operands.cuh): ||c - fp16 plane|| for the
-    // mixed passes, ||c - hi - lo|| for the bf16 split.  fp32 inputs (x = hi + lo + res, |res| <= 2^-8 |lo| per element) add
-    // x_res . c and, in the split scheme, the omitted x_lo . c_lo:  ||x_lo|| * caux.
-    // (a hi-only single pass, n_passes == 1, also leaves out the lo plane: diagnostics / pass-scheme experiments)
-    const float cres = __ldg(p.cmax + 2) + (p.n_passes == 1 ? __ldg(p.cmax + 3) : 0.f);
-    const float caux = p.n_a == 2 ? 0x1.02p-8f * cmax + __ldg(p.cmax + 3) : 0.f;
-    const uint32_t te_remote0 = mapa_cluster(smem_u32(&ctrl->t_empty[0]), 0);
-    const uint32_t te_remote1 = mapa_cluster(smem_u32(&ctrl->t_empty[1]), 0);
-    // number of 16-column pieces of a code tile owned by this warp (pieces 4q + 2*half + {0,1} below BN/16)
-    int np_warp = 0;
-    while (np_warp < 64 && (4 * (np_warp >> 1) + 2 * half + (np_warp & 1)) < (p.BN >> 4)) ++np_warp;
-    if (p.dbg_mode & 1) np_warp = 0;
-    uint32_t it = 0;
-    long long w_tfull = 0, w_work = 0, w_merge = 0, w_nfull = 0;
-    const long long estart = PROF_CLOCK();
-    float epi_loss = 0.f;
-    for (int t = 0; t < my_tiles; ++t) {
-      const int tile = (cluster_id + t * num_clusters) * 2 + static_cast<int>(rank);
-      RowState st;                 // exact tagged top-3, rebuilt once per row sweep from the live groups
-      ScanReg sc;                  // hot-loop state: running maximum + the live 16-column group, in registers (epilogue.cuh)
-      ScanQueue<16> sq;            // further live groups of a near tie (thread-local memory, rarely touched)
-      float* my_share = &ctrl->share[t & 1][half][row_in_tile];
-      const float* partner_share = &ctrl->share[t & 1][1 - half][row_in_tile];
-
-      for (int ct = 0; ct < p.num_code_tiles; ++ct, ++it) {
-        const uint32_t as = it & 1;
-        { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->t_full[as]), (it >> 1) & 1); w_tfull += PROF_CLOCK() - c0; }
-        const long long cw0 = PROF_CLOCK();
-        tc_fence_after();
-        if (ct == 0) {  // the store warps computed this tile's row norms while the first accumulator was being built
-          { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->n_full[t & 1]), (t >> 1) & 1); w_nfull += PROF_CLOCK() - c0; }
-          // band = 2 * (MMA error bound) + 2 * (tag perturbation: 16 ulp <= 2^-19 |score|, |score| <= |x||c| + |c|^2/2)
-          // + (Euclid) the width over which the reference's own evaluation collapses distinct d^2 into one distance:
-          // d = sqrt(fl(fl(x2 + y2) - 2xy)) has ~d^2 * 2^-23 of resolution in d^2 (vqp:58-62); with a small-norm codebook
-          // (the default init) that exceeds the MMA band.  Rows inside it go to the exact re-score, which evaluates the
-          // reference formula including the sqrt.  In score units (d^2 / 2), with a 2x safety factor:
-          const float x2 = ctrl->xn2[t & 1][row_in_tile];
-          const float xn = sqrtf(x2);
-          const float xc = xn * cmax;
-          const bool euclid = p.metric != VQB_METRIC_COSINE;
-          // 2 * |score error|: what the passes leave out of the codebook (||x|| * cres) and of the row (xaux * caux), both by
-          // Cauchy-Schwarz on exact norms; the fp32 accumulation in the tensor core (margin_rel relative to ||x|| max||c||,
-          // 2^-20 relative to the bias it starts from); then the tag slack and the sqrt-collapse width.
-          sc.init(2.f * (xn * cres + ctrl->xlo[t & 1][row_in_tile] * caux + p.margin_rel * xc + (euclid ? 0x1p-21f * cmax * cmax : 0.f)) +
-                  0x1p-18f * (xc + (euclid ? 0.5f * cmax * cmax : 0.f)) +
-                  (euclid ? 0x1p-22f * (x2 + cmax * cmax) : 0.f) + 1e-30f);
-          // the slot of the NEXT row tile (same parity as the previous one) was last read before the pair barrier of
-          // that tile's merge, which both warps of the pair have passed
-          ctrl->share[(t + 1) & 1][half][row_in_tile] = -3.4e38f;
-        } else {
-          sc.raise(*partner_share);
-        }
-        const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(lg * 32) << 16) + as * 256;
-        const int code0 = ct * p.BN;
-        // This warp owns the 16-column pieces 4q + 2*half + {0,1} of the tile.  Two register buffers: the
-        // tcgen05.ld of the next piece is in flight while the current one is scanned.
-        auto piece_col = [&](int j) { return (4 * (j >> 1) + 2 * half + (j & 1)) << 4; };
-        const int np = np_warp;
-        auto scan16 = [&](const uint32_t (&r)[16], int cbase) {
-#ifdef VQB_PROFILE
-          if (p.dbg_mode & 16) { sc.t1 = fmaxf(sc.t1, max16(r)); return; }  // timing experiment: TMEM loads + max tree only
-#endif
-          sc.scan16<true, false>(sq, r, cbase, p.mul1);
-        };
-        // The accumulator stage goes back to the MMA issuer as soon as this warp's LAST tcgen05.ld has completed (the
-        // final piece is scanned from registers afterwards): the release -> MMA -> t_full loop is the critical path.
-        auto release_stage = [&]() {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {  // the leader's barrier gates the MMA issue into this accumulator stage of BOTH CTAs
-            if (leader) mbar_arrive(smem_u32(&ctrl->t_empty[as]));
-            else mbar_arrive_cluster_relaxed(as ? te_remote1 : te_remote0);
-          }
-        };
-        uint32_t buf0[16], buf1[16];
-#ifdef VQB_PROFILE
-        if (p.dbg_mode & 32) {  // timing experiment: the scan arithmetic alone, on (stale) registers
-#pragma unroll
-          for (int e = 0; e < 16; ++e) { buf0[e] = __float_as_uint(st.t3) + e + it; buf1[e] = buf0[e] ^ 0x3000u; }
-          release_stage();
-          for (int j = 0; j < np; j += 2) {
-            scan16(buf0, code0 + piece_col(j));
-            if (j + 1 < np) scan16(buf1, code0 + piece_col(j + 1));
-          }
-          w_work += PROF_CLOCK() - cw0;
-          continue;
-        }
-#endif
-        if (np > 0) tmem_ld_32x32b_x16(t_addr + piece_col(0), buf0);
-        else release_stage();
-        for (int j = 0; j < np; j += 2) {
-          tmem_wait_ld();
-          if (j + 1 < np) tmem_ld_32x32b_x16(t_addr + piece_col(j + 1), buf1);
-          else release_stage();
-          scan16(buf0, code0 + piece_col(j));
-          if (j + 1 < np) {
-            tmem_wait_ld();
-            if (j + 2 < np) tmem_ld_32x32b_x16(t_addr + piece_col(j + 2), buf0);
-            else release_stage();
-            scan16(buf1, code0 + piece_col(j + 1));
-          }
-        }
-        *my_share = sc.t1;
-        w_work += PROF_CLOCK() - cw0;
-      }
-      const long long cm0 = PROF_CLOCK();
-      sc.finish(sq, st, p.tagmask, p.mul1, p.mulm1);
-
-      // ---- merge the two column slices of each row (upper half publishes, lower half finishes the row)
-      MergeSlot* slot = &ctrl->merge[t & 1][row_in_tile];
-      if (half == 1) publish(slot, st);
-      named_bar_sync(pair_bar, 64);   // ONE call site for both warps of the pair (compute-sanitizer synccheck pairs barriers by PC)
-      if (half == 0) {
-        const RowResult rr = merge_slices(st, slot, 1, 0);
-        const int n = rr.n, i0 = rr.i0, i1 = rr.i1;
-        const float best = rr.best;
-        const int64_t row = static_cast<int64_t>(tile) * BM + row_in_tile;
-        // padding rows of a masked batch (vqp:1116-1119) are searched like any other row — the tile is dense — but take no
-        // part in anything afterwards: index -1, no tail (the caller pre-filled their outputs), no loss (vqp:1317-1325), no
-        // statistics (vqp:599-600: no histogram count, -1 in the provisional indices), never flagged
-        const bool live = row < p.N && (p.row_mask == nullptr || __ldg(p.row_mask + row) != 0);
-        if (TAIL >= 1 && p.fo.loss_sum && live && n < 2) {
-          // ||q - x||^2 = ||x||^2 - 2(x.c - 0.5||c||^2)  — the score already holds it (cosine: bias is 0, add ||c||^2).
-          // Differs from the reference's bf16 evaluation by << 1e-3 relative (DESIGN.md 4.1); flagged rows get the
-          // exact evaluation in vqb_fix_flagged.
-          float d2 = ctrl->xn2[t & 1][row_in_tile] - 2.f * best;
-          if (p.metric == VQB_METRIC_COSINE) d2 += __ldg(p.cnorm2 + i0);
-          epi_loss += fmaxf(d2, 0.f);
-        }
-        if (p.fo.enabled) {  // hand the certified winners of this tile to the store warps
-          mbar_wait(smem_u32(&ctrl->g_empty[t & 1]), ((t >> 1) & 1) ^ 1);
-          ctrl->gidx[t & 1][row_in_tile] = (live && n < 2) ? i0 : -1;
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&ctrl->g_full[t & 1]));
-        }
-        if (row < p.N && !live) {
-          p.idx[row] = -1;
-          if (p.idx_prov) p.idx_prov[row] = -1;
-        } else if (row < p.N) {
-          p.idx[row] = i0;
-          if (p.idx_prov) p.idx_prov[row] = (n < 2) ? i0 : -1;
-          if (p.hist && n < 2) atomicAdd(p.hist + static_cast<size_t>(tile >> p.hist_shift) * p.K + i0, 1);   // RED, fire and forget
-          if (p.dbg_best) p.dbg_best[row] = best;
-          if (n >= 2) {
-            // 2 or 3 candidates: front of the list (exact re-score of those codes); more: BACK of the list, growing
-            // downwards (whole-row exact re-scan) — the two kinds never share a slot (at most N entries in total)
-            const bool many = n > 3;
-            const int s = many ? static_cast<int>(p.N) - 1 - atomicAdd(p.flag_count + 1, 1) : atomicAdd(p.flag_count, 1);
-            vqb_flag_entry e;
-            e.row = static_cast<int32_t>(row);
-            e.cand0 = many ? 0 : i0;     // (cand0, cand1) of a re-scanned row is its 64-bit arg-max key: starts at 0
-            e.cand1 = many ? 0 : i1;
-            e.cand2 = rr.i2;
-            e.count = n;
-            e.pad[0] = e.pad[1] = e.pad[2] = 0;
-            p.flagged[s] = e;
-          }
-        }
-      }
-      w_merge += PROF_CLOCK() - cm0;
-    }
-    if (TAIL >= 1 && p.fo.loss_sum && half == 0) {
-      const double w = warp_sum(static_cast<double>(epi_loss));
-      if (lane == 0) atomicAdd(p.fo.loss_sum, w);
-    }
-    if (p.prof && lane == 0 && (ew == 0 || ew == 4)) {
-      long long* o = p.prof + blockIdx.x * 16 + 8 + (ew >> 2) * 4;
-      o[0] = w_tfull; o[1] = w_work; o[2] = w_merge; o[3] = PROF_CLOCK() - estart;
-      if (ew == 0) p.prof[blockIdx.x * 16 + 7] = w_nfull;
-    }
-  }
-
-  if (warp >= NUM_EPI_WARPS && warp < NUM_EPI_WARPS + NUM_STORE_WARPS) {
-    // ================================================================ store warps: row norms + fused gather tail
-    const int sw = warp - NUM_EPI_WARPS;
+  } else if (warp <= NUM_STORE_WARPS) {
+    // ================================================================ store warps: fused gather tail
+    const int sw = warp - 1;
     float lsum = 0.f;
-    // ||x||^2 of the 32 rows [sw*32, sw*32+32) of row tile t, from the A tile in smem, as soon as it has landed.
-    // Only the leader's barriers see the TMA bytes; its store warp 0 forwards "landed" to the follower.
-    // fp32 accumulation: the norm scales the certification band AND carries the commitment loss
-    // (sum ||q - x||^2 = sum ||x||^2 - 2 score), so it must be as exact as the scores.
-    auto bf16x2 = [](uint32_t w, float& v0, float& v1) { v0 = __uint_as_float(w << 16); v1 = __uint_as_float(w & 0xFFFF0000u); };
-    auto row_norms = [&](int t) {
-      float* xlo = ctrl->xlo[t & 1];
-      if (p.stream_a) {  // A is not resident: the norms come from the bf16 planes in global memory (L2: the TMA reads them next)
-        const int64_t row_t0 = static_cast<int64_t>((cluster_id + t * num_clusters) * 2 + static_cast<int>(rank)) * BM;
-        for (int i = 0; i < 32; ++i) {
-          const int64_t row = row_t0 + sw * 32 + i;
-          float acc = 0.f, alo = 0.f;
-          if (row < p.N) {
-            const uint16_t* h = p.a_global + row * p.D;
-            for (int c = lane * 8; c < p.D; c += 256) {
-              const uint4 u = __ldg(reinterpret_cast<const uint4*>(h + c));
-              uint4 l = make_uint4(0u, 0u, 0u, 0u);
-              if (p.n_a == 2) l = __ldg(reinterpret_cast<const uint4*>(h + p.N * p.D + c));
-              const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-              const uint32_t wl[4] = {l.x, l.y, l.z, l.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float h0, h1, l0, l1;
-                bf16x2(w[e], h0, h1);
-                bf16x2(wl[e], l0, l1);
-                acc = fmaf(h0 + l0, h0 + l0, acc);
-                acc = fmaf(h1 + l1, h1 + l1, acc);
-                alo = fmaf(l0, l0, alo);
-                alo = fmaf(l1, l1, alo);
-              }
-            }
-          }
-          acc = warp_sum(acc);
-          alo = warp_sum(alo);
-          if (lane == 0) { ctrl->xn2[t & 1][sw * 32 + i] = acc; xlo[sw * 32 + i] = sqrtf(alo) * 1.0001f; }
-        }
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(smem_u32(&ctrl->a_read));
-          mbar_arrive(smem_u32(&ctrl->n_full[t & 1]));
-        }
-        return;
-      }
-      const int sub = lane >> 3, chunk = lane & 7;  // conflict-free: a warp reads 4 full 128 B rows per request
-      {
-        if (leader) {
-          for (int s2 = 0; s2 < n_sub; ++s2) mbar_wait(smem_u32(&ctrl->a_full[s2]), t & 1);
-          if (sw == 0 && lane == 0) mbar_arrive_cluster(mapa_cluster(smem_u32(&ctrl->a_ready), 1));
-        } else {
-          mbar_wait_cluster(smem_u32(&ctrl->a_ready), t & 1);
-        }
-        // two rows per lane in flight, two partial sums per row: the dependent-FMA chain, not smem, bounds this loop.
-        // Two instantiations: the store warps share issue slots with the epilogue warps, and the ||x_lo|| sums of the
-        // fp32 path cost the bf16 path 30 % of the epilogue's throughput when they ran unconditionally.
-        auto resident = [&](auto lo_tag) {
-          constexpr bool LO = decltype(lo_tag)::value;
-          for (int i = 0; i < 8; i += 2) {
-            const int r0 = sw * 32 + i * 4 + sub, r1 = r0 + 4;
-            const uint32_t off0 = (r0 >> 3) * 1024 + (r0 & 7) * 128 + ((chunk ^ (r0 & 7)) << 4);
-            const uint32_t off1 = (r1 >> 3) * 1024 + (r1 & 7) * 128 + ((chunk ^ (r1 & 7)) << 4);
-            float acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
-            float alo[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // ||x_lo||^2 (fp32 inputs): sizes the x-side residual of the band
-#pragma unroll 4
-            for (int kb = 0; kb < p.KB; ++kb) {
-              uint4 u[2], l[2];
-              u[0] = *reinterpret_cast<const uint4*>(a_gen + kb * A_SUB_BYTES + off0);
-              u[1] = *reinterpret_cast<const uint4*>(a_gen + kb * A_SUB_BYTES + off1);
-              if (LO) {
-                l[0] = *reinterpret_cast<const uint4*>(a_gen + (p.KB + kb) * A_SUB_BYTES + off0);
-                l[1] = *reinterpret_cast<const uint4*>(a_gen + (p.KB + kb) * A_SUB_BYTES + off1);
-              }
-#pragma unroll
-              for (int b = 0; b < 2; ++b) {
-                const uint32_t w[4] = {u[b].x, u[b].y, u[b].z, u[b].w};
-                const uint32_t wl[4] = {l[b].x, l[b].y, l[b].z, l[b].w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  float h0, h1;
-                  bf16x2(w[e], h0, h1);
-                  if (LO) {
-                    float l0, l1;
-                    bf16x2(wl[e], l0, l1);
-                    alo[b][0] = fmaf(l0, l0, alo[b][0]);
-                    alo[b][1] = fmaf(l1, l1, alo[b][1]);
-                    h0 += l0;
-                    h1 += l1;
-                  }
-                  acc[b][0] = fmaf(h0, h0, acc[b][0]);
-                  acc[b][1] = fmaf(h1, h1, acc[b][1]);
-                }
-              }
-            }
-            float a0 = acc[0][0] + acc[0][1], a1 = acc[1][0] + acc[1][1];
-            float b0 = alo[0][0] + alo[0][1], b1 = alo[1][0] + alo[1][1];
-#pragma unroll
-            for (int m = 1; m <= 4; m <<= 1) {
-              a0 += __shfl_xor_sync(0xffffffffu, a0, m);
-              a1 += __shfl_xor_sync(0xffffffffu, a1, m);
-              if (LO) {
-                b0 += __shfl_xor_sync(0xffffffffu, b0, m);
-                b1 += __shfl_xor_sync(0xffffffffu, b1, m);
-              }
-            }
-            if (chunk == 0) {
-              ctrl->xn2[t & 1][r0] = a0; ctrl->xn2[t & 1][r1] = a1;
-              xlo[r0] = LO ? sqrtf(b0) * 1.0001f : 0.f; xlo[r1] = LO ? sqrtf(b1) * 1.0001f : 0.f;
-            }
-          }
-        };
-        if (p.n_a == 2) resident(std::true_type{}); else resident(std::false_type{});
-      }
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(smem_u32(&ctrl->a_read));        // the producer may refill A once the MMAs are done with it too
-        mbar_arrive(smem_u32(&ctrl->n_full[t & 1])); // release: the xn2 writes above are visible to the epilogue
-      }
-    };
-    if (my_tiles > 0) row_norms(0);
-    for (int t = 0; t < my_tiles; ++t) {
-      const int tile = (cluster_id + t * num_clusters) * 2 + static_cast<int>(rank);
-      // norms of the NEXT tile first: its A tile lands during this tile's last code tile, long before this tile's
-      // winners are published (xn2[(t+1)&1] was last read by the merge of tile t-1, which preceded our gather of t-1)
-      if (t + 1 < my_tiles) row_norms(t + 1);
-      if (!p.fo.enabled) continue;
+    for (int t = 0; p.fo.enabled && t < my_tiles; ++t) {
+      const int tile = static_cast<int>(blockIdx.x) + t * static_cast<int>(gridDim.x);
       mbar_wait(smem_u32(&ctrl->g_full[t & 1]), (t >> 1) & 1);
-      const int* gi = ctrl->gidx[t & 1] + sw * 32;
+      const int* gi = ctrl->gidx[t & 1];
       if (TAIL >= 1) {
         // copy mode: q[row] <- codebook row: bf16 inputs copy the bf16 hi plane (== embed.type(bf16)), fp32 inputs the fp32 row.
         // resid mode (a ResidualVQ stage): residual[row] <- x[row] - that same row, rounded once (rvq:524, vqp:1178); the x
-        // rows were just read by the TMA (L2).  A few instructions per element: these warps share their issue slots with the
-        // epilogue (the generic tail below made a stage 75 % slower than a plain search).
+        // rows were just read by the TMA (L2).
         constexpr int CB = 4;  // rows per batch: independent 16-byte loads in flight per lane
         const bool bf = p.fo.dtype == VQB_DTYPE_BF16;
         const int row_bytes = p.D * (bf ? 2 : 4);
         const uint8_t* src = bf ? reinterpret_cast<const uint8_t*>(p.b_hi) : reinterpret_cast<const uint8_t*>(p.fo.embed);
         const uint8_t* xin = TAIL == 2 ? static_cast<const uint8_t*>(p.fo.x_eff) : nullptr;
         uint8_t* dst = static_cast<uint8_t*>(TAIL == 2 ? p.fo.resid_out : p.fo.q_out);
-        for (int r0 = 0; r0 < 32; r0 += CB) {
+        for (int r0 = sw * CB; r0 < BM; r0 += NUM_STORE_WARPS * CB) {
           int ks[CB];
 #pragma unroll
           for (int b = 0; b < CB; ++b) ks[b] = gi[r0 + b];
-          const int64_t row_base = static_cast<int64_t>(tile) * BM + sw * 32 + r0;
+          const int64_t row_base = static_cast<int64_t>(tile) * BM + r0;
           if (p.fo.idx64_out && lane < CB && ks[lane & (CB - 1)] >= 0) {
             int kk = 0;
 #pragma unroll
@@ -756,24 +239,21 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
           }
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&ctrl->g_empty[t & 1]));
-        continue;
-      }
-      if (TAIL != 0) continue;   // (not reached: the branch above ends with continue; lets the compiler drop the generic tail)
-      constexpr int GB = 2;
-      for (int r0 = 0; r0 < 32; r0 += GB) {
-        int64_t rows[GB];
-        int ks[GB];
-        bool any = false;
+      } else {
+        constexpr int GB = 2;
+        for (int r0 = sw * GB; r0 < BM; r0 += NUM_STORE_WARPS * GB) {
+          int64_t rows[GB];
+          int ks[GB];
+          bool any = false;
 #pragma unroll
-        for (int b = 0; b < GB; ++b) {
-          ks[b] = gi[r0 + b];
-          rows[b] = ks[b] >= 0 ? static_cast<int64_t>(tile) * BM + sw * 32 + r0 + b : -1;
-          any |= ks[b] >= 0;
+          for (int b = 0; b < GB; ++b) {
+            ks[b] = gi[r0 + b];
+            rows[b] = ks[b] >= 0 ? static_cast<int64_t>(tile) * BM + r0 + b : -1;
+            any |= ks[b] >= 0;
+          }
+          if (!any) continue;
+          lsum += tail_rows<GB>(p.fo, rows, ks, p.D, lane);
         }
-        if (!any) continue;
-        lsum += tail_rows<GB>(p.fo, rows, ks, p.D, lane);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(smem_u32(&ctrl->g_empty[t & 1]));
@@ -782,19 +262,235 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const double w = warp_sum(static_cast<double>(lsum));
       if (lane == 0) atomicAdd(p.fo.loss_sum, w);
     }
-  }
+  } else {
+    // ================================================================ consumers (warpgroups 1 and 2)
+    const int wg = (warp >> 2) - 1;                              // 0: rows 0..63, 1: rows 64..127
+    const int q = lane & 3;                                      // column slice of the thread's rows
+    const int rit0 = wg * WM + (warp & 3) * 16 + (lane >> 2);    // the thread's rows: rit0 and rit0 + 8
+    const float cmax = __ldg(p.cmax);
+    // Exact norms of what the pass scheme leaves out of the codebook operand (code_operands.cuh): ||c - hi - lo|| for the
+    // bf16 split.  fp32 inputs (x = hi + lo + res, |res| <= 2^-8 |lo| per element) add x_res . c and the omitted
+    // x_lo . c_lo:  ||x_lo|| * caux.  (A hi-only single pass, n_passes == 1, also leaves out the lo plane.)
+    const float cres = __ldg(p.cmax + 2) + (p.n_passes == 1 ? __ldg(p.cmax + 3) : 0.f);
+    const float caux = p.n_a == 2 ? 0x1.02p-8f * cmax + __ldg(p.cmax + 3) : 0.f;
+    const int last_pass_a0 = p.n_passes >= 2 ? 1 : 0;  // last pass of a k-block that reads A plane 0
+    const int n_items = p.KB * p.n_passes;
+    const uint32_t a_row_off = wg * WM * 128;          // this warpgroup's 64 rows inside an A sub-tile (1024 B aligned)
+    long long w_full = 0;
+    const long long cstart = PROF_CLOCK();
+    float acc[64];
+    int stage = 0;
+    uint32_t ph = 0;
+    float epi_loss = 0.f;
+    auto release = [&](int st, int sub) {   // this warp's MMAs of a ring stage (and A sub-tile) have completed
+      if (lane == 0) {
+        mbar_arrive(smem_u32(&ctrl->b_empty[st]));
+        if (sub >= 0) mbar_arrive(smem_u32(&ctrl->a_empty[sub]));
+      }
+    };
+    for (int t = 0; t < my_tiles; ++t) {
+      const int tile = static_cast<int>(blockIdx.x) + t * static_cast<int>(gridDim.x);
+      ScanReg sc[2];               // hot-loop state of the two rows: running maximum + the live group, in registers
+      ScanQueue<16> sq[2];         // further live groups of a near tie (thread-local memory, rarely touched)
+      float x2[2] = {0.f, 0.f}, xlo[2] = {0.f, 0.f};
 
-  // ------------------------------------------------------------------ teardown
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // neither CTA may exit (or free TMEM) while its peer can still signal / read it
-  if (warp == WARP_MMA) tmem_dealloc_2sm(tmem_base, TMEM_COLS);
+      for (int ct = 0; ct < p.num_code_steps; ++ct) {
+        const bool last_ct = ct == p.num_code_steps - 1;
+        // seed the accumulators with -0.5||c||^2 (Euclid; 0 for cosine): b1 + b2 + b3 is exact in fp32.  Codes past Kpad
+        // (tiny codebooks) score -3e38: the TMA zero-fills their operand rows.
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+          for (int b = 0; b < 2; ++b) {
+            const int c = ct * WN + 8 * j + 2 * q + b;
+            float s = -3.0e38f;
+            if (c < p.Kpad) {
+              const uint2 u = __ldg(reinterpret_cast<const uint2*>(p.bext + static_cast<int64_t>(c) * 16));
+              s = (__uint_as_float(u.x << 16) + __uint_as_float(u.x & 0xFFFF0000u)) + __uint_as_float(u.y << 16);
+            }
+            acc[4 * j + b] = s;
+            acc[4 * j + 2 + b] = s;
+          }
+        }
+        // Items of a code step in k-block-major order (kb, ps) — the order the producer stages them in.  One wgmma group
+        // stays in flight: the stage of item i - 1 is released once item i has been issued.
+        int kb = 0, ps = 0;
+        int pend_stage = -1, pend_sub = -1;
+        for (int i = 0; i < n_items; ++i) {
+          const int aplane = (ps == 2) ? 1 : 0;
+          const int sub = aplane * p.KB + kb;
+          if (ct == 0 && !p.stream_a) mbar_wait(smem_u32(&ctrl->a_full[sub]), t & 1);
+          { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_full[stage]), ph); w_full += PROF_CLOCK() - c0; }
+          const uint32_t st_addr = b_base + stage * stage_stride;
+          const uint32_t a_addr = (p.stream_a ? st_addr : a_base + sub * A_SUB_BYTES) + a_row_off;
+          const uint64_t ad = wgmma_desc_sw128(a_addr);
+          const uint64_t bd = wgmma_desc_sw128(st_addr + a_stage_bytes);
+          fence_regs(acc);
+          wgmma_fence();
+          // four K=16 steps, descriptors advance by 32 B.  A ragged last k-block (D % 64 != 0) runs them all too: the TMA
+          // zero-fills both operands past D, so the extra steps add exact zeros (a data-dependent step count would make
+          // ptxas serialise the wgmmas)
+          wgmma_m64n128k16_bf16(acc, ad, bd);
+          wgmma_m64n128k16_bf16(acc, ad + 2, bd + 2);
+          wgmma_m64n128k16_bf16(acc, ad + 4, bd + 4);
+          wgmma_m64n128k16_bf16(acc, ad + 6, bd + 6);
+          wgmma_commit();
+          wgmma_wait<1>();
+          fence_regs(acc);
+          if (pend_stage >= 0) release(pend_stage, pend_sub);
+          const bool last_use = last_ct && !p.stream_a && (aplane == 1 ? ps == 2 : ps == last_pass_a0);
+          pend_stage = stage;
+          pend_sub = last_use ? sub : -1;
+          if (++stage == p.n_stages) { stage = 0; ph ^= 1; }
+          if (++ps == p.n_passes) { ps = 0; ++kb; }
+        }
+        if (ct == 0) {
+          // ||x||^2 of the thread's two rows (the quad splits each row), from the bf16 planes in global memory (L2: the TMA
+          // just read them), while the last MMAs of the step run.  fp32 accumulation: the norm scales the certification band
+          // AND carries the commitment loss (sum ||q - x||^2 = sum ||x||^2 - 2 score), so it must be as exact as the scores.
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int64_t row = static_cast<int64_t>(tile) * BM + rit0 + 8 * h;
+            float a = 0.f, alo = 0.f;
+            if (row < p.N) {
+              const uint16_t* hp = p.a_global + row * p.D;
+              for (int c = q * 8; c < p.D; c += 32) {
+                const uint4 u = __ldg(reinterpret_cast<const uint4*>(hp + c));
+                uint4 l = make_uint4(0u, 0u, 0u, 0u);
+                if (p.n_a == 2) l = __ldg(reinterpret_cast<const uint4*>(hp + p.N * p.D + c));
+                const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+                const uint32_t wl[4] = {l.x, l.y, l.z, l.w};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const float h0 = __uint_as_float(w[e] << 16), h1 = __uint_as_float(w[e] & 0xFFFF0000u);
+                  const float l0 = __uint_as_float(wl[e] << 16), l1 = __uint_as_float(wl[e] & 0xFFFF0000u);
+                  a = fmaf(h0 + l0, h0 + l0, a);
+                  a = fmaf(h1 + l1, h1 + l1, a);
+                  alo = fmaf(l0, l0, alo);
+                  alo = fmaf(l1, l1, alo);
+                }
+              }
+            }
+            a += __shfl_xor_sync(0xffffffffu, a, 1);
+            a += __shfl_xor_sync(0xffffffffu, a, 2);
+            alo += __shfl_xor_sync(0xffffffffu, alo, 1);
+            alo += __shfl_xor_sync(0xffffffffu, alo, 2);
+            x2[h] = a;
+            xlo[h] = alo;   // squared: the sqrt (a subroutine call) waits until no wgmma is in flight
+          }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        release(pend_stage, pend_sub);
+
+        if (ct == 0) {
+          const bool euclid = p.metric != VQB_METRIC_COSINE;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            // band = 2 * (MMA error bound) + 2 * (tag perturbation: 16 ulp <= 2^-19 |score|, |score| <= |x||c| + |c|^2/2)
+            // + (Euclid) the width over which the reference's own evaluation collapses distinct d^2 into one distance:
+            // d = sqrt(fl(fl(x2 + y2) - 2xy)) has ~d^2 * 2^-23 of resolution in d^2 (vqp:58-62); with a small-norm codebook
+            // (the default init) that exceeds the MMA band.  Rows inside it go to the exact re-score, which evaluates the
+            // reference formula including the sqrt.  In score units (d^2 / 2), with a 2x safety factor.
+            // 2 * |score error|: what the passes leave out of the codebook (||x|| * cres) and of the row (xaux * caux), both by
+            // Cauchy-Schwarz on exact norms; the fp32 accumulation in the tensor core (margin_rel relative to ||x|| max||c||,
+            // 2^-20 relative to the bias it starts from); then the tag slack and the sqrt-collapse width.
+            const float xn = sqrtf(x2[h]);
+            const float xc = xn * cmax;
+            xlo[h] = p.n_a == 2 ? sqrtf(xlo[h]) * 1.0001f : 0.f;
+            sc[h].init(2.f * (xn * cres + xlo[h] * caux + p.margin_rel * xc + (euclid ? 0x1p-21f * cmax * cmax : 0.f)) +
+                       0x1p-18f * (xc + (euclid ? 0.5f * cmax * cmax : 0.f)) +
+                       (euclid ? 0x1p-22f * (x2[h] + cmax * cmax) : 0.f) + 1e-30f);
+          }
+        } else {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {  // the row's running maximum over the quad raises every slice's skip threshold
+            float m = sc[h].t1;
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+            sc[h].raise(m);
+          }
+        }
+        // Per row, the thread holds two groups of 16 scores: group g = 8-column blocks 8g..8g+7, columns 2q, 2q + 1 of each
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int g = 0; g < 2; ++g) {
+            uint32_t r[16];
+#pragma unroll
+            for (int e = 0; e < 16; ++e) r[e] = __float_as_uint(acc[4 * (8 * g + (e >> 1)) + 2 * h + (e & 1)]);
+            sc[h].scan16<true, false>(sq[h], r, ct * WN + 64 * g + 2 * q, p.mul1);
+          }
+        }
+      }
+
+      // ---- merge the four column slices of each row (lanes 1..3 of the quad publish, lane 0 finishes the row)
+      if (p.fo.enabled) mbar_wait(smem_u32(&ctrl->g_empty[t & 1]), ((t >> 1) & 1) ^ 1);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int rit = rit0 + 8 * h;
+        RowState st;
+        sc[h].finish(sq[h], st, p.tagmask, p.mul1, p.mulm1);
+        MergeSlot* slots = ctrl->merge[rit];
+        if (q != 0) publish(&slots[q - 1], st);
+        __syncwarp();
+        if (q == 0) {
+          const RowResult rr = merge_slices(st, slots, 3, 1);
+          const int n = rr.n, i0 = rr.i0, i1 = rr.i1;
+          const float best = rr.best;
+          const int64_t row = static_cast<int64_t>(tile) * BM + rit;
+          // padding rows of a masked batch (vqp:1116-1119) are searched like any other row — the tile is dense — but take no
+          // part in anything afterwards: index -1, no tail (the caller pre-filled their outputs), no loss (vqp:1317-1325), no
+          // statistics (vqp:599-600: no histogram count, -1 in the provisional indices), never flagged
+          const bool live = row < p.N && (p.row_mask == nullptr || __ldg(p.row_mask + row) != 0);
+          if (TAIL >= 1 && p.fo.loss_sum && live && n < 2) {
+            // ||q - x||^2 = ||x||^2 - 2(x.c - 0.5||c||^2)  — the score already holds it (cosine: bias is 0, add ||c||^2).
+            // Differs from the reference's bf16 evaluation by << 1e-3 relative (DESIGN.md 4.1); flagged rows get the
+            // exact evaluation in vqb_fix_flagged.
+            float d2 = x2[h] - 2.f * best;
+            if (p.metric == VQB_METRIC_COSINE) d2 += __ldg(p.cnorm2 + i0);
+            epi_loss += fmaxf(d2, 0.f);
+          }
+          if (p.fo.enabled) ctrl->gidx[t & 1][rit] = (live && n < 2) ? i0 : -1;   // hand the certified winners to the store warps
+          if (row < p.N && !live) {
+            p.idx[row] = -1;
+            if (p.idx_prov) p.idx_prov[row] = -1;
+          } else if (row < p.N) {
+            p.idx[row] = i0;
+            if (p.idx_prov) p.idx_prov[row] = (n < 2) ? i0 : -1;
+            if (p.hist && n < 2) atomicAdd(p.hist + static_cast<size_t>(tile >> p.hist_shift) * p.K + i0, 1);   // RED, fire and forget
+            if (p.dbg_best) p.dbg_best[row] = best;
+            if (n >= 2) {
+              // 2 or 3 candidates: front of the list (exact re-score of those codes); more: BACK of the list, growing
+              // downwards (whole-row exact re-scan) — the two kinds never share a slot (at most N entries in total)
+              const bool many = n > 3;
+              const int s = many ? static_cast<int>(p.N) - 1 - atomicAdd(p.flag_count + 1, 1) : atomicAdd(p.flag_count, 1);
+              vqb_flag_entry e;
+              e.row = static_cast<int32_t>(row);
+              e.cand0 = many ? 0 : i0;     // (cand0, cand1) of a re-scanned row is its 64-bit arg-max key: starts at 0
+              e.cand1 = many ? 0 : i1;
+              e.cand2 = rr.i2;
+              e.count = n;
+              e.pad[0] = e.pad[1] = e.pad[2] = 0;
+              p.flagged[s] = e;
+            }
+          }
+        }
+        __syncwarp();   // the slots are reused by the next row / tile
+      }
+      if (p.fo.enabled && lane == 0) mbar_arrive(smem_u32(&ctrl->g_full[t & 1]));
+    }
+    if (TAIL >= 1 && p.fo.loss_sum) {
+      const double w = warp_sum(static_cast<double>(epi_loss));
+      if (lane == 0) atomicAdd(p.fo.loss_sum, w);
+    }
+    if (p.prof && threadIdx.x == 128) { p.prof[blockIdx.x * 16 + 2] = w_full; p.prof[blockIdx.x * 16 + 3] = PROF_CLOCK() - cstart; }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -873,10 +569,7 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   if (N <= 0 || D <= 0 || K <= 0 || (n_a != 1 && n_a != 2)) return VQB_E_INVALID;
   // Passes (bf16 operands, fp32 accumulation): A = the input rows (n_a = 1) or the bf16 hi / lo planes of an fp32 input
   // (n_a = 2), B = the bf16 hi / lo codebook planes — (x,c_hi)+(x,c_lo) [+ (x_lo,c_hi)]: residual ~2^-17 ||x|| ||c||, carried
-  // exactly by the band.  A SINGLE pass with fp16 operands (11 mantissa bits, residual ~2^-12) was built and measured in
-  // round 2 and removed again: tcgen05 kind::f16 rejects bf16 x fp16 in one instruction (illegal instruction), so the rows
-  // had to be converted to fp16 in a double-buffered A tile by the store warps; the kernel then turned epilogue-bound
-  // (261 vs 282 kcycles) while 22x more rows went to the exact re-score — slower per step.  DESIGN.md section 8.
+  // exactly by the band.  DESIGN.md section 8.
   if (n_passes == 0) n_passes = n_a + 1;
   if (n_passes != n_a + 1 && !(n_passes == 1 && n_a == 1)) return VQB_E_UNSUPPORTED;
   if (D % 8 != 0) return VQB_E_UNSUPPORTED;
@@ -889,55 +582,44 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
 
   AssignParams p;
   p.N = N; p.D = D; p.K = K;
-  p.BN = code_tile(K);
   p.Kpad = vqb_padded_codes(K);
   p.n_a = n_a; p.n_passes = n_passes; p.KB = KB;
   p.num_row_tiles = static_cast<int>((N + BM - 1) / BM);
-  p.num_code_tiles = p.Kpad / p.BN;
+  p.num_code_steps = (p.Kpad + WN - 1) / WN;
   p.margin_rel = margin_rel;
   p.cmax = cmax; p.idx = idx; p.idx_prov = idx_prov; p.hist = hist; p.hist_shift = hist_shift; p.flagged = flagged; p.flag_count = flag_count; p.dbg_best = dbg_best;
   p.row_mask = row_mask;
   p.prof = g_prof;
-  p.dbg_mode = g_dbg_mode;
   p.tagmask = 0xFFFFFFF0u; p.mul1 = 1u; p.mulm1 = 0xFFFFFFFFu;
   rc = make_fused(&p.fo, fused, D, N);
   if (rc) return rc;
   p.metric = metric;
   p.cnorm2 = cnorm2;
   p.b_hi = static_cast<const uint16_t*>(b_planes);   // plane 0: bf16(c) == the quantized row for bf16 inputs
+  p.bext = static_cast<const uint16_t*>(bext);
   // pure-copy tail: nothing needs x again (no residual / running sum / fused statistics); the cosine loss needs ||c||^2
   p.copy_mode = p.fo.enabled && !p.fo.resid_out && !p.fo.qsum && !p.fo.stats_sum &&
                 !(metric == VQB_METRIC_COSINE && p.fo.loss_sum && !cnorm2);
   // residual-only tail of a ResidualVQ stage on the raw rows (Euclidean, or inputs that were already unit vectors)
   p.resid_mode = p.fo.enabled && p.fo.resid_out && !p.fo.q_out && !p.fo.qsum && !p.fo.stats_sum &&
                  (!p.fo.x_raw || p.fo.x_raw == p.fo.x_eff) && !(metric == VQB_METRIC_COSINE && p.fo.loss_sum && !cnorm2);
-  p.score_loss = p.copy_mode || p.resid_mode;
-  // A stationary in smem when it leaves room for >= 3 ring stages; else (fp32 split input with D > 256) its k-blocks are
-  // streamed through the ring next to the codebook's (re-read from L2 for every code tile)
+  // A stationary in smem when it leaves room for a useful ring; else (fp32 split input with D > 256) its k-blocks are
+  // streamed through the ring next to the codebook's (re-read from L2 for every code step)
   p.stream_a = n_a * KB > MAX_A_SUB ? 1 : 0;
   p.a_global = static_cast<const uint16_t*>(a_planes);
   const int a_bytes = p.stream_a ? 0 : n_a * KB * A_SUB_BYTES;
-  const int b_stage = (p.BN / 2) * BK * 2 + (p.stream_a ? A_SUB_BYTES : 0);
-  const int x_stage = (p.BN / 2) * 32;
-  const int fixed = SMEM_CTRL_BYTES + 1024 /*align*/ + a_bytes + AEXT_BYTES + 1024 /*align of B ring*/;
-  int xstages = 2;
-  int stages = (SMEM_LIMIT - fixed - xstages * x_stage) / b_stage;
-  if (stages < 3) {  // tight (fp32 split input, D = 256): single-buffer the bias block to keep B stages
-    xstages = 1;
-    stages = (SMEM_LIMIT - fixed - xstages * x_stage) / b_stage;
-  }
+  const int stage_bytes = B_SUB_BYTES + (p.stream_a ? A_SUB_BYTES : 0);
+  const int fixed = SMEM_CTRL_BYTES + 1024 /*align*/ + a_bytes;
+  int stages = (SMEM_LIMIT - fixed) / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   if (stages < 2) return VQB_E_UNSUPPORTED;
   p.n_stages = stages;
-  p.n_xstages = xstages;
-  const int smem_bytes = fixed + xstages * x_stage + stages * b_stage;
+  const int smem_bytes = fixed + stages * stage_bytes;
 
-  CUtensorMap tmA, tmB, tmX;
+  CUtensorMap tmA, tmB;
   rc = make_map(&tmA, a_planes, D, N, n_a, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);  // plane stride = N*D either way
   if (rc) return rc;
-  rc = make_map(&tmB, b_planes, D, p.Kpad, 3, BK, p.BN / 2, CU_TENSOR_MAP_SWIZZLE_128B);   // planes: bf16 hi, bf16 lo, fp16
-  if (rc) return rc;
-  rc = make_map(&tmX, bext, 16, p.Kpad, 1, 16, p.BN / 2, CU_TENSOR_MAP_SWIZZLE_32B);
+  rc = make_map(&tmB, b_planes, D, p.Kpad, 3, BK, WN, CU_TENSOR_MAP_SWIZZLE_128B);   // planes: bf16 hi, bf16 lo, fp16
   if (rc) return rc;
 
   static bool attr_set = false;
@@ -948,24 +630,10 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
     if (e != cudaSuccess) return static_cast<int>(e);
     attr_set = true;
   }
-  const int num_pairs = (p.num_row_tiles + 1) / 2;
-  const int max_clusters = num_sms() / 2;
-  const int clusters = num_pairs < max_clusters ? num_pairs : max_clusters;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = smem_bytes;
-  cfg.stream = static_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t le = p.copy_mode    ? cudaLaunchKernelEx(&cfg, vq_assign_kernel<1>, tmA, tmB, tmX, p)
-                   : p.resid_mode ? cudaLaunchKernelEx(&cfg, vq_assign_kernel<2>, tmA, tmB, tmX, p)
-                                  : cudaLaunchKernelEx(&cfg, vq_assign_kernel<0>, tmA, tmB, tmX, p);
-  if (le != cudaSuccess) return static_cast<int>(le);
+  const int grid = p.num_row_tiles < num_sms() ? p.num_row_tiles : num_sms();
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (p.copy_mode) vq_assign_kernel<1><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, p);
+  else if (p.resid_mode) vq_assign_kernel<2><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, p);
+  else vq_assign_kernel<0><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, p);
   return static_cast<int>(cudaGetLastError());
 }

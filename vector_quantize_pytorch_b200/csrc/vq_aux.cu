@@ -529,9 +529,9 @@ extern "C" const char* vqb_strerror(int code) {
   switch (code) {
     case VQB_OK: return "ok";
     case VQB_E_INVALID: return "vqb200: invalid argument (null pointer, non-positive size or bad enum)";
-    case VQB_E_UNSUPPORTED: return "vqb200: shape not supported by the sm_100a kernels (need D % 8 == 0, D <= 1024)";
+    case VQB_E_UNSUPPORTED: return "vqb200: shape not supported by the sm_90a kernels (need D % 8 == 0, D <= 1024)";
     case VQB_E_ALIGN: return "vqb200: pointer is not 16-byte aligned";
-    case VQB_E_NO_DEVICE: return "vqb200: no CUDA device or device is not compute capability 10.x (B200)";
+    case VQB_E_NO_DEVICE: return "vqb200: no CUDA device or device is not compute capability 9.x (H100)";
     case VQB_E_DRIVER: return "vqb200: cuTensorMapEncodeTiled unavailable or failed";
     case VQB_E_WORKSPACE: return "vqb200: workspace too small";
     default: break;

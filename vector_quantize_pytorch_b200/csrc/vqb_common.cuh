@@ -30,7 +30,7 @@ inline int check_device() {
   int sms, major;
   int rc = device_props(&sms, &major);
   if (rc) return rc;
-  return major == 10 ? VQB_OK : VQB_E_NO_DEVICE;
+  return major == 9 ? VQB_OK : VQB_E_NO_DEVICE;   // the library carries sm_90a code only
 }
 inline int num_sms() {
   int sms = 1, major;

@@ -5,7 +5,7 @@ ranks (one process per GPU) and the only exchange is the SUM of the per-rank bat
 reference issues two all-reduces per codebook per stage (vector_quantize_pytorch.py:603, :607); here
 every codebook touched by a forward writes its statistics into ONE packed fp32 buffer
 `[cluster_size (K, padded to 4) | embed_sum (K x D)]*` and a single `all_reduce` (NCCL over NVLink on
-B200, gloo in the CPU tests) covers them all.  After the reduction every rank applies the identical EMA
+GPUs, gloo in the CPU tests) covers them all.  After the reduction every rank applies the identical EMA
 kernel to identical numbers, so the replicas' codebooks stay bit-identical.
 """
 from __future__ import annotations

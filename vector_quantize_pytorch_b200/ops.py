@@ -17,14 +17,13 @@ from ._C import lib, check
 # Cauchy-Schwarz on the EXACT norms of what the pass scheme leaves out (csrc/code_operands.cuh, vq_assign.cu) — single fp16
 # pass: cres = max_k ||c - fp16 plane||, xaux = norm of the row's flushed elements; bf16 split: cres = max_k ||c - hi - lo||,
 # and for fp32 inputs xaux = ||x_lo|| with caux = 2^-8 max||c|| + max||c_lo|| — plus `margin` for the fp32 accumulation in the
-# tensor core alone: the TOTAL error of the bf16 split was measured at <= 2^-19.3 ||x|| max||c|| on B200, so 2^-18 for the
-# accumulation share keeps > 2.5x.  tests/test_parity_gpu.py::test_score_error_inside_margin asserts the bound for every
+# tensor core alone (2^-18; its room is measured on the GPU by the test below).  tests/test_parity_gpu.py::test_score_error_inside_margin asserts the bound for every
 # scheme on randn, heavy-tailed, tiny, unit-norm and default-init data.  See DESIGN.md 4.1.
 DEFAULT_MARGIN = 2.0 ** -18
 
 _DT = {torch.float32: _C.DTYPE_F32, torch.bfloat16: _C.DTYPE_BF16}
 
-# bench.py instrumentation: when PROFILE_EVENTS is a list, `search` brackets the tcgen05 kernel with CUDA
+# bench.py instrumentation: when PROFILE_EVENTS is a list, `search` brackets the search kernel with CUDA
 # events on the launching stream; LAUNCHES counts the kernels this library enqueues.
 PROFILE_EVENTS = None
 LAUNCHES = 0
@@ -45,7 +44,7 @@ def _dtype_code(t: torch.Tensor) -> int:
 def _require_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("vqb200 has no CPU path: tensors must live on a CUDA (B200, sm_100) device")
+            raise RuntimeError("vqb200 has no CPU path: tensors must live on a CUDA (H100, sm_90) device")
 
 
 def _p(t):

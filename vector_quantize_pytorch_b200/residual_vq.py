@@ -283,7 +283,7 @@ class ResidualVQ(nn.Module):
         if beam_size is not None and beam_size > 1:
             _unsupported("beam search")
         if not x.is_cuda:
-            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (B200, sm_100) device")
+            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
         if mask is not None:
             return self._forward_masked(x, mask, return_all_codes, freeze_codebook, rand_quantize_dropout_fixed_seed)
         if not _projected:   # _projected: the masked path hands in compacted rows that went through project_in already

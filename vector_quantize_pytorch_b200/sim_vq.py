@@ -41,7 +41,7 @@ class SimVQ(nn.Module):
 
     def forward(self, x):
         if not x.is_cuda:
-            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (B200, sm_100) device")
+            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
         if self.channel_first:
             x = x.movedim(1, -1)
         shape = x.shape

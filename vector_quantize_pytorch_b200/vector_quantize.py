@@ -3,7 +3,7 @@ default path: heads=1, no mask, Euclidean or cosine codebook with EMA updates.
 
 forward(x) -> (quantize [x.dtype, x.shape], embed_ind [int64, x.shape[:-1]], loss [fp32 scalar]).
 Layout handling, projections, STE / rotation trick stay PyTorch glue; the search, gather, commitment
-loss and EMA run in the sm_100a kernels.  Unsupported constructor / forward options raise.
+loss and EMA run in the sm_90a kernels.  Unsupported constructor / forward options raise.
 """
 from __future__ import annotations
 
@@ -33,7 +33,7 @@ def straight_through(src, tgt):  # vqp:282-283
 
 
 class _RotateTo(torch.autograd.Function):
-    """Rotation-trick gradient estimator (arXiv:2410.06424 §4.2; reference vqp:287-318) on the sm_100a kernels: the forward
+    """Rotation-trick gradient estimator (arXiv:2410.06424 §4.2; reference vqp:287-318) on the sm_90a kernels: the forward
     value (numerically the quantized vector) and d/d src — the direction / norm factors are constants of the backward pass,
     exactly like the reference's `.detach()`s."""
 
@@ -274,7 +274,7 @@ class VectorQuantize(nn.Module):
         cbk = self._codebook
         emb = cbk.embed
         if not emb.is_cuda:
-            raise RuntimeError("vqb200 has no CPU path: move the module to a CUDA (B200) device")
+            raise RuntimeError("vqb200 has no CPU path: move the module to a CUDA (H100) device")
         if x_host.is_cuda or x_host.dtype not in (torch.float32, torch.bfloat16):
             raise TypeError("forward_host expects a float32 / bfloat16 CPU tensor (pinned for full overlap)")
         dev = emb.device
@@ -361,7 +361,7 @@ class VectorQuantize(nn.Module):
         if x.requires_grad and torch.is_grad_enabled():
             _unsupported("mask / lens on inputs that require grad")
         if not x.is_cuda:
-            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (B200, sm_100) device")
+            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
         assert x.ndim == 3 and mask.shape == x.shape[:2]
         freeze_codebook = self.freeze_codebook if freeze_codebook is None else freeze_codebook
         cbk = self._codebook
@@ -509,7 +509,7 @@ class VectorQuantize(nn.Module):
         if topk is not None or codebook_transform_fn is not None:
             _unsupported("topk / codebook_transform_fn")
         if not x.is_cuda:
-            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (B200, sm_100) device")
+            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
 
         freeze_codebook = self.freeze_codebook if freeze_codebook is None else freeze_codebook
         ema_update = self._codebook.ema_update if ema_update is None else ema_update
