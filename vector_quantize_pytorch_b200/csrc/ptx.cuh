@@ -65,6 +65,19 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
+// 1-D bulk copy global -> shared (bytes: a multiple of 16, both addresses 16-byte aligned), completion counted on `bar`.
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
+               : "memory");
+}
+// Pull a 3-D box into L2 only (no shared memory, no barrier): warms the next tile's operand while this one computes.
+__device__ __forceinline__ void tma_prefetch_l2_3d(const CUtensorMap* m, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+
 // ---------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor for a K-major bf16 operand tile stored as rows of 128 B with the 128-byte swizzle
 // (what a TMA box of 64 bf16 x R rows with CU_TENSOR_MAP_SWIZZLE_128B produces): 8-row groups are 1024 B apart (SBO),

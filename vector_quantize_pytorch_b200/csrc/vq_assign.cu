@@ -47,6 +47,7 @@ constexpr int NUM_STORE_WARPS = 3;      // warps 1..3 (warp 0 is the TMA produce
 constexpr int NUM_THREADS = 128 + NUM_CONSUMER_WARPS * 32;
 constexpr int SMEM_CTRL_BYTES = 14336;  // barriers + winner hand-off + merge area
 constexpr int SMEM_LIMIT = 232448;      // 227 KiB opt-in maximum per CTA
+constexpr int SEED_BYTES = WN * 32;     // one code step of bext ([128 codes][16] bf16): the accumulator seeds
 
 struct AssignParams {
   int64_t N;
@@ -54,6 +55,8 @@ struct AssignParams {
   int n_a, n_passes;   // pass 0 (a0,c_hi), 1 (a0,c_lo), 2 (a1,c_hi): bf16 operands, fp32 accumulation
   int KB;              // ceil(D / 64)
   int n_stages;
+  int n_seed;          // seed slots: ceil(n_stages / items per code step), so that a slot is refilled only after every
+                       // consumer released the first item of the step that last used it
   int stream_a;        // A does not fit in smem next to a useful B ring (fp32 split input with D > 256): its k-blocks travel
                        // through the ring together with the codebook k-blocks (re-read from L2 for every code step)
   const uint16_t* a_global;   // [n_a][N][D] bf16: the A planes in global memory (row norms)
@@ -110,6 +113,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   // ring stage = [A k-block (stream_a only) | codebook k-block of the code step]
   const uint32_t a_stage_bytes = p.stream_a ? A_SUB_BYTES : 0;
   const uint32_t stage_stride = a_stage_bytes + B_SUB_BYTES;
+  const uint32_t seed_base = b_base + p.n_stages * stage_stride;             // [n_seed][128 codes][16] bf16
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -138,13 +142,17 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (warp == 0) {
     // ================================================================ TMA producer
     if (lane == 0) {
-      long long w_empty = 0;
+      long long w_empty = 0, w_aempty = 0;
       const long long pstart = PROF_CLOCK();
-      int stage = 0;
+      int stage = 0, gstep = 0;
       uint32_t ph = 0;
       for (int t = 0; t < my_tiles; ++t) {
         const int row0 = (static_cast<int>(blockIdx.x) + t * static_cast<int>(gridDim.x)) * BM;
-        for (int ct = 0; ct < p.num_code_steps; ++ct) {
+        if (!p.stream_a && t + 1 < my_tiles) {   // the next tile's x into L2: its refill below then does not wait on HBM
+          for (int ap = 0; ap < p.n_a; ++ap)
+            for (int kb = 0; kb < p.KB; ++kb) tma_prefetch_l2_3d(&tmA, kb * BK, row0 + static_cast<int>(gridDim.x) * BM, ap);
+        }
+        for (int ct = 0; ct < p.num_code_steps; ++ct, ++gstep) {
           // k-block-major: all passes of a k-block back to back, so that in the LAST code step of a row tile an A sub-tile
           // is released (and refilled for the next row tile) as early as possible
           for (int kb = 0; kb < p.KB; ++kb) {
@@ -153,12 +161,18 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               const int aplane = (ps == 2) ? 1 : 0;
               if (!p.stream_a && ct == 0 && (ps == 0 || ps == 2)) {  // refill this A sub-tile once the previous row tile released it
                 const int sub = aplane * p.KB + kb;
-                mbar_wait(smem_u32(&ctrl->a_empty[sub]), (t & 1) ^ 1);
+                { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->a_empty[sub]), (t & 1) ^ 1); w_aempty += PROF_CLOCK() - c0; }
                 mbar_arrive_expect_tx(smem_u32(&ctrl->a_full[sub]), A_SUB_BYTES);
                 tma_load_3d(a_base + sub * A_SUB_BYTES, &tmA, smem_u32(&ctrl->a_full[sub]), kb * BK, row0, aplane);
               }
               { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_empty[stage]), ph ^ 1); w_empty += PROF_CLOCK() - c0; }
-              mbar_arrive_expect_tx(smem_u32(&ctrl->b_full[stage]), stage_stride);
+              // the step's seeds ride on the barrier of its first item
+              const int seed_codes = min(WN, p.Kpad - ct * WN);
+              const uint32_t seed_bytes = (kb == 0 && ps == 0) ? seed_codes * 32 : 0;
+              mbar_arrive_expect_tx(smem_u32(&ctrl->b_full[stage]), stage_stride + seed_bytes);
+              if (seed_bytes)
+                bulk_load(seed_base + (gstep % p.n_seed) * SEED_BYTES, p.bext + static_cast<int64_t>(ct) * WN * 16, seed_bytes,
+                          smem_u32(&ctrl->b_full[stage]));
               if (p.stream_a)
                 tma_load_3d(b_base + stage * stage_stride, &tmA, smem_u32(&ctrl->b_full[stage]), kb * BK, row0, aplane);
               tma_load_3d(b_base + stage * stage_stride + a_stage_bytes, &tmB, smem_u32(&ctrl->b_full[stage]), kb * BK,
@@ -168,7 +182,11 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
         }
       }
-      if (p.prof) { p.prof[blockIdx.x * 16 + 0] = w_empty; p.prof[blockIdx.x * 16 + 1] = PROF_CLOCK() - pstart; }
+      if (p.prof) {
+        p.prof[blockIdx.x * 16 + 0] = w_empty;
+        p.prof[blockIdx.x * 16 + 1] = PROF_CLOCK() - pstart;
+        p.prof[blockIdx.x * 16 + 6] = w_aempty;
+      }
     }
   } else if (warp <= NUM_STORE_WARPS) {
     // ================================================================ store warps: fused gather tail
@@ -276,10 +294,10 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int last_pass_a0 = p.n_passes >= 2 ? 1 : 0;  // last pass of a k-block that reads A plane 0
     const int n_items = p.KB * p.n_passes;
     const uint32_t a_row_off = wg * WM * 128;          // this warpgroup's 64 rows inside an A sub-tile (1024 B aligned)
-    long long w_full = 0;
+    long long w_full = 0, w_afull = 0, w_gap = 0, gap0 = -1;   // gap: last commit of a step -> first wait of the next
     const long long cstart = PROF_CLOCK();
     float acc[64];
-    int stage = 0;
+    int stage = 0, gstep = 0;
     uint32_t ph = 0;
     float epi_loss = 0.f;
     auto release = [&](int st, int sub) {   // this warp's MMAs of a ring stage (and A sub-tile) have completed
@@ -296,20 +314,26 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
       for (int ct = 0; ct < p.num_code_steps; ++ct) {
         const bool last_ct = ct == p.num_code_steps - 1;
-        // seed the accumulators with -0.5||c||^2 (Euclid; 0 for cosine): b1 + b2 + b3 is exact in fp32.  Codes past Kpad
-        // (tiny codebooks) score -3e38: the TMA zero-fills their operand rows.
+        // seed the accumulators with -0.5||c||^2 (Euclid; 0 for cosine): b1 + b2 + b3 is exact in fp32.  The producer
+        // loaded the step's bext rows into shared memory on the barrier of the step's first item.  Codes past Kpad (tiny
+        // codebooks) score -3e38: the TMA zero-fills their operand rows.
+        if (gap0 >= 0) w_gap += PROF_CLOCK() - gap0;
+        { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_full[stage]), ph); w_full += PROF_CLOCK() - c0; }
+        {
+          const uint2* seeds = reinterpret_cast<const uint2*>(smem + (seed_base - smem_base) + (gstep % p.n_seed) * SEED_BYTES);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
+          for (int j = 0; j < 16; ++j) {
 #pragma unroll
-          for (int b = 0; b < 2; ++b) {
-            const int c = ct * WN + 8 * j + 2 * q + b;
-            float s = -3.0e38f;
-            if (c < p.Kpad) {
-              const uint2 u = __ldg(reinterpret_cast<const uint2*>(p.bext + static_cast<int64_t>(c) * 16));
-              s = (__uint_as_float(u.x << 16) + __uint_as_float(u.x & 0xFFFF0000u)) + __uint_as_float(u.y << 16);
+            for (int b = 0; b < 2; ++b) {
+              const int cl = 8 * j + 2 * q + b;
+              float s = -3.0e38f;
+              if (ct * WN + cl < p.Kpad) {
+                const uint2 u = seeds[cl * 4];
+                s = (__uint_as_float(u.x << 16) + __uint_as_float(u.x & 0xFFFF0000u)) + __uint_as_float(u.y << 16);
+              }
+              acc[4 * j + b] = s;
+              acc[4 * j + 2 + b] = s;
             }
-            acc[4 * j + b] = s;
-            acc[4 * j + 2 + b] = s;
           }
         }
         // Items of a code step in k-block-major order (kb, ps) — the order the producer stages them in.  One wgmma group
@@ -319,8 +343,8 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = 0; i < n_items; ++i) {
           const int aplane = (ps == 2) ? 1 : 0;
           const int sub = aplane * p.KB + kb;
-          if (ct == 0 && !p.stream_a) mbar_wait(smem_u32(&ctrl->a_full[sub]), t & 1);
-          { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_full[stage]), ph); w_full += PROF_CLOCK() - c0; }
+          if (ct == 0 && !p.stream_a) { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->a_full[sub]), t & 1); w_afull += PROF_CLOCK() - c0; }
+          if (i > 0) { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_full[stage]), ph); w_full += PROF_CLOCK() - c0; }
           const uint32_t st_addr = b_base + stage * stage_stride;
           const uint32_t a_addr = (p.stream_a ? st_addr : a_base + sub * A_SUB_BYTES) + a_row_off;
           const uint64_t ad = wgmma_desc_sw128(a_addr);
@@ -335,6 +359,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           wgmma_m64n128k16_bf16(acc, ad + 4, bd + 4);
           wgmma_m64n128k16_bf16(acc, ad + 6, bd + 6);
           wgmma_commit();
+          if (i == n_items - 1) gap0 = PROF_CLOCK();
           wgmma_wait<1>();
           fence_regs(acc);
           if (pend_stage >= 0) release(pend_stage, pend_sub);
@@ -382,6 +407,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         wgmma_wait<0>();
         fence_regs(acc);
         release(pend_stage, pend_sub);
+        ++gstep;
 
         if (ct == 0) {
           const bool euclid = p.metric != VQB_METRIC_COSINE;
@@ -484,7 +510,12 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const double w = warp_sum(static_cast<double>(epi_loss));
       if (lane == 0) atomicAdd(p.fo.loss_sum, w);
     }
-    if (p.prof && threadIdx.x == 128) { p.prof[blockIdx.x * 16 + 2] = w_full; p.prof[blockIdx.x * 16 + 3] = PROF_CLOCK() - cstart; }
+    if (p.prof && threadIdx.x == 128) {
+      p.prof[blockIdx.x * 16 + 2] = w_full;
+      p.prof[blockIdx.x * 16 + 3] = PROF_CLOCK() - cstart;
+      p.prof[blockIdx.x * 16 + 4] = w_gap;
+      p.prof[blockIdx.x * 16 + 5] = w_afull;
+    }
   }
 }
 
@@ -610,11 +641,16 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   const int a_bytes = p.stream_a ? 0 : n_a * KB * A_SUB_BYTES;
   const int stage_bytes = B_SUB_BYTES + (p.stream_a ? A_SUB_BYTES : 0);
   const int fixed = SMEM_CTRL_BYTES + 1024 /*align*/ + a_bytes;
-  int stages = (SMEM_LIMIT - fixed) / stage_bytes;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
+  // ring stages + seed slots (one slot per code step the ring can run ahead).  The tightest case, fp32 at D = 256, keeps
+  // its 5 stages: 15 KiB + 128 KiB of A + 5 * 16 KiB + 4 KiB of seeds = exactly 227 KiB.
+  const int n_items = KB * n_passes;
+  int stages = MAX_STAGES;
+  auto seed_slots = [&](int st) { return (st + n_items - 1) / n_items; };
+  while (stages >= 2 && fixed + stages * stage_bytes + seed_slots(stages) * SEED_BYTES > SMEM_LIMIT) --stages;
   if (stages < 2) return VQB_E_UNSUPPORTED;
   p.n_stages = stages;
-  const int smem_bytes = fixed + stages * stage_bytes;
+  p.n_seed = seed_slots(stages);
+  const int smem_bytes = fixed + stages * stage_bytes + p.n_seed * SEED_BYTES;
 
   CUtensorMap tmA, tmB;
   rc = make_map(&tmA, a_planes, D, N, n_a, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);  // plane stride = N*D either way
