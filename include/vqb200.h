@@ -139,6 +139,10 @@ int vqb_debug_set_mode(int mode); /* nonzero: diagnostics mode (the forward chai
 /* How vqb_vq_forward's CUDA-graph cache served the calls so far: out4 = {replayed, patched (cudaGraphExecUpdate),
  * instantiated, enqueued launch by launch after a capture / instantiate failure} (host array of 4 int64). */
 int vqb_debug_graph_stats(long long* out4);
+/* The shared-memory plan vqb_assign launches with for (n_a, D, n_passes) — host only, no device needed.  out6 (host int[6]) =
+ * {stream_a (A k-blocks travel through the ring), ring stages, seed slots, ring items per code step, ceil(D/64), dynamic smem
+ * bytes}.  Returns the code vqb_assign returns for that input (VQB_E_INVALID / VQB_E_UNSUPPORTED) when it is not supported. */
+int vqb_debug_assign_plan(int n_a, int D, int n_passes, int* out6);
 
 /* Exact re-score of the flagged rows with the reference's own fp32 formula and tie rule
  * (-(x2 + y2 - 2xy).clamp(1e-8).sqrt(), first maximal index; :58-62, :140).  Rewrites idx[row]. */

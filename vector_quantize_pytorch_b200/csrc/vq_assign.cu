@@ -99,6 +99,26 @@ __device__ __forceinline__ float tail_rows(const FusedOut& fo, const int64_t (&r
   return gather_rows<VQB_DTYPE_F32, GB>(fo, rows, ks, D, lane);
 }
 
+// sum((q - x)^2) over one 16-byte chunk of a row and its code row, rounded like F.mse_loss in the rows' dtype (vqp:1327):
+// the square of each fp32 difference, rounded to bf16 for bf16 rows.  The order of the difference does not change its square.
+__device__ __forceinline__ float sq_diff16(const uint4& xa, const uint4& ca, bool bf) {
+  const uint32_t xw[4] = {xa.x, xa.y, xa.z, xa.w}, cw[4] = {ca.x, ca.y, ca.z, ca.w};
+  float s = 0.f;
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    if (bf) {
+      const float d0 = __uint_as_float(xw[e] << 16) - __uint_as_float(cw[e] << 16);
+      const float d1 = __uint_as_float(xw[e] & 0xFFFF0000u) - __uint_as_float(cw[e] & 0xFFFF0000u);
+      s += bf16_round(d0 * d0);
+      s += bf16_round(d1 * d1);
+    } else {
+      const float d = __uint_as_float(xw[e]) - __uint_as_float(cw[e]);
+      s += d * d;
+    }
+  }
+  return s;
+}
+
 // TAIL selects the work of the store warps at compile time (one instantiation each: the variants do not share a register
 // budget): 0 = none / generic (x re-read: running sum, fused statistics, cosine residual), 1 = copy mode, 2 = resid mode.
 template <int TAIL>
@@ -204,12 +224,17 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const bool bf = p.fo.dtype == VQB_DTYPE_BF16;
         const int row_bytes = p.D * (bf ? 2 : 4);
         const uint8_t* src = bf ? reinterpret_cast<const uint8_t*>(p.b_hi) : reinterpret_cast<const uint8_t*>(p.fo.embed);
-        const uint8_t* xin = TAIL == 2 ? static_cast<const uint8_t*>(p.fo.x_eff) : nullptr;
+        const uint8_t* xin = static_cast<const uint8_t*>(p.fo.x_eff);
         uint8_t* dst = static_cast<uint8_t*>(TAIL == 2 ? p.fo.resid_out : p.fo.q_out);
         for (int r0 = sw * CB; r0 < BM; r0 += NUM_STORE_WARPS * CB) {
           int ks[CB];
+          bool ex[CB];   // the row's loss is evaluated here, from x and the code row
 #pragma unroll
-          for (int b = 0; b < CB; ++b) ks[b] = gi[r0 + b];
+          for (int b = 0; b < CB; ++b) {
+            const int g = gi[r0 + b];
+            ex[b] = g < -1;
+            ks[b] = ex[b] ? -2 - g : g;
+          }
           const int64_t row_base = static_cast<int64_t>(tile) * BM + r0;
           if (p.fo.idx64_out && lane < CB && ks[lane & (CB - 1)] >= 0) {
             int kk = 0;
@@ -217,12 +242,17 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int b = 0; b < CB; ++b) kk = (lane == b) ? ks[b] : kk;
             p.fo.idx64_out[(row_base + lane) * p.fo.idx_stride] = kk;
           }
-          if (dst) {
+          if (dst || (ex[0] | ex[1] | ex[2] | ex[3])) {
             for (int off = lane * 16; off < row_bytes; off += 512) {
               uint4 v[CB];
 #pragma unroll
               for (int b = 0; b < CB; ++b)
                 if (ks[b] >= 0) v[b] = __ldg(reinterpret_cast<const uint4*>(src + static_cast<int64_t>(ks[b]) * row_bytes + off));
+              if (TAIL == 1) {
+#pragma unroll
+                for (int b = 0; b < CB; ++b)
+                  if (ex[b]) lsum += sq_diff16(*reinterpret_cast<const uint4*>(xin + (row_base + b) * row_bytes + off), v[b], bf);
+              }
               if (TAIL == 2) {
                 uint4 x[CB];
 #pragma unroll
@@ -231,6 +261,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
                 for (int b = 0; b < CB; ++b) {
                   if (ks[b] < 0) continue;
+                  if (ex[b]) lsum += sq_diff16(x[b], v[b], bf);
                   const uint32_t xw[4] = {x[b].x, x[b].y, x[b].z, x[b].w}, cw[4] = {v[b].x, v[b].y, v[b].z, v[b].w};
                   uint32_t rw[4];
                   if (bf) {
@@ -253,7 +284,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               }
 #pragma unroll
               for (int b = 0; b < CB; ++b)
-                if (ks[b] >= 0) *reinterpret_cast<uint4*>(dst + (row_base + b) * row_bytes + off) = v[b];
+                if (dst && ks[b] >= 0) *reinterpret_cast<uint4*>(dst + (row_base + b) * row_bytes + off) = v[b];
             }
           }
         }
@@ -276,7 +307,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       __syncwarp();
       if (lane == 0) mbar_arrive(smem_u32(&ctrl->g_empty[t & 1]));
     }
-    if (TAIL == 0 && p.fo.enabled && p.fo.loss_sum) {
+    if (p.fo.enabled && p.fo.loss_sum) {   // generic tail: every row; copy / resid: the rows left to the store warps
       const double w = warp_sum(static_cast<double>(lsum));
       if (lane == 0) atomicAdd(p.fo.loss_sum, w);
     }
@@ -469,15 +500,20 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           // part in anything afterwards: index -1, no tail (the caller pre-filled their outputs), no loss (vqp:1317-1325), no
           // statistics (vqp:599-600: no histogram count, -1 in the provisional indices), never flagged
           const bool live = row < p.N && (p.row_mask == nullptr || __ldg(p.row_mask + row) != 0);
+          bool exact_loss = false;
           if (TAIL >= 1 && p.fo.loss_sum && live && n < 2) {
             // ||q - x||^2 = ||x||^2 - 2(x.c - 0.5||c||^2)  — the score already holds it (cosine: bias is 0, add ||c||^2).
-            // Differs from the reference's bf16 evaluation by << 1e-3 relative (DESIGN.md 4.1); flagged rows get the
-            // exact evaluation in vqb_fix_flagged.
+            // Its error is about the band W (the score's error bound, twice).  A row close to its code (a trained
+            // codebook) cancels in this difference, so unless d2 leads W by 2^14 the store warps evaluate sum((q - x)^2)
+            // from the rows themselves; randn-like rows (d2 ~ 6e4 W at config 2) never take that path.  Flagged rows get the exact
+            // evaluation in vqb_fix_flagged.
             float d2 = x2[h] - 2.f * best;
             if (p.metric == VQB_METRIC_COSINE) d2 += __ldg(p.cnorm2 + i0);
-            epi_loss += fmaxf(d2, 0.f);
+            exact_loss = !(d2 >= 0x1p14f * st.W);
+            if (!exact_loss) epi_loss += d2;
           }
-          if (p.fo.enabled) ctrl->gidx[t & 1][rit] = (live && n < 2) ? i0 : -1;   // hand the certified winners to the store warps
+          // hand the certified winners to the store warps: k, or -2 - k when the row's loss is left to them
+          if (p.fo.enabled) ctrl->gidx[t & 1][rit] = (live && n < 2) ? (exact_loss ? -2 - i0 : i0) : -1;
           if (row < p.N && !live) {
             p.idx[row] = -1;
             if (p.idx_prov) p.idx_prov[row] = -1;
@@ -555,9 +591,56 @@ static int make_map(CUtensorMap* m, const void* base, int cols, int64_t rows, in
   return r == CUDA_SUCCESS ? VQB_OK : VQB_E_DRIVER;
 }
 
+// Shared-memory layout of one launch: whether A stays resident, ring stages, seed slots.  Host only, no device needed.
+struct AssignPlan {
+  int stream_a, n_stages, n_seed, n_items, KB, smem_bytes;
+};
+
+static int assign_plan(int n_a, int D, int n_passes, AssignPlan* pl) {
+  if (D <= 0 || (n_a != 1 && n_a != 2)) return VQB_E_INVALID;
+  // Passes (bf16 operands, fp32 accumulation): A = the input rows (n_a = 1) or the bf16 hi / lo planes of an fp32 input
+  // (n_a = 2), B = the bf16 hi / lo codebook planes — (x,c_hi)+(x,c_lo) [+ (x_lo,c_hi)]: residual ~2^-17 ||x|| ||c||, carried
+  // exactly by the band.  DESIGN.md section 8.
+  if (n_passes == 0) n_passes = n_a + 1;
+  if (n_passes != n_a + 1 && !(n_passes == 1 && n_a == 1)) return VQB_E_UNSUPPORTED;
+  if (D % 8 != 0) return VQB_E_UNSUPPORTED;
+  const int KB = (D + BK - 1) / BK;
+  // A stationary in smem when it leaves room for a useful ring; else (fp32 split input with D > 256) its k-blocks are
+  // streamed through the ring next to the codebook's (re-read from L2 for every code step)
+  const int stream_a = n_a * KB > MAX_A_SUB ? 1 : 0;
+  const int a_bytes = stream_a ? 0 : n_a * KB * A_SUB_BYTES;
+  const int stage_bytes = B_SUB_BYTES + (stream_a ? A_SUB_BYTES : 0);
+  const int fixed = SMEM_CTRL_BYTES + 1024 /*align*/ + a_bytes;
+  // ring stages + seed slots (one slot per code step the ring can run ahead).  The tightest case, fp32 at D = 256, keeps
+  // its 5 stages: 15 KiB + 128 KiB of A + 5 * 16 KiB + 4 KiB of seeds = exactly 227 KiB.
+  const int n_items = KB * n_passes;
+  int stages = MAX_STAGES;
+  auto seed_slots = [&](int st) { return (st + n_items - 1) / n_items; };
+  while (stages >= 2 && fixed + stages * stage_bytes + seed_slots(stages) * SEED_BYTES > SMEM_LIMIT) --stages;
+  if (stages < 2) return VQB_E_UNSUPPORTED;
+  pl->stream_a = stream_a;
+  pl->n_stages = stages;
+  pl->n_seed = seed_slots(stages);
+  pl->n_items = n_items;
+  pl->KB = KB;
+  pl->smem_bytes = fixed + stages * stage_bytes + pl->n_seed * SEED_BYTES;
+  return VQB_OK;
+}
+
 }  // namespace vqb
 
 using namespace vqb;
+
+// The launch plan vqb_assign would use for (n_a, D, n_passes): out6 = {stream_a, n_stages, n_seed, n_items, KB, smem_bytes}.
+extern "C" int vqb_debug_assign_plan(int n_a, int D, int n_passes, int* out6) {
+  if (!out6) return VQB_E_INVALID;
+  AssignPlan pl;
+  const int rc = assign_plan(n_a, D, n_passes, &pl);
+  if (rc) return rc;
+  out6[0] = pl.stream_a; out6[1] = pl.n_stages; out6[2] = pl.n_seed;
+  out6[3] = pl.n_items; out6[4] = pl.KB; out6[5] = pl.smem_bytes;
+  return VQB_OK;
+}
 
 extern "C" int vqb_padded_codes(int K) {
   if (K <= 0) return 0;
@@ -597,24 +680,21 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
                        int32_t* hist, int hist_shift, vqb_flag_entry* flagged, int32_t* flag_count, float* dbg_best,
                        const vqb_fused_outputs* fused, int metric, const float* cnorm2, void* stream, const uint8_t* row_mask) {
   if (!a_planes || !b_planes || !bext || !cmax || !idx || !flagged || !flag_count) return VQB_E_INVALID;
-  if (N <= 0 || D <= 0 || K <= 0 || (n_a != 1 && n_a != 2)) return VQB_E_INVALID;
-  // Passes (bf16 operands, fp32 accumulation): A = the input rows (n_a = 1) or the bf16 hi / lo planes of an fp32 input
-  // (n_a = 2), B = the bf16 hi / lo codebook planes — (x,c_hi)+(x,c_lo) [+ (x_lo,c_hi)]: residual ~2^-17 ||x|| ||c||, carried
-  // exactly by the band.  DESIGN.md section 8.
+  if (N <= 0 || K <= 0) return VQB_E_INVALID;
+  AssignPlan plan;
+  int rc = assign_plan(n_a, D, n_passes, &plan);
+  if (rc) return rc;
   if (n_passes == 0) n_passes = n_a + 1;
-  if (n_passes != n_a + 1 && !(n_passes == 1 && n_a == 1)) return VQB_E_UNSUPPORTED;
-  if (D % 8 != 0) return VQB_E_UNSUPPORTED;
-  const int KB = (D + BK - 1) / BK;
   if (N > (static_cast<int64_t>(1) << 31) - BM) return VQB_E_UNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(a_planes) | reinterpret_cast<uintptr_t>(b_planes) | reinterpret_cast<uintptr_t>(bext)) & 15)
     return VQB_E_ALIGN;
-  int rc = check_device();
+  rc = check_device();
   if (rc) return rc;
 
   AssignParams p;
   p.N = N; p.D = D; p.K = K;
   p.Kpad = vqb_padded_codes(K);
-  p.n_a = n_a; p.n_passes = n_passes; p.KB = KB;
+  p.n_a = n_a; p.n_passes = n_passes; p.KB = plan.KB;
   p.num_row_tiles = static_cast<int>((N + BM - 1) / BM);
   p.num_code_steps = (p.Kpad + WN - 1) / WN;
   p.margin_rel = margin_rel;
@@ -634,23 +714,11 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   // residual-only tail of a ResidualVQ stage on the raw rows (Euclidean, or inputs that were already unit vectors)
   p.resid_mode = p.fo.enabled && p.fo.resid_out && !p.fo.q_out && !p.fo.qsum && !p.fo.stats_sum &&
                  (!p.fo.x_raw || p.fo.x_raw == p.fo.x_eff) && !(metric == VQB_METRIC_COSINE && p.fo.loss_sum && !cnorm2);
-  // A stationary in smem when it leaves room for a useful ring; else (fp32 split input with D > 256) its k-blocks are
-  // streamed through the ring next to the codebook's (re-read from L2 for every code step)
-  p.stream_a = n_a * KB > MAX_A_SUB ? 1 : 0;
+  p.stream_a = plan.stream_a;
   p.a_global = static_cast<const uint16_t*>(a_planes);
-  const int a_bytes = p.stream_a ? 0 : n_a * KB * A_SUB_BYTES;
-  const int stage_bytes = B_SUB_BYTES + (p.stream_a ? A_SUB_BYTES : 0);
-  const int fixed = SMEM_CTRL_BYTES + 1024 /*align*/ + a_bytes;
-  // ring stages + seed slots (one slot per code step the ring can run ahead).  The tightest case, fp32 at D = 256, keeps
-  // its 5 stages: 15 KiB + 128 KiB of A + 5 * 16 KiB + 4 KiB of seeds = exactly 227 KiB.
-  const int n_items = KB * n_passes;
-  int stages = MAX_STAGES;
-  auto seed_slots = [&](int st) { return (st + n_items - 1) / n_items; };
-  while (stages >= 2 && fixed + stages * stage_bytes + seed_slots(stages) * SEED_BYTES > SMEM_LIMIT) --stages;
-  if (stages < 2) return VQB_E_UNSUPPORTED;
-  p.n_stages = stages;
-  p.n_seed = seed_slots(stages);
-  const int smem_bytes = fixed + stages * stage_bytes + p.n_seed * SEED_BYTES;
+  p.n_stages = plan.n_stages;
+  p.n_seed = plan.n_seed;
+  const int smem_bytes = plan.smem_bytes;
 
   CUtensorMap tmA, tmB;
   rc = make_map(&tmA, a_planes, D, N, n_a, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);  // plane stride = N*D either way

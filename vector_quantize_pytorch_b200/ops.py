@@ -112,9 +112,10 @@ def search(x: torch.Tensor, ops: CodebookOperands, embed: torch.Tensor, *, margi
            debug_best: bool = False, fix: bool = True, normalise: bool = True, fused: dict | None = None) -> SearchResult:
     """Nearest code of every row of x (N, D).  Replaces cdist/einsum + argmax (vqp:58-62, :741-747, :130-145).
 
-    fused: optional dict(q_out=, idx64_out=, idx_stride=, loss_sum=, resid_out=, qsum=) of output tensors — the
+    fused: optional dict(q_out=, idx64_out=, idx_stride=, loss_sum=, resid_out=, qsum=, planes_out=) of output tensors — the
     gather / commitment-loss / residual tail (see `gather`) then runs INSIDE the search kernel (store warps) and
-    the re-score kernels, and no separate gather launch is needed."""
+    the re-score kernels, and no separate gather launch is needed.  planes_out (fp32 rows with resid_out): 2-byte
+    [2][N][D], the bf16 hi / lo split of the residual (the next ResidualVQ stage's A operand)."""
     _require_cuda(x, embed)
     assert x.dim() == 2 and x.is_contiguous()
     N, D = x.shape
@@ -150,7 +151,8 @@ def search(x: torch.Tensor, ops: CodebookOperands, embed: torch.Tensor, *, margi
             fo = _C.FusedOutputs(x_eff=_p(x_eff), embed=_p(embed), q_out=_p(fused.get("q_out")),
                                  idx64_out=_p(fused.get("idx64_out")), idx_stride=int(fused.get("idx_stride", 1)),
                                  loss_sum=_p(fused.get("loss_sum")), x_raw=_p(x) if x_eff is not x else None,
-                                 resid_out=_p(fused.get("resid_out")), qsum=_p(fused.get("qsum")), stats_cnt=None, stats_sum=None, dtype=dt)
+                                 resid_out=_p(fused.get("resid_out")), qsum=_p(fused.get("qsum")), stats_cnt=None, stats_sum=None, dtype=dt,
+                                 planes_out=_p(fused.get("planes_out")))
         fo_ref = ctypes.byref(fo) if fo is not None else None
         prof = PROFILE_EVENTS
         if prof is not None:
