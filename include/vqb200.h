@@ -143,6 +143,10 @@ int vqb_debug_graph_stats(long long* out4);
  * {stream_a (A k-blocks travel through the ring), ring stages, seed slots, ring items per code step, ceil(D/64), dynamic smem
  * bytes}.  Returns the code vqb_assign returns for that input (VQB_E_INVALID / VQB_E_UNSUPPORTED) when it is not supported. */
 int vqb_debug_assign_plan(int n_a, int D, int n_passes, int* out6);
+/* The counting-sort plan of the EMA statistics (vqb_ema_stats, vqb_vq_forward) for N rows and K codes on a device with `sms`
+ * SMs — host only.  out3 (host int[3]) = {G: row slabs of the CTA-local sort, 0 when the global-atomic kernels run; shift: a
+ * slab is 128 << shift rows (31 on the global path); the slab bound vqb_ema_stats_workspace sizes the histograms for}. */
+int vqb_debug_stats_plan(int64_t N, int K, int sms, int* out3);
 
 /* Exact re-score of the flagged rows with the reference's own fp32 formula and tie rule
  * (-(x2 + y2 - 2xy).clamp(1e-8).sqrt(), first maximal index; :58-62, :140).  Rewrites idx[row]. */

@@ -42,13 +42,13 @@ static int64_t sort_ctas_bound(int64_t N, int K) {
   return g < 1 ? 1 : g;
 }
 // Slabs of (128 << shift) rows — whole row tiles of the search kernel, which can therefore count its certified winners
-// per slab itself (AssignParams::hist).  At most one slab per SM (the scatter is a single wave), at least 512 rows each.
-static int sort_ctas(int64_t N, int K, int* shift) {
+// per slab itself (AssignParams::hist).  At most one slab per SM (`sms`; the scatter is a single wave), at least 512 rows each.
+static int sort_ctas(int64_t N, int K, int sms, int* shift) {
   // Few rows per code: a global cursor per code sees little contention, while the per-CTA histograms would move
   // sort_ctas * K counters three times (config 4: N/K = 4, measured 1.58 -> 1.71 ms per step with the CTA-local path).
   if (K > SORT_MAX_K || N < 32 * static_cast<int64_t>(K)) { *shift = 31; return 0; }   // -> global-atomic kernels
   const int64_t tiles = (N + 127) / 128;
-  int64_t cap = num_sms();
+  int64_t cap = sms;
   if (cap > 256) cap = 256;   // colscan_kernel: 32 warps x 8 slabs in registers
   if (cap > SORT_MAX_CELLS / K) cap = SORT_MAX_CELLS / K;
   if (cap < 1) cap = 1;
@@ -504,6 +504,18 @@ extern "C" size_t vqb_ema_stats_workspace(int64_t N, int K) {
   return carve(nullptr, nullptr, N, K);
 }
 
+// The sort plan of the statistics for (N, K) on a device with `sms` SMs: out3 = {slabs G (0: global-atomic path), shift
+// (slabs of 128 << shift rows; 31 on the global path), the device-independent slab bound the workspace is sized with}.
+extern "C" int vqb_debug_stats_plan(int64_t N, int K, int sms, int* out3) {
+  if (!out3 || N <= 0 || K <= 0 || sms <= 0) return VQB_E_INVALID;
+  if (N >= (static_cast<int64_t>(1) << 31)) return VQB_E_UNSUPPORTED;
+  int shift = 31;
+  out3[0] = sort_ctas(N, K, sms, &shift);
+  out3[1] = shift;
+  out3[2] = static_cast<int>(sort_ctas_bound(N, K));
+  return VQB_OK;
+}
+
 // ---- the statistics chain in three steps, so that vq_forward.cu can interleave it with the search and the re-score:
 //   stats_begin  (before the search)  zero the packed statistics and the histogram the search kernel counts into
 //   stats_scan   (after the search)   [histogram, unless the search made it] + slab scan + code scan + cluster sizes
@@ -533,7 +545,7 @@ int vqb::stats_begin(float* stats, int dtype, int64_t N, int D, int K, void* wor
                                   static_cast<cudaStream_t>(stats_stream ? stats_stream : stream));
   if (e != cudaSuccess) return static_cast<int>(e);
   int shift = 31;
-  const int G = sort_ctas(N, K, &shift);
+  const int G = sort_ctas(N, K, num_sms(), &shift);
   // [caller's counters (zero_before bytes) | ticket block | slab histograms, when the search kernel counts into them]
   e = cudaMemsetAsync(reinterpret_cast<uint8_t*>(ws.ticket) - zero_before, 0,
                       zero_before + 256 + ((G > 0 && prehist) ? sizeof(int32_t) * static_cast<size_t>(G) * K : 0), s);
@@ -555,7 +567,7 @@ int vqb::stats_scan(const int32_t* idx, int dtype, int64_t N, int D, int K, floa
   if (!idx) return VQB_E_INVALID;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int shift = 31;
-  const int G = sort_ctas(N, K, &shift);
+  const int G = sort_ctas(N, K, num_sms(), &shift);
   if (G > 0) {
     static bool attr_set = false;
     if (!attr_set) {  // K ints of dynamic smem: up to 64 KiB
@@ -587,7 +599,7 @@ int vqb::stats_sum(const void* x_eff, int dtype, int64_t N, int D, const int32_t
   if (!x_eff || !idx) return VQB_E_INVALID;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int shift = 31;
-  const int G = sort_ctas(N, K, &shift);
+  const int G = sort_ctas(N, K, num_sms(), &shift);
   if (G > 0) {
     scatter_cta_kernel<<<G, SORT_THREADS, static_cast<size_t>(K) * sizeof(int32_t), s>>>(idx, N, K, static_cast<int64_t>(128) << shift,
                                                                                         ws.cta_counts, ws.offsets, ws.perm);
