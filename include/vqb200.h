@@ -78,14 +78,15 @@ const char* vqb_strerror(int code);
 int vqb_padded_codes(int K);
 
 /* Derive the tensor-core operands of a codebook from its fp32 rows (embed, K x D):
- *   planes  2-byte [3][Kpad][D] : [0] bf16 hi = bf16(c), [1] bf16 lo = bf16(c - hi), [2] fp16(c), |c| clamped to 65504
- *                               (rows >= K are zero)
+ *   planes  bf16 [2][Kpad][D] : [0] hi = bf16(c), [1] lo = bf16(c - hi)  (rows >= K are zero)
  *   bext    bf16 [Kpad][16]   : -bias as three bf16 terms in columns 0..2 (rest 0); rows >= K hold -3e38.
  *                               A K=16 MMA against [1 1 1 0..] seeds the accumulator with -bias.
  *   bias    f32  [Kpad]       : euclid 0.5*||c||^2, cosine 0, rows >= K +inf (informational)
  *   cnorm2  f32  [K]          : ||c||^2 (f64-accumulated), used by the exact re-score
- *   cmax    f32  [4]          : [0] max_k ||c||, [1] max_k ||c - fp16 plane||, [2] max_k ||c - hi - lo||, [3] max_k ||lo||: the
- *                               exact residual norms that size the certification band of each pass scheme
+ *   cmax    f32  [3]          : [0] max_k ||c||, [1] max_k ||c - hi - lo||, [2] max_k ||lo||: the exact norms that size the
+ *                               certification band of the search
+ * Buffers sized for an older, larger layout (planes [3][Kpad][D], cmax [4]) still work: only the leading part is used.
+ * Supported: D % 8 == 0, D <= 1024 (VQB_E_UNSUPPORTED otherwise, as for vqb_assign).
  * Replaces nothing in the reference (it searches the fp32 rows directly, :710-712, :743); this is
  * the layout change that lets the search run on the tensor cores.  Also done by vqb_ema_apply. */
 int vqb_codebook_prepare(const float* embed, int K, int D, int metric, void* planes, void* bext, float* bias,
@@ -106,8 +107,7 @@ int vqb_input_prepare(const void* x, int dtype, int64_t N, int D, int metric, vo
  *             input (vqb_input_prepare).
  *   n_passes  n_a + 1 : the "split" scheme, bf16 hi / lo codebook planes into ONE fp32 accumulator:
  *                       (x,c_hi)+(x,c_lo) for bf16 rows, +(x_lo,c_hi) for fp32 rows;
- *             0       : automatic (= n_a + 1);
- *             1       : diagnostics only (n_a == 1): hi plane alone, band widened by max||c_lo||.
+ *             0       : automatic (= n_a + 1).
  *             Anything else returns VQB_E_UNSUPPORTED.
  *   b_planes/bext/cmax           from vqb_codebook_prepare / vqb_ema_apply
  *   margin_rel                   m, the tensor-core accumulation share of the certification band
@@ -183,7 +183,8 @@ int vqb_ema_stats(const void* x_eff, int dtype, int64_t N, int D, const int32_t*
  *   do_lerp      : cluster_size.lerp_(stats[:K], 1-decay); embed_avg.lerp_(stats[off:], 1-decay)
  *   do_normalise : embed = embed_avg / (laplace(cluster_size) * sum(cluster_size)); l2norm if cosine;
  *                  planes / bext / bias / cnorm2 / cmax are regenerated (all five required then)
- *   scratch      : f32[2] used internally */
+ *   scratch      : f32[2] used internally
+ * Supported: D % 8 == 0, D <= 1024 (VQB_E_UNSUPPORTED otherwise). */
 int vqb_ema_apply(float* cluster_size, float* embed_avg, float* embed, const float* stats, int K, int D, double decay,
                   double eps, int metric, int do_lerp, int do_normalise, void* planes, void* bext, float* bias,
                   float* cnorm2, float* cmax, float* scratch, void* stream);

@@ -49,6 +49,10 @@ def test_argument_errors_are_return_codes_not_crashes():
     assert lib.vqb_gather(None, 0, 1, 8, None, None, None, None, 1, None, None, None, None, None) == -1
     assert lib.vqb_ema_stats(None, 0, 1, 8, None, 4, None, None, 0, None) == -1
     assert lib.vqb_decode(None, 0, 1, 1, 8, None, 1, None, 0, None) == -1
+    # D > 1024 (the longest row a warp keeps in registers) is rejected before any CUDA call
+    p = 0x10000   # non-null, 16-byte aligned; never dereferenced
+    assert lib.vqb_codebook_prepare(p, 10, 1032, 0, p, p, p, p, p, None) == -2
+    assert lib.vqb_ema_apply_weighted(p, p, p, p, 10, 1032, 0.8, 1e-5, 0, 1, 1, None, p, p, p, p, p, p, None) == -2
 
 
 def test_no_cpu_fallback():

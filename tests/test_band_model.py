@@ -141,8 +141,8 @@ def test_reference_winner_is_always_a_candidate(dtype, cb_kind, row_kind, cosine
     x2 = (x.astype(np.float64) ** 2).sum(-1)
     cn = np.sqrt((e64 * e64).sum(-1))
     cmax = float(cn.max())
-    cres = float(np.sqrt(((e64 - csum) ** 2).sum(-1)).max())                    # cmax[2]
-    clo = float(np.sqrt((c_lo.astype(np.float64) ** 2).sum(-1)).max())          # cmax[3]
+    cres = float(np.sqrt(((e64 - csum) ** 2).sum(-1)).max())                    # cmax[1]
+    clo = float(np.sqrt((c_lo.astype(np.float64) ** 2).sum(-1)).max())          # cmax[2]
     caux = (float.fromhex("0x1.02p-8") * cmax + clo) if dtype == "fp32" else 0.0
     xlo_norm = np.sqrt((x_lo.astype(np.float64) ** 2).sum(-1))
     s = s + rng.choice([-1.0, 1.0], size=s.shape) * (MARGIN * np.sqrt(x2) * cmax)[:, None]   # accumulation error, full amplitude

@@ -270,27 +270,26 @@ def w32(decay, weight, K):
     return w.double()
 
 
-# D, K, cosine, code_weight, do_lerp, do_normalise, row path of ema_rows_kernel
+# D, K, cosine, code_weight, do_lerp, do_normalise, NV of ema_rows_kernel (float4 of the row per lane: 4 for D <= 512, else 8)
 APPLY_CASES = [
-    (64, 1000, False, None, True, True, "registers"),
-    (64, 37, True, "zeros", True, True, "registers"),
-    (512, 700, True, None, True, True, "registers"),
-    (512, 300, False, "zeros", True, True, "registers"),
-    (520, 333, True, "zeros", True, True, "memory"),
-    (520, 1000, False, None, False, True, "memory"),     # update_ema of the k-means init: no lerp
-    (1024, 100, True, None, False, True, "memory"),
-    (1024, 257, False, "zeros", True, True, "memory"),
-    (64, 1000, True, None, False, True, "registers"),
-    (520, 100, True, None, True, False, "lerp"),         # lerp only (track_cluster_size_and_embed_avg): embed, operands untouched
-    (256, 100, False, "zeros", True, False, "lerp"),
+    (64, 1000, False, None, True, True, 4),
+    (64, 37, True, "zeros", True, True, 4),
+    (512, 700, True, None, True, True, 4),
+    (512, 300, False, "zeros", True, True, 4),
+    (520, 333, True, "zeros", True, True, 8),
+    (520, 1000, False, None, False, True, 8),     # update_ema of the k-means init: no lerp
+    (1024, 100, True, None, False, True, 8),
+    (1024, 257, False, "zeros", True, True, 8),
+    (64, 1000, True, None, False, True, 4),
+    (520, 100, True, None, True, False, 8),       # lerp only (track_cluster_size_and_embed_avg): embed, operands untouched
+    (256, 100, False, "zeros", True, False, 4),
 ]
 
 
-@pytest.mark.parametrize("D,K,cosine,weight,do_lerp,do_normalise,path", APPLY_CASES)
-def test_ema_apply(D, K, cosine, weight, do_lerp, do_normalise, path):
+@pytest.mark.parametrize("D,K,cosine,weight,do_lerp,do_normalise,nv", APPLY_CASES)
+def test_ema_apply(D, K, cosine, weight, do_lerp, do_normalise, nv):
     from vector_quantize_pytorch_b200 import ops
-    # ema_rows_kernel keeps a row in registers for D <= 512; longer rows go through memory between the phases
-    assert path == ("lerp" if not do_normalise else "registers" if D <= 512 else "memory")
+    assert nv == (4 if D <= 512 else 8)
     Kpad = ops.padded_codes(K)
     decay, eps = 0.8, 1e-5
     gen = torch.Generator().manual_seed(D * 1009 + K)
@@ -342,9 +341,9 @@ def test_ema_apply(D, K, cosine, weight, do_lerp, do_normalise, path):
             assert torch.equal(bits(getattr(cb, f)), bits(t)), f"{f} written without do_normalise"
         return
     worst.append(assert_within(emb, e[0], e[1], "embed"))
-    assert_operands(cb, emb, cosine, f"D={D} K={K} (Kpad {Kpad}) {path}")
+    assert_operands(cb, emb, cosine, f"D={D} K={K} (Kpad {Kpad}) NV={nv}")
     assert cb.cmax[0] < cmax0[0], "the step should have shrunk the largest code norm"
-    print(f"D={D} K={K} Kpad={Kpad} {'cosine' if cosine else 'euclid'} {path}: worst error / bound "
+    print(f"D={D} K={K} Kpad={Kpad} {'cosine' if cosine else 'euclid'} NV={nv}: worst error / bound "
           + " ".join(f"{v:.3f}" for v in worst))
 
 
@@ -375,7 +374,7 @@ def check_module_codebook(book, cs0, ea0, batches, K, D, cosine, decay, ops_befo
 VQ_CASES = [
     ("bf16", 256, 1024, 262144, False),    # config 2: CTA sort, 128 slabs of 16 row tiles on 132 SMs
     ("bf16", 256, 1000, 65536, True),
-    ("fp32", 640, 500, 40000, False),      # D > 512: ema_rows_kernel's memory path
+    ("fp32", 640, 500, 40000, False),      # D > 512: ema_rows_kernel with 8 float4 per lane
 ]
 
 

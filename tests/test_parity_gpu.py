@@ -178,12 +178,10 @@ SCORE_CASES = [
 
 
 @pytest.mark.parametrize("dt,D,K,dist", SCORE_CASES)
-@pytest.mark.parametrize("scheme", ["split"])
-def test_score_error_inside_margin(dt, D, K, dist, scheme):
-    """The band that certifies a row must bound the real tensor-core error of EVERY pass scheme with room to spare:
+def test_score_error_inside_margin(dt, D, K, dist):
+    """The band that certifies a row must bound the real tensor-core error of the bf16 hi / lo passes with room to spare:
     |score_mma - score_exact| <= ||x|| * cres + ||x_lo|| * caux + margin * ||x|| * max||c|| + 2^-21 max||c||^2, by
-    Cauchy-Schwarz on the exact residual norms the operand-preparation kernel reports (ops.CodebookOperands.cmax).
-    split = bf16 hi / lo codebook planes; single = ONE pass with fp16 operands (rows converted to fp16 in shared memory)."""
+    Cauchy-Schwarz on the exact residual norms the operand-preparation kernel reports (ops.CodebookOperands.cmax)."""
     from vector_quantize_pytorch_b200 import ops
     torch.manual_seed(5)
     N = 8192 if K <= 4096 else 2048
@@ -202,11 +200,7 @@ def test_score_error_inside_margin(dt, D, K, dist, scheme):
     c = c.to(DEV).contiguous()
     cb = ops.prepare_codebook(c, False)
     n_a = 1 if dt == "bf16" else 2
-    single = scheme == "single"
-    if single and not (dt == "bf16" and D <= 256 and K >= 256):
-        pytest.skip("the single fp16 pass needs bf16 rows, D <= 256 (double-buffered A tile) and a full code tile")
-    n_passes = 1 if single else n_a + 1
-    res = ops.search(x, cb, c, debug_best=True, fix=False, n_passes=n_passes)
+    res = ops.search(x, cb, c, debug_best=True, fix=False, n_passes=n_a + 1)
     torch.cuda.synchronize()
     s = x.double() @ c.double().T - 0.5 * (c.double() ** 2).sum(-1)[None]
     got = s.gather(1, res.idx.long()[:, None])[:, 0]
@@ -214,23 +208,22 @@ def test_score_error_inside_margin(dt, D, K, dist, scheme):
     xd = x.double()
     xn = xd.norm(dim=-1)
     cmax = c.double().norm(dim=-1).max()
-    cm = cb.cmax.cpu().double()
+    cm = cb.cmax.cpu().double()   # max||c||, max||c - hi - lo||, max||lo||
     # the residual norms are what the kernel believes: they must be true upper bounds of what the operand planes leave out
     hi = cb.planes[0, :K].view(torch.bfloat16).float().double()
     lo = cb.planes[1, :K].view(torch.bfloat16).float().double()
-    assert (c.double() - cb.planes[2, :K].float().double()).norm(dim=-1).max().item() <= cm[1].item()
-    assert (c.double() - hi - lo).norm(dim=-1).max().item() <= cm[2].item()
-    assert lo.norm(dim=-1).max().item() <= cm[3].item()
+    assert (c.double() - hi - lo).norm(dim=-1).max().item() <= cm[1].item()
+    assert lo.norm(dim=-1).max().item() <= cm[2].item()
     # the kernel's per-score allowance (half of its band without the tag / sqrt terms), vq_assign.cu
     allow = ops.DEFAULT_MARGIN * xn * cmax + 2.0 ** -21 * cmax * cmax
-    allow = allow + xn * cm[1 if single else 2] + (2.0 ** -20 * cmax if single else 0.0)
+    allow = allow + xn * cm[1]
     if dt == "fp32":
         xhi = x.bfloat16().float()
         xlo = (x - xhi).bfloat16().double().norm(dim=-1)
-        allow = allow + xlo * (2.0 ** -8 * 1.01 * cmax + cm[3])
+        allow = allow + xlo * (2.0 ** -8 * 1.01 * cmax + cm[2])
     worst = (err / allow.clamp_min(1e-300)).max().item()
-    print(f"{dt} D={D} K={K} {dist} {scheme}: worst error / allowance = {worst:.3f}")
-    assert worst < 1.0, (dt, D, K, dist, scheme, worst)
+    print(f"{dt} D={D} K={K} {dist}: worst error / allowance = {worst:.3f}")
+    assert worst < 1.0, (dt, D, K, dist, worst)
 
 
 def test_flagged_rows_are_rescored_exactly():

@@ -79,6 +79,7 @@ def test_plan_rejects_what_the_search_rejects():
     assert plan(1, 60, 2)[0] == VQB_E_UNSUPPORTED      # D % 8 != 0
     assert plan(2, 64, 2)[0] == VQB_E_UNSUPPORTED      # the fp32 split needs three passes
     assert plan(1, 64, 3)[0] == VQB_E_UNSUPPORTED
+    assert plan(1, 64, 1)[0] == VQB_E_UNSUPPORTED      # one pass is not a scheme the search runs
     assert plan(1, 64, 0)[1] == plan(1, 64, 2)[1]       # 0 = automatic: n_a + 1 passes
     assert plan(2, 512, 0)[1] == plan(2, 512, 3)[1]
     from vector_quantize_pytorch_b200 import _C

@@ -63,7 +63,7 @@ struct AssignParams {
   const uint16_t* bext;       // [Kpad][16] bf16: -0.5||c||^2 as three bf16 terms (code_operands.cuh)
   int num_row_tiles, num_code_steps;
   float margin_rel;
-  const float* cmax;   // [4]
+  const float* cmax;   // [CMAX_SLOTS] (code_operands.cuh)
   int32_t* idx;
   int32_t* idx_prov;   // optional: idx with -1 for flagged rows
   int32_t* hist;       // optional [slabs][K]: histogram of the certified winners per slab of (128 << hist_shift) rows — the
@@ -316,13 +316,11 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int wg = (warp >> 2) - 1;                              // 0: rows 0..63, 1: rows 64..127
     const int q = lane & 3;                                      // column slice of the thread's rows
     const int rit0 = wg * WM + (warp & 3) * 16 + (lane >> 2);    // the thread's rows: rit0 and rit0 + 8
-    const float cmax = __ldg(p.cmax);
-    // Exact norms of what the pass scheme leaves out of the codebook operand (code_operands.cuh): ||c - hi - lo|| for the
-    // bf16 split.  fp32 inputs (x = hi + lo + res, |res| <= 2^-8 |lo| per element) add x_res . c and the omitted
-    // x_lo . c_lo:  ||x_lo|| * caux.  (A hi-only single pass, n_passes == 1, also leaves out the lo plane.)
-    const float cres = __ldg(p.cmax + 2) + (p.n_passes == 1 ? __ldg(p.cmax + 3) : 0.f);
-    const float caux = p.n_a == 2 ? 0x1.02p-8f * cmax + __ldg(p.cmax + 3) : 0.f;
-    const int last_pass_a0 = p.n_passes >= 2 ? 1 : 0;  // last pass of a k-block that reads A plane 0
+    const float cmax = __ldg(p.cmax + CMAX_NORM);
+    // Exact norms of what the passes leave out of the codebook operand (code_operands.cuh): ||c - hi - lo||.  fp32 inputs
+    // (x = hi + lo + res, |res| <= 2^-8 |lo| per element) add x_res . c and the omitted x_lo . c_lo:  ||x_lo|| * caux.
+    const float cres = __ldg(p.cmax + CMAX_RES);
+    const float caux = p.n_a == 2 ? 0x1.02p-8f * cmax + __ldg(p.cmax + CMAX_LO) : 0.f;
     const int n_items = p.KB * p.n_passes;
     const uint32_t a_row_off = wg * WM * 128;          // this warpgroup's 64 rows inside an A sub-tile (1024 B aligned)
     long long w_full = 0, w_afull = 0, w_gap = 0, gap0 = -1;   // gap: last commit of a step -> first wait of the next
@@ -394,7 +392,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           wgmma_wait<1>();
           fence_regs(acc);
           if (pend_stage >= 0) release(pend_stage, pend_sub);
-          const bool last_use = last_ct && !p.stream_a && (aplane == 1 ? ps == 2 : ps == last_pass_a0);
+          const bool last_use = last_ct && !p.stream_a && (aplane == 1 ? ps == 2 : ps == 1);  // pass 1: the last one of a k-block on A plane 0
           pend_stage = stage;
           pend_sub = last_use ? sub : -1;
           if (++stage == p.n_stages) { stage = 0; ph ^= 1; }
@@ -602,7 +600,7 @@ static int assign_plan(int n_a, int D, int n_passes, AssignPlan* pl) {
   // (n_a = 2), B = the bf16 hi / lo codebook planes — (x,c_hi)+(x,c_lo) [+ (x_lo,c_hi)]: residual ~2^-17 ||x|| ||c||, carried
   // exactly by the band.  DESIGN.md section 8.
   if (n_passes == 0) n_passes = n_a + 1;
-  if (n_passes != n_a + 1 && !(n_passes == 1 && n_a == 1)) return VQB_E_UNSUPPORTED;
+  if (n_passes != n_a + 1) return VQB_E_UNSUPPORTED;
   if (D % 8 != 0) return VQB_E_UNSUPPORTED;
   const int KB = (D + BK - 1) / BK;
   // A stationary in smem when it leaves room for a useful ring; else (fp32 split input with D > 256) its k-blocks are
@@ -723,7 +721,7 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   CUtensorMap tmA, tmB;
   rc = make_map(&tmA, a_planes, D, N, n_a, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);  // plane stride = N*D either way
   if (rc) return rc;
-  rc = make_map(&tmB, b_planes, D, p.Kpad, 3, BK, WN, CU_TENSOR_MAP_SWIZZLE_128B);   // planes: bf16 hi, bf16 lo, fp16
+  rc = make_map(&tmB, b_planes, D, p.Kpad, 2, BK, WN, CU_TENSOR_MAP_SWIZZLE_128B);   // planes: bf16 hi, bf16 lo
   if (rc) return rc;
 
   static bool attr_set = false;

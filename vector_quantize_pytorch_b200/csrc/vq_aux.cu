@@ -4,19 +4,24 @@
 #include "vqb_common.cuh"
 #include "code_operands.cuh"
 #include "gather_row.cuh"
-#include <cuda_fp16.h>
 
 namespace vqb {
 
 constexpr int ROW_THREADS = 256;  // 8 warps = 8 rows in flight per CTA
 
+template <int NV>
 __global__ void codebook_prepare_kernel(const float* __restrict__ embed, int K, int Kpad, int D, int metric,
                                         uint16_t* planes, uint16_t* bext, float* bias, float* cnorm2, float* cmax) {
   const int lane = threadIdx.x & 31;
   const int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (k >= Kpad) return;
-  write_code_operands(k < K ? embed + static_cast<int64_t>(k) * D : nullptr, k, K, Kpad, D, metric, planes, bext, bias,
-                      cnorm2, cmax, lane);
+  if (k >= K) {
+    write_padding_operands(k, Kpad, D, planes, bext, bias, lane);
+    return;
+  }
+  float4 c[NV];
+  load_code_row<NV>(embed + static_cast<int64_t>(k) * D, D, lane, c);
+  write_code_operands<NV>(c, k, Kpad, D, metric, planes, bext, bias, cnorm2, cmax, lane);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -544,15 +549,16 @@ extern "C" int vqb_codebook_prepare(const float* embed, int K, int D, int metric
                                     float* cnorm2, float* cmax, void* stream) {
   if (!embed || !planes || !bext || !bias || !cnorm2 || !cmax || K <= 0 || D <= 0) return VQB_E_INVALID;
   if (metric != VQB_METRIC_EUCLID && metric != VQB_METRIC_COSINE) return VQB_E_INVALID;
-  if (D % 8 != 0) return VQB_E_UNSUPPORTED;
+  if (D % 8 != 0 || D > CODE_ROW_MAX_D) return VQB_E_UNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(embed) | reinterpret_cast<uintptr_t>(planes)) & 15) return VQB_E_ALIGN;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaError_t e = cudaMemsetAsync(cmax, 0, 4 * sizeof(float), s);
+  cudaError_t e = cudaMemsetAsync(cmax, 0, CMAX_SLOTS * sizeof(float), s);
   if (e != cudaSuccess) return static_cast<int>(e);
   const int Kpad = vqb_padded_codes(K);
   const int wpb = ROW_THREADS / 32;
-  codebook_prepare_kernel<<<(Kpad + wpb - 1) / wpb, ROW_THREADS, 0, s>>>(embed, K, Kpad, D, metric,
-                                                                         static_cast<uint16_t*>(planes), static_cast<uint16_t*>(bext), bias, cnorm2, cmax);
+  auto kernel = D <= 4 * 128 ? codebook_prepare_kernel<4> : codebook_prepare_kernel<8>;
+  kernel<<<(Kpad + wpb - 1) / wpb, ROW_THREADS, 0, s>>>(embed, K, Kpad, D, metric, static_cast<uint16_t*>(planes),
+                                                        static_cast<uint16_t*>(bext), bias, cnorm2, cmax);
   return static_cast<int>(cudaGetLastError());
 }
 

@@ -346,10 +346,45 @@ __device__ __forceinline__ float lerp_f32(float a, float b, float w) {  // torch
   return (fabsf(w) < 0.5f) ? a + w * (b - a) : b - (b - a) * (1.f - w);
 }
 
+// Statistics sources of the apply kernels: element i (float4 at i) of the packed statistics [cluster_size | embed_sum].
+struct LocalStats {
+  const float* p;
+  __device__ __forceinline__ float load(int64_t i) const { return p[i]; }
+  __device__ __forceinline__ float4 load4(int64_t i) const { return *reinterpret_cast<const float4*>(p + i); }
+};
+// The sum over the ranks' buffers (vqp:603, :607).  Every peer load is in flight before the first add (NVLink latency ~2 us),
+// and the adds run in rank order from 0: every rank performs the identical fp32 additions, so the replicas stay bit-identical.
+struct PeerStats {
+  EmaStats s;
+  __device__ __forceinline__ float load(int64_t i) const {
+    float v[MAX_PEERS];
+#pragma unroll
+    for (int r = 0; r < MAX_PEERS; ++r)
+      if (r < s.world) v[r] = s.p[r][i];
+    float n = 0.f;
+#pragma unroll
+    for (int r = 0; r < MAX_PEERS; ++r)
+      if (r < s.world) n += v[r];
+    return n;
+  }
+  __device__ __forceinline__ float4 load4(int64_t i) const {
+    float4 v[MAX_PEERS];
+#pragma unroll
+    for (int r = 0; r < MAX_PEERS; ++r)
+      if (r < s.world) v[r] = *reinterpret_cast<const float4*>(s.p[r] + i);
+    float4 n = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int r = 0; r < MAX_PEERS; ++r)
+      if (r < s.world) { n.x += v[r].x; n.y += v[r].y; n.z += v[r].z; n.w += v[r].w; }
+    return n;
+  }
+};
+
 // single CTA: cluster_size.lerp_ (vqp:616) and its sum (vqp:577); zero cmax for the atomicMax that follows
 // n_lerp statistics slices (slice_stride floats apart) are applied one after the other — the Q stages of a ResidualVQ that
 // share one codebook (rvq:302-306: every layer lerps the same buffers in turn) in ONE launch.
-__global__ void ema_sizes_kernel(float* cluster_size, const float* stats, int K, float w, const float* __restrict__ code_weight,
+template <class Src>
+__global__ void ema_sizes_kernel(float* cluster_size, const Src src, int K, float w, const float* __restrict__ code_weight,
                                  int n_lerp, int64_t slice_stride, float* scratch, float* cmax) {
   __shared__ double part[32];
   double s = 0.0;
@@ -357,7 +392,7 @@ __global__ void ema_sizes_kernel(float* cluster_size, const float* stats, int K,
     float c = cluster_size[k];
     if (n_lerp) {  // (1 - decay) * weight, an fp32 product (vqp:86-97)
       const float wk = code_weight ? __fmul_rn(w, code_weight[k]) : w;
-      for (int j = 0; j < n_lerp; ++j) c = lerp_f32(c, stats[j * slice_stride + k], wk);
+      for (int j = 0; j < n_lerp; ++j) c = lerp_f32(c, src.load(j * slice_stride + k), wk);
       cluster_size[k] = c;
     }
     s += c;
@@ -369,116 +404,99 @@ __global__ void ema_sizes_kernel(float* cluster_size, const float* stats, int K,
     double t = 0.0;
     for (int i = 0; i < (blockDim.x >> 5); ++i) t += part[i];
     scratch[0] = static_cast<float>(t);
-    if (cmax) { cmax[0] = 0.f; cmax[1] = 0.f; cmax[2] = 0.f; cmax[3] = 0.f; }
+    if (cmax) { cmax[CMAX_NORM] = 0.f; cmax[CMAX_RES] = 0.f; cmax[CMAX_LO] = 0.f; }
   }
 }
 
-// one warp per (padded) code: embed_avg.lerp_ (vqp:617); embed = embed_avg / smoothed (vqp:576-584);
-// refresh the tensor-core operands of that row.
-__global__ void ema_rows_kernel(const float* __restrict__ cluster_size, float* embed_avg, float* embed,
-                                const float* __restrict__ stats, int64_t soff, int K, int Kpad, int D, float w,
-                                const float* __restrict__ code_weight, float eps, float keps, int metric,
-                                int n_lerp, int64_t slice_stride, int do_normalise, const float* __restrict__ scratch,
-                                uint16_t* planes, uint16_t* bext, float* bias, float* cnorm2, float* cmax) {
+// one warp per (padded) code: embed_avg.lerp_ (vqp:617); embed = embed_avg / smoothed (vqp:576-584); refresh the tensor-core
+// operands of that row.  The row stays in registers (D <= 128 NV): one round trip for the loads, and every later phase —
+// lerp, divide, l2norm, operand split — works on registers (this kernel sits on the critical path of every step).
+template <int NV, class Src>
+__global__ void ema_rows_kernel(const float* __restrict__ cluster_size, float* embed_avg, float* embed, const Src src,
+                                int64_t soff, int K, int Kpad, int D, float w, const float* __restrict__ code_weight, float eps,
+                                float keps, int metric, int n_lerp, int64_t slice_stride, int do_normalise,
+                                const float* __restrict__ scratch, uint16_t* planes, uint16_t* bext, float* bias, float* cnorm2,
+                                float* cmax) {
   const int lane = threadIdx.x & 31;
   const int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (k >= Kpad) return;
   if (k >= K) {
-    if (do_normalise) write_code_operands(nullptr, k, K, Kpad, D, metric, planes, bext, bias, cnorm2, cmax, lane);
+    if (do_normalise) write_padding_operands(k, Kpad, D, planes, bext, bias, lane);
     return;
   }
   float* avg = embed_avg + static_cast<int64_t>(k) * D;
   float* emb = embed + static_cast<int64_t>(k) * D;
-  if (D <= 512 && do_normalise) {
-    // Register-resident row (the common case): one round trip for the loads, every later phase — lerp, divide, l2norm, operand
-    // split — works on registers; the memory version below re-reads the row between the phases (4 dependent round trips of a
-    // kernel that sits on the critical path of every step).  Same arithmetic in the same order.
-    constexpr int NV = 4;
-    float4 a[NV];
-    if (code_weight) w = __fmul_rn(w, code_weight[k]);
-    const float* es = stats + soff + static_cast<int64_t>(k) * D;
+  float4 a[NV];
+  load_code_row<NV>(avg, D, lane, a);
+  if (code_weight) w = __fmul_rn(w, code_weight[k]);
+  const int64_t roff = soff + static_cast<int64_t>(k) * D;
+  for (int q = 0; q < n_lerp; ++q) {
+    float4 b[NV];
 #pragma unroll
     for (int j = 0; j < NV; ++j) {
       const int i = j * 128 + lane * 4;
-      a[j] = i < D ? *reinterpret_cast<const float4*>(avg + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+      if (i < D) b[j] = src.load4(q * slice_stride + roff + i);
     }
-    for (int q = 0; q < n_lerp; ++q) {
-      float4 b[NV];
-#pragma unroll
-      for (int j = 0; j < NV; ++j) {
-        const int i = j * 128 + lane * 4;
-        if (i < D) b[j] = *reinterpret_cast<const float4*>(es + q * slice_stride + i);
-      }
-#pragma unroll
-      for (int j = 0; j < NV; ++j) {
-        const int i = j * 128 + lane * 4;
-        if (i >= D) continue;
-        a[j].x = lerp_f32(a[j].x, b[j].x, w); a[j].y = lerp_f32(a[j].y, b[j].y, w);
-        a[j].z = lerp_f32(a[j].z, b[j].z, w); a[j].w = lerp_f32(a[j].w, b[j].w, w);
-      }
-    }
-    const float total = scratch[0];
-    const float denom = __fmul_rn(__fdiv_rn(__fadd_rn(cluster_size[k], eps), __fadd_rn(total, keps)), total);
-    double n2 = 0.0;
 #pragma unroll
     for (int j = 0; j < NV; ++j) {
       const int i = j * 128 + lane * 4;
       if (i >= D) continue;
-      if (n_lerp) *reinterpret_cast<float4*>(avg + i) = a[j];
-      a[j] = make_float4(__fdiv_rn(a[j].x, denom), __fdiv_rn(a[j].y, denom), __fdiv_rn(a[j].z, denom), __fdiv_rn(a[j].w, denom));
-      if (metric == VQB_METRIC_COSINE)
-        n2 += static_cast<double>(a[j].x) * a[j].x + static_cast<double>(a[j].y) * a[j].y + static_cast<double>(a[j].z) * a[j].z +
-              static_cast<double>(a[j].w) * a[j].w;
+      a[j].x = lerp_f32(a[j].x, b[j].x, w); a[j].y = lerp_f32(a[j].y, b[j].y, w);
+      a[j].z = lerp_f32(a[j].z, b[j].z, w); a[j].w = lerp_f32(a[j].w, b[j].w, w);
     }
-    if (metric == VQB_METRIC_COSINE) {  // l2norm(embed_normalized)     vqp:581-582, eps 1e-6 (:37-38)
-      const float nrm = fmaxf(static_cast<float>(sqrt(warp_sum(n2))), 1e-6f);
-#pragma unroll
-      for (int j = 0; j < NV; ++j)
-        a[j] = make_float4(__fdiv_rn(a[j].x, nrm), __fdiv_rn(a[j].y, nrm), __fdiv_rn(a[j].z, nrm), __fdiv_rn(a[j].w, nrm));
-    }
+  }
+  if (n_lerp) {
 #pragma unroll
     for (int j = 0; j < NV; ++j) {
       const int i = j * 128 + lane * 4;
-      if (i < D) *reinterpret_cast<float4*>(emb + i) = a[j];
-    }
-    write_code_operands_regs<NV>(a, k, K, Kpad, D, metric, planes, bext, bias, cnorm2, cmax, lane);
-    return;
-  }
-  if (n_lerp) {
-    if (code_weight) w = __fmul_rn(w, code_weight[k]);
-    const float* es = stats + soff + static_cast<int64_t>(k) * D;
-    for (int i = lane * 4; i < D; i += 128) {
-      float4 a = *reinterpret_cast<float4*>(avg + i);
-      for (int j = 0; j < n_lerp; ++j) {
-        const float4 b = *reinterpret_cast<const float4*>(es + j * slice_stride + i);
-        a.x = lerp_f32(a.x, b.x, w); a.y = lerp_f32(a.y, b.y, w); a.z = lerp_f32(a.z, b.z, w); a.w = lerp_f32(a.w, b.w, w);
-      }
-      *reinterpret_cast<float4*>(avg + i) = a;
+      if (i < D) *reinterpret_cast<float4*>(avg + i) = a[j];
     }
   }
   if (!do_normalise) return;
-  const float total = scratch[0];
   // laplace_smoothing(cluster_size, K, eps) * cluster_size.sum()      vqp:152-154, :577
+  const float total = scratch[0];
   const float denom = __fmul_rn(__fdiv_rn(__fadd_rn(cluster_size[k], eps), __fadd_rn(total, keps)), total);
   double n2 = 0.0;
-  for (int i = lane * 4; i < D; i += 128) {
-    const float4 a = *reinterpret_cast<const float4*>(avg + i);
-    float4 e = make_float4(__fdiv_rn(a.x, denom), __fdiv_rn(a.y, denom), __fdiv_rn(a.z, denom), __fdiv_rn(a.w, denom));
+#pragma unroll
+  for (int j = 0; j < NV; ++j) {
+    const int i = j * 128 + lane * 4;
+    if (i >= D) continue;
+    a[j] = make_float4(__fdiv_rn(a[j].x, denom), __fdiv_rn(a[j].y, denom), __fdiv_rn(a[j].z, denom), __fdiv_rn(a[j].w, denom));
     if (metric == VQB_METRIC_COSINE)
-      n2 += static_cast<double>(e.x) * e.x + static_cast<double>(e.y) * e.y + static_cast<double>(e.z) * e.z + static_cast<double>(e.w) * e.w;
-    *reinterpret_cast<float4*>(emb + i) = e;
+      n2 += static_cast<double>(a[j].x) * a[j].x + static_cast<double>(a[j].y) * a[j].y + static_cast<double>(a[j].z) * a[j].z +
+            static_cast<double>(a[j].w) * a[j].w;
   }
   if (metric == VQB_METRIC_COSINE) {  // l2norm(embed_normalized)     vqp:581-582, eps 1e-6 (:37-38)
     const float nrm = fmaxf(static_cast<float>(sqrt(warp_sum(n2))), 1e-6f);
-    __syncwarp();
-    for (int i = lane * 4; i < D; i += 128) {
-      float4 e = *reinterpret_cast<float4*>(emb + i);
-      e.x = __fdiv_rn(e.x, nrm); e.y = __fdiv_rn(e.y, nrm); e.z = __fdiv_rn(e.z, nrm); e.w = __fdiv_rn(e.w, nrm);
-      *reinterpret_cast<float4*>(emb + i) = e;
-    }
+#pragma unroll
+    for (int j = 0; j < NV; ++j)
+      a[j] = make_float4(__fdiv_rn(a[j].x, nrm), __fdiv_rn(a[j].y, nrm), __fdiv_rn(a[j].z, nrm), __fdiv_rn(a[j].w, nrm));
   }
-  __syncwarp();
-  write_code_operands(emb, k, K, Kpad, D, metric, planes, bext, bias, cnorm2, cmax, lane);
+#pragma unroll
+  for (int j = 0; j < NV; ++j) {
+    const int i = j * 128 + lane * 4;
+    if (i < D) *reinterpret_cast<float4*>(emb + i) = a[j];
+  }
+  write_code_operands<NV>(a, k, Kpad, D, metric, planes, bext, bias, cnorm2, cmax, lane);
+}
+
+template <class Src>
+static void ema_launch(int part, const Src& src, float* cluster_size, float* embed_avg, float* embed, int K, int D, float w,
+                       const float* code_weight, float eps, float keps, int metric, int n_lerp, int64_t slice_stride,
+                       int do_normalise, uint16_t* planes, uint16_t* bext, float* bias, float* cnorm2, float* cmax,
+                       float* scratch, cudaStream_t s) {
+  if (part & 1)
+    ema_sizes_kernel<Src><<<1, 1024, 0, s>>>(cluster_size, src, K, w, code_weight, n_lerp, slice_stride, scratch,
+                                             do_normalise ? cmax : nullptr);
+  if (part & 2) {
+    const int Kpad = vqb_padded_codes(K);
+    const int wpb = 8;
+    const int64_t soff = vqb_stats_offset(K);
+    auto rows = D <= 4 * 128 ? ema_rows_kernel<4, Src> : ema_rows_kernel<8, Src>;
+    rows<<<(Kpad + wpb - 1) / wpb, wpb * 32, 0, s>>>(cluster_size, embed_avg, embed, src, soff, K, Kpad, D, w, code_weight, eps, keps,
+                                                    metric, n_lerp, slice_stride, do_normalise, scratch, planes, bext, bias, cnorm2,
+                                                    cmax);
+  }
 }
 
 }  // namespace vqb
@@ -641,36 +659,47 @@ extern "C" int vqb_ema_apply_weighted(float* cluster_size, float* embed_avg, flo
                                       double decay, double eps, int metric, int do_lerp, int do_normalise,
                                       const float* code_weight, void* planes, void* bext, float* bias, float* cnorm2,
                                       float* cmax, float* scratch, void* stream) {
-  return ema_apply_part(3, cluster_size, embed_avg, embed, stats, K, D, decay, eps, metric, do_lerp ? 1 : 0, do_normalise, code_weight,
-                        planes, bext, bias, cnorm2, cmax, scratch, stream);
+  return ema_apply_part(3, local_stats(stats), cluster_size, embed_avg, embed, K, D, decay, eps, metric, do_lerp ? 1 : 0,
+                        do_normalise, code_weight, planes, bext, bias, cnorm2, cmax, scratch, stream);
+}
+
+extern "C" int vqb_ema_apply_peers(float* cluster_size, float* embed_avg, float* embed, const void* const* peer_stats_host,
+                                   int world, int64_t slice_offset, int K, int D, double decay, double eps, int metric,
+                                   int do_normalise, const float* code_weight, void* planes, void* bext, float* bias,
+                                   float* cnorm2, float* cmax, float* scratch, void* stream) {
+  EmaStats src;
+  const int rc = peer_stats(&src, peer_stats_host, world, slice_offset);
+  if (rc) return rc;
+  return ema_apply_part(3, src, cluster_size, embed_avg, embed, K, D, decay, eps, metric, 1, do_normalise, code_weight, planes,
+                        bext, bias, cnorm2, cmax, scratch, stream);
 }
 
 // part: 1 = the cluster sizes (needs only the counts of the statistics), 2 = the rows (needs part 1 and the row sums), 3 = both
-int vqb::ema_apply_part(int part, float* cluster_size, float* embed_avg, float* embed, const float* stats, int K, int D,
+int vqb::ema_apply_part(int part, const EmaStats& src, float* cluster_size, float* embed_avg, float* embed, int K, int D,
                         double decay, double eps, int metric, int n_lerp, int do_normalise, const float* code_weight,
                         void* planes, void* bext, float* bias, float* cnorm2, float* cmax, float* scratch, void* stream,
                         int64_t slice_stride) {
   if (!cluster_size || !embed_avg || !embed || !scratch || K <= 0 || D <= 0 || n_lerp < 0) return VQB_E_INVALID;
-  const int do_lerp = n_lerp > 0;
-  if (do_lerp && (!stats || (slice_stride & 3))) return VQB_E_INVALID;
+  if (n_lerp && (!src.p[0] || (slice_stride & 3))) return VQB_E_INVALID;
+  if (!n_lerp && src.world) return VQB_E_INVALID;
   if (do_normalise && (!planes || !bext || !bias || !cnorm2 || !cmax)) return VQB_E_INVALID;
-  if (D % 8 != 0) return VQB_E_UNSUPPORTED;
+  if (D % 8 != 0 || D > CODE_ROW_MAX_D) return VQB_E_UNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(embed_avg) | reinterpret_cast<uintptr_t>(embed) | reinterpret_cast<uintptr_t>(planes)) & 15)
     return VQB_E_ALIGN;
   const int64_t soff = vqb_stats_offset(K);
-  if (do_lerp && ((reinterpret_cast<uintptr_t>(stats) | reinterpret_cast<uintptr_t>(stats + soff)) & 15)) return VQB_E_ALIGN;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  for (int r = 0; n_lerp && r < (src.world ? src.world : 1); ++r)
+    if ((reinterpret_cast<uintptr_t>(src.p[r]) | reinterpret_cast<uintptr_t>(src.p[r] + soff)) & 15) return VQB_E_ALIGN;
   const float w = static_cast<float>(1.0 - decay);  // (1. - decay) evaluated in python float, then fp32 (vqp:97)
   const float epsf = static_cast<float>(eps);
   const float keps = static_cast<float>(static_cast<double>(K) * eps);  // n_categories * eps in python float (vqp:154)
-  if (part & 1)
-    ema_sizes_kernel<<<1, 1024, 0, s>>>(cluster_size, stats, K, w, code_weight, n_lerp, slice_stride, scratch, do_normalise ? cmax : nullptr);
-  if (part & 2) {
-    const int Kpad = vqb_padded_codes(K);
-    const int wpb = 8;
-    ema_rows_kernel<<<(Kpad + wpb - 1) / wpb, wpb * 32, 0, s>>>(cluster_size, embed_avg, embed, stats, soff, K, Kpad, D, w, code_weight, epsf, keps,
-                                                              metric, n_lerp, slice_stride, do_normalise, scratch,
-                                                              static_cast<uint16_t*>(planes), static_cast<uint16_t*>(bext), bias, cnorm2, cmax);
-  }
+  uint16_t* pl = static_cast<uint16_t*>(planes);
+  uint16_t* be = static_cast<uint16_t*>(bext);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (src.world)
+    ema_launch(part, PeerStats{src}, cluster_size, embed_avg, embed, K, D, w, code_weight, epsf, keps, metric, n_lerp, slice_stride,
+               do_normalise, pl, be, bias, cnorm2, cmax, scratch, s);
+  else
+    ema_launch(part, LocalStats{src.p[0]}, cluster_size, embed_avg, embed, K, D, w, code_weight, epsf, keps, metric, n_lerp,
+               slice_stride, do_normalise, pl, be, bias, cnorm2, cmax, scratch, s);
   return static_cast<int>(cudaGetLastError());
 }

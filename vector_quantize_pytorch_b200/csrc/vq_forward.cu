@@ -350,8 +350,8 @@ int rvq_enqueue(const void* ctx, void* stream) {
     if (op.kind == VQB_RVQ_STAGE) {
       rc = vq_forward_enqueue(&op.stage, os, ls ? op.lane : 0);
     } else if (op.kind == VQB_RVQ_EMA) {
-      rc = ema_apply_part(3, op.ema.cluster_size, op.ema.embed_avg, op.ema.embed, op.ema.stats, op.ema.K, op.ema.D, op.ema.decay,
-                          op.ema.eps, op.ema.metric, op.ema.do_lerp ? (op.ema.n_lerp > 1 ? op.ema.n_lerp : 1) : 0,
+      rc = ema_apply_part(3, local_stats(op.ema.stats), op.ema.cluster_size, op.ema.embed_avg, op.ema.embed, op.ema.K, op.ema.D,
+                          op.ema.decay, op.ema.eps, op.ema.metric, op.ema.do_lerp ? (op.ema.n_lerp > 1 ? op.ema.n_lerp : 1) : 0,
                           op.ema.do_normalise, nullptr, op.ema.planes, op.ema.bext, op.ema.bias, op.ema.cnorm2, op.ema.cmax,
                           op.ema.scratch, os, op.ema.slice_stride);
     } else if (op.kind == VQB_RVQ_ACCUMULATE) {
@@ -360,10 +360,13 @@ int rvq_enqueue(const void* ctx, void* stream) {
     } else if (op.kind == VQB_RVQ_BARRIER) {
       rc = vqb_peer_barrier(op.bar.flags, op.bar.rank, op.bar.world, op.bar.epoch, os);
     } else if (op.kind == VQB_RVQ_EMA_PEERS) {
-      rc = ema_apply_peers_part(3, op.emap.cluster_size, op.emap.embed_avg, op.emap.embed, op.emap.peer_stats, op.emap.world,
-                                op.emap.slice_offset, op.emap.K, op.emap.D, op.emap.decay, op.emap.eps, op.emap.metric,
-                                op.emap.do_normalise, nullptr, op.emap.planes, op.emap.bext, op.emap.bias, op.emap.cnorm2,
-                                op.emap.cmax, op.emap.scratch, os, op.emap.n_lerp > 1 ? op.emap.n_lerp : 1, op.emap.slice_stride);
+      EmaStats src;
+      rc = peer_stats(&src, op.emap.peer_stats, op.emap.world, op.emap.slice_offset);
+      if (rc == VQB_OK)
+        rc = ema_apply_part(3, src, op.emap.cluster_size, op.emap.embed_avg, op.emap.embed, op.emap.K, op.emap.D, op.emap.decay,
+                            op.emap.eps, op.emap.metric, op.emap.n_lerp > 1 ? op.emap.n_lerp : 1, op.emap.do_normalise, nullptr,
+                            op.emap.planes, op.emap.bext, op.emap.bias, op.emap.cnorm2, op.emap.cmax, op.emap.scratch, os,
+                            op.emap.slice_stride);
     } else {
       rc = VQB_E_INVALID;
     }
@@ -596,46 +599,40 @@ static int vq_forward_enqueue(const vqb_vq_forward_args* a, void* stream, int la
                               stream);
     if (rc) return rc;
   }
-  // ---- EMA (vqp:586-617, :576-584)
-  if (a->update && !fused_stats) {
-    if (side) {  // the re-scored rows join the statistics of the certified ones (cluster sizes are in place after the scan)
-      if (cudaStreamWaitEvent(s, side->counts, 0) != cudaSuccess) return static_cast<int>(cudaGetLastError());
-      rc = stats_add_flagged(x_eff, a->dtype, a->N, a->D, flagged, flag_count, a->idx32, a->K, a->stats, stream);
-      if (rc) return rc;
-      if (a->update == 2) {  // cluster-size half of the EMA: does not need the row sums
-        rc = ema_apply_part(1, a->cluster_size, a->embed_avg, a->embed, a->stats, a->K, a->D, a->decay, a->eps, a->metric, 1,
-                            a->do_normalise, nullptr, a->planes, a->bext, a->bias, a->cnorm2, a->cmax, a->scratch, stream);
-        if (rc) return rc;
-      } else if (a->update == 3) {
-        // multi-GPU: a first barrier as soon as this rank's COUNTS are complete — it absorbs the skew between the ranks while
-        // the segmented sums still run — and the cluster-size half of the EMA over every rank's counts
+  // ---- EMA (vqp:586-617, :576-584).  update 3 (multi-GPU): every rank sums all ranks' statistics inside its EMA kernels, after a
+  // barrier
+  EmaStats src = local_stats(a->stats);
+  if (a->update == 3) {
+    rc = peer_stats(&src, a->peer_stats, a->peer_world, a->peer_slice_offset);
+    if (rc) return rc;
+  }
+  auto ema = [&](int part) {
+    return ema_apply_part(part, src, a->cluster_size, a->embed_avg, a->embed, a->K, a->D, a->decay, a->eps, a->metric, 1,
+                          a->do_normalise, nullptr, a->planes, a->bext, a->bias, a->cnorm2, a->cmax, a->scratch, stream);
+  };
+  if (side) {  // the re-scored rows join the statistics of the certified ones (cluster sizes are in place after the scan)
+    if (cudaStreamWaitEvent(s, side->counts, 0) != cudaSuccess) return static_cast<int>(cudaGetLastError());
+    rc = stats_add_flagged(x_eff, a->dtype, a->N, a->D, flagged, flag_count, a->idx32, a->K, a->stats, stream);
+    if (rc) return rc;
+    if (a->update >= 2) {
+      // cluster-size half of the EMA: does not need the row sums.  Multi-GPU: a first barrier as soon as this rank's COUNTS are
+      // complete — it absorbs the skew between the ranks while the segmented sums still run
+      if (a->update == 3) {
         rc = vqb_peer_barrier(a->peer_flags, a->peer_rank, a->peer_world, a->peer_epoch, stream);
         if (rc) return rc;
-        rc = ema_apply_peers_part(1, a->cluster_size, a->embed_avg, a->embed, a->peer_stats, a->peer_world, a->peer_slice_offset,
-                                  a->K, a->D, a->decay, a->eps, a->metric, a->do_normalise, nullptr, a->planes, a->bext, a->bias,
-                                  a->cnorm2, a->cmax, a->scratch, stream);
-        if (rc) return rc;
       }
-      if (cudaStreamWaitEvent(s, side->join, 0) != cudaSuccess) return static_cast<int>(cudaGetLastError());
-    } else {
-      rc = vqb_ema_stats(x_eff, a->dtype, a->N, a->D, a->idx32, a->K, a->stats, ws + w.stats_ws, stats_ws_bytes, stream);
+      rc = ema(1);
       if (rc) return rc;
     }
+    if (cudaStreamWaitEvent(s, side->join, 0) != cudaSuccess) return static_cast<int>(cudaGetLastError());
+  } else if (a->update && !fused_stats) {
+    rc = vqb_ema_stats(x_eff, a->dtype, a->N, a->D, a->idx32, a->K, a->stats, ws + w.stats_ws, stats_ws_bytes, stream);
+    if (rc) return rc;
   }
-  if (a->update) {
-    if (a->update == 2) {
-      rc = ema_apply_part((side && !fused_stats) ? 2 : 3, a->cluster_size, a->embed_avg, a->embed, a->stats, a->K, a->D, a->decay,
-                          a->eps, a->metric, 1, a->do_normalise, nullptr, a->planes, a->bext, a->bias, a->cnorm2, a->cmax,
-                          a->scratch, stream);
-      if (rc) return rc;
-    } else if (a->update == 3) {  // multi-GPU: barrier, then every rank sums all ranks' statistics inside its EMA kernels
-      rc = vqb_peer_barrier(a->peer_flags, a->peer_rank, a->peer_world, a->peer_epoch, stream);
-      if (rc) return rc;
-      rc = ema_apply_peers_part((side && !fused_stats) ? 2 : 3, a->cluster_size, a->embed_avg, a->embed, a->peer_stats,
-                                a->peer_world, a->peer_slice_offset, a->K, a->D, a->decay, a->eps, a->metric, a->do_normalise,
-                                nullptr, a->planes, a->bext, a->bias, a->cnorm2, a->cmax, a->scratch, stream);
-      if (rc) return rc;
-    }
+  if (a->update < 2) return VQB_OK;
+  if (a->update == 3) {
+    rc = vqb_peer_barrier(a->peer_flags, a->peer_rank, a->peer_world, a->peer_epoch, stream);
+    if (rc) return rc;
   }
-  return VQB_OK;
+  return ema(side ? 2 : 3);
 }

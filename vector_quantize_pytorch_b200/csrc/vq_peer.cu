@@ -7,18 +7,17 @@
 // peer's address space over NVLink / NVSwitch); after one cross-GPU barrier (flag writes with system-scope
 // release / acquire) the EMA kernels of every rank read all R copies directly with peer loads and add them in rank
 // order 0..R-1 — every rank performs the identical fp32 additions, so the replicas' codebooks stay bit-identical, and
-// the whole step (search -> statistics -> barrier -> reduce + lerp + normalise + operand refresh) is ONE graph.
+// the whole step (search -> statistics -> barrier -> reduce + lerp + normalise + operand refresh) is ONE graph.  This file
+// holds the barrier and checks the peer pointers; the EMA kernels (vq_ema.cu) are the ones of the single-GPU update, with
+// the sum over the ranks as their statistics source.
 //
 // Protocol (per step, per rank): statistics kernels write my buffer[parity] -> peer_barrier -> apply kernels read every
 // peer's buffer[parity].  The buffers are double-buffered by step parity: a rank may only overwrite buffer[parity]
 // two steps later, i.e. after it has passed the NEXT step's barrier, which every peer reaches only after its reads
 // of this step have completed (stream order).
 #include "vqb_common.cuh"
-#include "code_operands.cuh"
 
 namespace vqb {
-
-constexpr int MAX_PEERS = 16;
 
 __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {
   asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
@@ -55,106 +54,6 @@ __global__ void peer_barrier_kernel(const PeerFlags flags, int rank, int world, 
   if (threadIdx.x == 0) *epoch = e;
 }
 
-__device__ __forceinline__ float lerp_f32p(float a, float b, float w) {  // torch.lerp
-  return (fabsf(w) < 0.5f) ? a + w * (b - a) : b - (b - a) * (1.f - w);
-}
-
-struct Peers {
-  const float* stats[MAX_PEERS];   // every rank's packed statistics buffer (already offset to this codebook's slice)
-  int world;
-};
-
-// single CTA: cluster_size.lerp_(sum over ranks) (vqp:603, :616) and its total (vqp:577); zero cmax
-__global__ void ema_sizes_peers_kernel(float* cluster_size, const Peers pr, int K, float w, const float* __restrict__ code_weight,
-                                       float* scratch, float* cmax, int n_lerp, int64_t slice_stride) {
-  __shared__ double part[32];
-  double s = 0.0;
-  for (int k = threadIdx.x; k < K; k += blockDim.x) {
-    const float wk = code_weight ? __fmul_rn(w, code_weight[k]) : w;
-    float c = cluster_size[k];
-    for (int j = 0; j < n_lerp; ++j) {   // the stages of a shared codebook, in order
-      float v[MAX_PEERS];
-#pragma unroll
-      for (int r = 0; r < MAX_PEERS; ++r)   // all peer loads in flight before the first add
-        if (r < pr.world) v[r] = pr.stats[r][j * slice_stride + k];
-      float n = 0.f;
-#pragma unroll
-      for (int r = 0; r < MAX_PEERS; ++r)   // rank order: identical on every rank
-        if (r < pr.world) n += v[r];
-      c = lerp_f32p(c, n, wk);
-    }
-    cluster_size[k] = c;
-    s += c;
-  }
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int i = 0; i < (blockDim.x >> 5); ++i) t += part[i];
-    scratch[0] = static_cast<float>(t);
-    if (cmax) { cmax[0] = 0.f; cmax[1] = 0.f; cmax[2] = 0.f; cmax[3] = 0.f; }
-  }
-}
-
-// one warp per (padded) code: embed_avg.lerp_(sum over ranks of embed_sum) (vqp:607, :617); embed = embed_avg / smoothed
-// (vqp:576-584); refresh the tensor-core operands of that row.
-__global__ void ema_rows_peers_kernel(const float* __restrict__ cluster_size, float* embed_avg, float* embed, const Peers pr,
-                                      int64_t soff, int K, int Kpad, int D, float w, const float* __restrict__ code_weight,
-                                      float eps, float keps, int metric, int do_normalise, const float* __restrict__ scratch,
-                                      uint16_t* planes, uint16_t* bext, float* bias, float* cnorm2, float* cmax, int n_lerp,
-                                      int64_t slice_stride) {
-  const int lane = threadIdx.x & 31;
-  const int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (k >= Kpad) return;
-  if (k >= K) {
-    if (do_normalise) write_code_operands(nullptr, k, K, Kpad, D, metric, planes, bext, bias, cnorm2, cmax, lane);
-    return;
-  }
-  float* avg = embed_avg + static_cast<int64_t>(k) * D;
-  float* emb = embed + static_cast<int64_t>(k) * D;
-  if (code_weight) w = __fmul_rn(w, code_weight[k]);
-  const int64_t roff = soff + static_cast<int64_t>(k) * D;
-  for (int i = lane * 4; i < D; i += 128) {
-    float4 a = *reinterpret_cast<float4*>(avg + i);
-    for (int j = 0; j < n_lerp; ++j) {
-      float4 v[MAX_PEERS];
-#pragma unroll
-      for (int r = 0; r < MAX_PEERS; ++r)   // all peer loads in flight before the first add (NVLink latency ~2 us)
-        if (r < pr.world) v[r] = *reinterpret_cast<const float4*>(pr.stats[r] + j * slice_stride + roff + i);
-      float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int r = 0; r < MAX_PEERS; ++r)
-        if (r < pr.world) { b.x += v[r].x; b.y += v[r].y; b.z += v[r].z; b.w += v[r].w; }
-      a.x = lerp_f32p(a.x, b.x, w); a.y = lerp_f32p(a.y, b.y, w); a.z = lerp_f32p(a.z, b.z, w); a.w = lerp_f32p(a.w, b.w, w);
-    }
-    *reinterpret_cast<float4*>(avg + i) = a;
-  }
-  if (!do_normalise) return;
-  const float total = scratch[0];
-  const float denom = __fmul_rn(__fdiv_rn(__fadd_rn(cluster_size[k], eps), __fadd_rn(total, keps)), total);
-  double n2 = 0.0;
-  __syncwarp();
-  for (int i = lane * 4; i < D; i += 128) {
-    const float4 a = *reinterpret_cast<const float4*>(avg + i);
-    float4 e = make_float4(__fdiv_rn(a.x, denom), __fdiv_rn(a.y, denom), __fdiv_rn(a.z, denom), __fdiv_rn(a.w, denom));
-    if (metric == VQB_METRIC_COSINE)
-      n2 += static_cast<double>(e.x) * e.x + static_cast<double>(e.y) * e.y + static_cast<double>(e.z) * e.z + static_cast<double>(e.w) * e.w;
-    *reinterpret_cast<float4*>(emb + i) = e;
-  }
-  if (metric == VQB_METRIC_COSINE) {
-    const float nrm = fmaxf(static_cast<float>(sqrt(warp_sum(n2))), 1e-6f);
-    __syncwarp();
-    for (int i = lane * 4; i < D; i += 128) {
-      float4 e = *reinterpret_cast<float4*>(emb + i);
-      e.x = __fdiv_rn(e.x, nrm); e.y = __fdiv_rn(e.y, nrm); e.z = __fdiv_rn(e.z, nrm); e.w = __fdiv_rn(e.w, nrm);
-      *reinterpret_cast<float4*>(emb + i) = e;
-    }
-  }
-  __syncwarp();
-  write_code_operands(emb, k, K, Kpad, D, metric, planes, bext, bias, cnorm2, cmax, lane);
-}
-
 }  // namespace vqb
 
 using namespace vqb;
@@ -168,44 +67,14 @@ extern "C" int vqb_peer_barrier(void* const* peer_flags_host, int rank, int worl
   return static_cast<int>(cudaGetLastError());
 }
 
-extern "C" int vqb_ema_apply_peers(float* cluster_size, float* embed_avg, float* embed, const void* const* peer_stats_host,
-                                   int world, int64_t slice_offset, int K, int D, double decay, double eps, int metric,
-                                   int do_normalise, const float* code_weight, void* planes, void* bext, float* bias,
-                                   float* cnorm2, float* cmax, float* scratch, void* stream) {
-  return ema_apply_peers_part(3, cluster_size, embed_avg, embed, peer_stats_host, world, slice_offset, K, D, decay, eps, metric,
-                              do_normalise, code_weight, planes, bext, bias, cnorm2, cmax, scratch, stream);
-}
-
-// part 1: cluster sizes (needs every rank's COUNTS), part 2: rows (needs part 1 and every rank's row sums), 3: both
-int vqb::ema_apply_peers_part(int part, float* cluster_size, float* embed_avg, float* embed, const void* const* peer_stats_host,
-                              int world, int64_t slice_offset, int K, int D, double decay, double eps, int metric,
-                              int do_normalise, const float* code_weight, void* planes, void* bext, float* bias, float* cnorm2,
-                              float* cmax, float* scratch, void* stream, int n_lerp, int64_t slice_stride) {
-  if (!cluster_size || !embed_avg || !embed || !scratch || !peer_stats_host || K <= 0 || D <= 0) return VQB_E_INVALID;
-  if (n_lerp < 1 || (slice_stride & 3)) return VQB_E_INVALID;
-  if (world < 1 || world > MAX_PEERS || slice_offset < 0 || (slice_offset & 3)) return VQB_E_INVALID;
-  if (do_normalise && (!planes || !bext || !bias || !cnorm2 || !cmax)) return VQB_E_INVALID;
-  if (D % 8 != 0) return VQB_E_UNSUPPORTED;
-  Peers pr;
-  pr.world = world;
-  for (int r = 0; r < MAX_PEERS; ++r) pr.stats[r] = nullptr;
+// peer_stats_host: host array of `world` device pointers to the ranks' packed statistics; slice_offset in floats
+int vqb::peer_stats(EmaStats* src, const void* const* peer_stats_host, int world, int64_t slice_offset) {
+  if (!peer_stats_host || world < 1 || world > MAX_PEERS || slice_offset < 0 || (slice_offset & 3)) return VQB_E_INVALID;
+  *src = EmaStats{};
+  src->world = world;
   for (int r = 0; r < world; ++r) {
     if (!peer_stats_host[r] || (reinterpret_cast<uintptr_t>(peer_stats_host[r]) & 15)) return VQB_E_ALIGN;
-    pr.stats[r] = static_cast<const float*>(peer_stats_host[r]) + slice_offset;
+    src->p[r] = static_cast<const float*>(peer_stats_host[r]) + slice_offset;
   }
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int64_t soff = vqb_stats_offset(K);
-  const float w = static_cast<float>(1.0 - decay);
-  const float epsf = static_cast<float>(eps);
-  const float keps = static_cast<float>(static_cast<double>(K) * eps);
-  if (part & 1)
-    ema_sizes_peers_kernel<<<1, 1024, 0, s>>>(cluster_size, pr, K, w, code_weight, scratch, do_normalise ? cmax : nullptr, n_lerp, slice_stride);
-  if (part & 2) {
-    const int Kpad = vqb_padded_codes(K);
-    const int wpb = 8;
-    ema_rows_peers_kernel<<<(Kpad + wpb - 1) / wpb, wpb * 32, 0, s>>>(
-        cluster_size, embed_avg, embed, pr, soff, K, Kpad, D, w, code_weight, epsf, keps, metric, do_normalise, scratch,
-        static_cast<uint16_t*>(planes), static_cast<uint16_t*>(bext), bias, cnorm2, cmax, n_lerp, slice_stride);
-  }
-  return static_cast<int>(cudaGetLastError());
+  return VQB_OK;
 }

@@ -10,6 +10,9 @@
 
 namespace vqb {
 
+// Slots of a codebook's cmax (f32 [3], code_operands.cuh): the exact norms that size the search's certification band.
+enum CmaxSlot { CMAX_NORM = 0 /* max ||c|| */, CMAX_RES = 1 /* max ||c - hi - lo|| */, CMAX_LO = 2 /* max ||lo|| */, CMAX_SLOTS = 3 };
+
 // MMA N-tile (codes per accumulator): 256 for real codebooks, the 16-rounded size for tiny ones.
 __host__ __device__ inline int code_tile(int K) { return K >= 256 ? 256 : ((K + 15) / 16) * 16; }
 
@@ -95,14 +98,24 @@ int stats_scan(const int32_t* idx, int dtype, int64_t N, int D, int K, float* st
                int prehist, void* stream);
 int stats_sum(const void* x_eff, int dtype, int64_t N, int D, const int32_t* idx, int K, float* stats, void* workspace,
               size_t workspace_bytes, void* stream);
-// vq_peer.cu: vqb_ema_apply_peers in two launches (part 1: cluster sizes — needs the ranks' counts —, 2: rows, 3: both)
-int ema_apply_peers_part(int part, float* cluster_size, float* embed_avg, float* embed, const void* const* peer_stats_host,
-                         int world, int64_t slice_offset, int K, int D, double decay, double eps, int metric, int do_normalise,
-                         const float* code_weight, void* planes, void* bext, float* bias, float* cnorm2, float* cmax,
-                         float* scratch, void* stream, int n_lerp = 1, int64_t slice_stride = 0);
-// vq_ema.cu: vqb_ema_apply_weighted in two launches (part 1: cluster sizes, 2: rows, 3: both)
-// n_lerp statistics slices, slice_stride floats apart, are applied in order (0: no lerp, only the normalisation)
-int ema_apply_part(int part, float* cluster_size, float* embed_avg, float* embed, const float* stats, int K, int D,
+// The statistics the EMA apply step lerps towards: one packed buffer p[0] (world == 0), or the sum of `world` ranks' packed
+// buffers p[0..world-1] read over peer memory, each already offset to this codebook's slice.
+constexpr int MAX_PEERS = 16;
+struct EmaStats {
+  const float* p[MAX_PEERS];
+  int world;
+};
+inline EmaStats local_stats(const float* stats) {
+  EmaStats s = {};
+  s.p[0] = stats;
+  return s;
+}
+// vq_peer.cu: the source of vqb_ema_apply_peers (checks the host array of peer pointers and the slice offset)
+int peer_stats(EmaStats* src, const void* const* peer_stats_host, int world, int64_t slice_offset);
+// vq_ema.cu: vqb_ema_apply_weighted / vqb_ema_apply_peers in two launches (part 1: cluster sizes — needs only the counts —,
+// 2: rows, 3: both).  n_lerp statistics slices, slice_stride floats apart, are applied in order (0: no lerp, only the
+// normalisation; local statistics only).
+int ema_apply_part(int part, const EmaStats& src, float* cluster_size, float* embed_avg, float* embed, int K, int D,
                    double decay, double eps, int metric, int n_lerp, int do_normalise, const float* code_weight,
                    void* planes, void* bext, float* bias, float* cnorm2, float* cmax, float* scratch, void* stream,
                    int64_t slice_stride = 0);

@@ -14,11 +14,11 @@ from ._C import lib, check
 
 # A row is certified by the tensor-core passes when its best score leads all others by more than the band
 #   2 * (||x|| * cres + xaux * caux + margin * ||x|| * max||c|| [+ 2^-21 max||c||^2]) + (tag slack, sqrt-collapse width):
-# Cauchy-Schwarz on the EXACT norms of what the pass scheme leaves out (csrc/code_operands.cuh, vq_assign.cu) — single fp16
-# pass: cres = max_k ||c - fp16 plane||, xaux = norm of the row's flushed elements; bf16 split: cres = max_k ||c - hi - lo||,
-# and for fp32 inputs xaux = ||x_lo|| with caux = 2^-8 max||c|| + max||c_lo|| — plus `margin` for the fp32 accumulation in the
-# tensor core alone (2^-18; its room is measured on the GPU by the test below).  tests/test_parity_gpu.py::test_score_error_inside_margin asserts the bound for every
-# scheme on randn, heavy-tailed, tiny, unit-norm and default-init data.  See DESIGN.md 4.1.
+# Cauchy-Schwarz on the EXACT norms of what the bf16 hi / lo passes leave out (csrc/code_operands.cuh, vq_assign.cu):
+# cres = max_k ||c - hi - lo||, and for fp32 inputs xaux = ||x_lo|| with caux = 2^-8 max||c|| + max||c_lo|| — plus `margin` for
+# the fp32 accumulation in the tensor core alone (2^-18; its room is measured on the GPU by the test below).
+# tests/test_parity_gpu.py::test_score_error_inside_margin asserts the bound on randn, heavy-tailed, tiny, unit-norm and
+# default-init data.  See DESIGN.md 4.1.
 DEFAULT_MARGIN = 2.0 ** -18
 
 _DT = {torch.float32: _C.DTYPE_F32, torch.bfloat16: _C.DTYPE_BF16}
@@ -62,11 +62,11 @@ def padded_codes(K: int) -> int:
 @dataclass
 class CodebookOperands:
     """Tensor-core view of one codebook (see vqb_codebook_prepare in include/vqb200.h)."""
-    planes: torch.Tensor  # 2-byte (3, Kpad, D): bf16 hi, bf16 lo (bit patterns), fp16(c) (csrc/code_operands.cuh)
+    planes: torch.Tensor  # 2-byte (2, Kpad, D): bf16 hi, bf16 lo (bit patterns) (csrc/code_operands.cuh)
     bext: torch.Tensor  # bf16 (Kpad, 16): -bias as three bf16 terms (the operand of the "bias MMA")
     bias: torch.Tensor  # f32 (Kpad,)
     cnorm2: torch.Tensor  # f32 (K,)
-    cmax: torch.Tensor  # f32 (4,): max||c||, max||c - fp16 plane||, max||c - bf16 hi - bf16 lo||, max||bf16 lo||
+    cmax: torch.Tensor  # f32 (3,): max||c||, max||c - bf16 hi - bf16 lo||, max||bf16 lo||
     scratch: torch.Tensor  # f32 (2,)
     K: int
     D: int
@@ -76,11 +76,11 @@ class CodebookOperands:
     def allocate(K: int, D: int, cosine: bool, device) -> "CodebookOperands":
         Kpad = padded_codes(K)
         return CodebookOperands(
-            planes=torch.empty((3, Kpad, D), dtype=torch.float16, device=device),
+            planes=torch.empty((2, Kpad, D), dtype=torch.float16, device=device),
             bext=torch.empty((Kpad, 16), dtype=torch.bfloat16, device=device),
             bias=torch.empty((Kpad,), dtype=torch.float32, device=device),
             cnorm2=torch.empty((K,), dtype=torch.float32, device=device),
-            cmax=torch.zeros((4,), dtype=torch.float32, device=device),
+            cmax=torch.zeros((3,), dtype=torch.float32, device=device),
             scratch=torch.zeros((2,), dtype=torch.float32, device=device),
             K=K, D=D, cosine=cosine)
 
