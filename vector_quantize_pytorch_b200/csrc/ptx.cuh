@@ -65,12 +65,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
-// 1-D bulk copy global -> shared (bytes: a multiple of 16, both addresses 16-byte aligned), completion counted on `bar`.
-__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
-               : "memory");
-}
 // Pull a 3-D box into L2 only (no shared memory, no barrier): warms the next tile's operand while this one computes.
 __device__ __forceinline__ void tma_prefetch_l2_3d(const CUtensorMap* m, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];"
@@ -88,6 +82,17 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
   d |= static_cast<uint64_t>(1) << 16;                  // [16,30) leading byte offset >> 4 (unused for SW128 K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;          // [32,46) stride byte offset >> 4
   d |= static_cast<uint64_t>(1) << 62;                  // [62,64) layout: 1 = SWIZZLE_128B
+  return d;
+}
+
+// Same for a tile of 32-byte rows with the 32-byte swizzle (a TMA box of 16 bf16 x R rows with CU_TENSOR_MAP_SWIZZLE_32B):
+// 8-row groups are 256 B apart, the tile base is 256 B aligned.  One K=16 step covers the whole row.
+__device__ __forceinline__ uint64_t wgmma_desc_sw32(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(256 >> 4) << 32;
+  d |= static_cast<uint64_t>(3) << 62;                  // 3 = SWIZZLE_32B
   return d;
 }
 
@@ -125,6 +130,32 @@ __device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t a
         "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc));
+}
+
+// D[64 x 128] = A[64 x 16] * B[128 x 16]^T with scale-d = 0 (D is overwritten, not accumulated), A from registers: the
+// thread's fragment of its rows r, r + 8 (r = 16 (t/32) + (t%32)/4) is {a01: row r, cols 2 (t%4) + 0/1 | a01: row r + 8,
+// same cols | 0 | 0}, so columns 8..15 of A are zero.  B as above, from shared memory.
+__device__ __forceinline__ void wgmma_m64n128k16_bf16_rs_set(float (&d)[64], uint32_t a01, uint64_t bdesc) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %67, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %64, %65, %65}, %66, p, 1, 1, 0;\n"
+      "}\n"
+      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]),
+        "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]),
+        "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]),
+        "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31]),
+        "=f"(d[32]), "=f"(d[33]), "=f"(d[34]), "=f"(d[35]), "=f"(d[36]), "=f"(d[37]), "=f"(d[38]), "=f"(d[39]),
+        "=f"(d[40]), "=f"(d[41]), "=f"(d[42]), "=f"(d[43]), "=f"(d[44]), "=f"(d[45]), "=f"(d[46]), "=f"(d[47]),
+        "=f"(d[48]), "=f"(d[49]), "=f"(d[50]), "=f"(d[51]), "=f"(d[52]), "=f"(d[53]), "=f"(d[54]), "=f"(d[55]),
+        "=f"(d[56]), "=f"(d[57]), "=f"(d[58]), "=f"(d[59]), "=f"(d[60]), "=f"(d[61]), "=f"(d[62]), "=f"(d[63])
+      : "r"(a01), "r"(0u), "l"(bdesc), "n"(0));
 }
 
 }  // namespace vqb

@@ -8,9 +8,9 @@
 //                                  k-block as the last code step of the previous tile releases it) and codebook tiles
 //                                  (B: 128 codes x 64 dims per ring stage) -> 128-byte-swizzled smem
 //   warps 1..3      store warps  : fused gather tail (quantized rows, int64 indices, residuals) of the tile just certified
-//   warpgroups 1, 2 consumers    : rows 0..63 / 64..127 of the tile.  Per step of 128 codes the accumulator registers are
-//                                  seeded with -0.5||c||^2 (the three bf16 terms of bext summed in fp32: the exact value),
-//                                  then wgmma m64n128k16 accumulates the split-precision passes (a0,c_hi)+(a0,c_lo)
+//   warpgroups 1, 2 consumers    : rows 0..63 / 64..127 of the tile.  Per step of 128 codes a bias MMA sets the
+//                                  accumulators to -0.5||c||^2 (the three bf16 terms of bext times [1 1 1 0 ...]: the
+//                                  exact value), then wgmma m64n128k16 accumulates the split-precision passes (a0,c_hi)+(a0,c_lo)
 //                                  [+(a1,c_hi)] on top (bf16 x bf16 -> fp32), and the certified arg-max scan
 //                                  (epilogue.cuh) reads the scores straight from the registers.  The two consumer
 //                                  warpgroups share the tensor cores: one scans while the other's MMAs run.
@@ -47,7 +47,7 @@ constexpr int NUM_STORE_WARPS = 3;      // warps 1..3 (warp 0 is the TMA produce
 constexpr int NUM_THREADS = 128 + NUM_CONSUMER_WARPS * 32;
 constexpr int SMEM_CTRL_BYTES = 14336;  // barriers + winner hand-off + merge area
 constexpr int SMEM_LIMIT = 232448;      // 227 KiB opt-in maximum per CTA
-constexpr int SEED_BYTES = WN * 32;     // one code step of bext ([128 codes][16] bf16): the accumulator seeds
+constexpr int SEED_BYTES = WN * 32;     // one code step of bext ([128 codes][16] bf16): B of the step's bias MMA
 
 struct AssignParams {
   int64_t N;
@@ -123,7 +123,8 @@ __device__ __forceinline__ float sq_diff16(const uint4& xa, const uint4& ca, boo
 // budget): 0 = none / generic (x re-read: running sum, fused statistics, cosine residual), 1 = copy mode, 2 = resid mode.
 template <int TAIL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const AssignParams p) {
+vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmS, const AssignParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   Ctrl* ctrl = reinterpret_cast<Ctrl*>(smem);
   const uint32_t smem_base = smem_u32(smem);
@@ -143,6 +144,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmS);
     for (int s = 0; s < n_sub; ++s) {
       mbar_init(smem_u32(&ctrl->a_full[s]), 1);
       mbar_init(smem_u32(&ctrl->a_empty[s]), NUM_CONSUMER_WARPS);
@@ -186,13 +188,11 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 tma_load_3d(a_base + sub * A_SUB_BYTES, &tmA, smem_u32(&ctrl->a_full[sub]), kb * BK, row0, aplane);
               }
               { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_empty[stage]), ph ^ 1); w_empty += PROF_CLOCK() - c0; }
-              // the step's seeds ride on the barrier of its first item
-              const int seed_codes = min(WN, p.Kpad - ct * WN);
-              const uint32_t seed_bytes = (kb == 0 && ps == 0) ? seed_codes * 32 : 0;
-              mbar_arrive_expect_tx(smem_u32(&ctrl->b_full[stage]), stage_stride + seed_bytes);
-              if (seed_bytes)
-                bulk_load(seed_base + (gstep % p.n_seed) * SEED_BYTES, p.bext + static_cast<int64_t>(ct) * WN * 16, seed_bytes,
-                          smem_u32(&ctrl->b_full[stage]));
+              // the step's seeds ride on the barrier of its first item (a whole box: rows past Kpad are zero-filled)
+              const bool seeds = kb == 0 && ps == 0;
+              mbar_arrive_expect_tx(smem_u32(&ctrl->b_full[stage]), stage_stride + (seeds ? SEED_BYTES : 0));
+              if (seeds)
+                tma_load_3d(seed_base + (gstep % p.n_seed) * SEED_BYTES, &tmS, smem_u32(&ctrl->b_full[stage]), 0, ct * WN, 0);
               if (p.stream_a)
                 tma_load_3d(b_base + stage * stage_stride, &tmA, smem_u32(&ctrl->b_full[stage]), kb * BK, row0, aplane);
               tma_load_3d(b_base + stage * stage_stride + a_stage_bytes, &tmB, smem_u32(&ctrl->b_full[stage]), kb * BK,
@@ -323,6 +323,8 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const float caux = p.n_a == 2 ? 0x1.02p-8f * cmax + __ldg(p.cmax + CMAX_LO) : 0.f;
     const int n_items = p.KB * p.n_passes;
     const uint32_t a_row_off = wg * WM * 128;          // this warpgroup's 64 rows inside an A sub-tile (1024 B aligned)
+    // A of the bias MMA: 1 at k = 0, 1, 2 of every row, 0 elsewhere (the thread's fragment holds columns 2q, 2q + 1)
+    const uint32_t bias_a = q == 0 ? 0x3F803F80u : (q == 1 ? 0x00003F80u : 0u);
     long long w_full = 0, w_afull = 0, w_gap = 0, gap0 = -1;   // gap: last commit of a step -> first wait of the next
     const long long cstart = PROF_CLOCK();
     float acc[64];
@@ -343,28 +345,14 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
       for (int ct = 0; ct < p.num_code_steps; ++ct) {
         const bool last_ct = ct == p.num_code_steps - 1;
-        // seed the accumulators with -0.5||c||^2 (Euclid; 0 for cosine): b1 + b2 + b3 is exact in fp32.  The producer
-        // loaded the step's bext rows into shared memory on the barrier of the step's first item.  Codes past Kpad (tiny
-        // codebooks) score -3e38: the TMA zero-fills their operand rows.
+        // The bias MMA (scale-d = 0) sets the accumulators to -0.5||c||^2 (Euclid; 0 for cosine, -3e38 for padding codes):
+        // A = [1 1 1 0 ...] times the step's bext rows, which the producer loaded into a seed slot on the barrier of the
+        // step's first item; b1 + b2 + b3 is exact in fp32.  It is committed with item 0, so the release of item 0's
+        // stage also proves that the slot has been read.
         if (gap0 >= 0) w_gap += PROF_CLOCK() - gap0;
         { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_full[stage]), ph); w_full += PROF_CLOCK() - c0; }
-        {
-          const uint2* seeds = reinterpret_cast<const uint2*>(smem + (seed_base - smem_base) + (gstep % p.n_seed) * SEED_BYTES);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-#pragma unroll
-            for (int b = 0; b < 2; ++b) {
-              const int cl = 8 * j + 2 * q + b;
-              float s = -3.0e38f;
-              if (ct * WN + cl < p.Kpad) {
-                const uint2 u = seeds[cl * 4];
-                s = (__uint_as_float(u.x << 16) + __uint_as_float(u.x & 0xFFFF0000u)) + __uint_as_float(u.y << 16);
-              }
-              acc[4 * j + b] = s;
-              acc[4 * j + 2 + b] = s;
-            }
-          }
-        }
+        wgmma_fence();
+        wgmma_m64n128k16_bf16_rs_set(acc, bias_a, wgmma_desc_sw32(seed_base + (gstep % p.n_seed) * SEED_BYTES));
         // Items of a code step in k-block-major order (kb, ps) — the order the producer stages them in.  One wgmma group
         // stays in flight: the stage of item i - 1 is released once item i has been issued.
         int kb = 0, ps = 0;
@@ -437,6 +425,13 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         fence_regs(acc);
         release(pend_stage, pend_sub);
         ++gstep;
+        if ((ct + 1) * WN > p.Kpad) {   // tiny codebooks: codes past Kpad (zero-filled seeds and operands) score -3e38
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int b = 0; b < 2; ++b)
+              if (ct * WN + 8 * j + 2 * q + b >= p.Kpad) { acc[4 * j + b] = -3.0e38f; acc[4 * j + 2 + b] = -3.0e38f; }
+        }
 
         if (ct == 0) {
           const bool euclid = p.metric != VQB_METRIC_COSINE;
@@ -449,7 +444,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             // reference formula including the sqrt.  In score units (d^2 / 2), with a 2x safety factor.
             // 2 * |score error|: what the passes leave out of the codebook (||x|| * cres) and of the row (xaux * caux), both by
             // Cauchy-Schwarz on exact norms; the fp32 accumulation in the tensor core (margin_rel relative to ||x|| max||c||,
-            // 2^-20 relative to the bias it starts from); then the tag slack and the sqrt-collapse width.
+            // 2^-20 relative to the bias the bias MMA sums); then the tag slack and the sqrt-collapse width.
             const float xn = sqrtf(x2[h]);
             const float xc = xn * cmax;
             xlo[h] = p.n_a == 2 ? sqrtf(xlo[h]) * 1.0001f : 0.f;
@@ -718,10 +713,12 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   p.n_seed = plan.n_seed;
   const int smem_bytes = plan.smem_bytes;
 
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmS;
   rc = make_map(&tmA, a_planes, D, N, n_a, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);  // plane stride = N*D either way
   if (rc) return rc;
   rc = make_map(&tmB, b_planes, D, p.Kpad, 2, BK, WN, CU_TENSOR_MAP_SWIZZLE_128B);   // planes: bf16 hi, bf16 lo
+  if (rc) return rc;
+  rc = make_map(&tmS, bext, 16, p.Kpad, 1, 16, WN, CU_TENSOR_MAP_SWIZZLE_32B);      // seeds: B of the bias MMA
   if (rc) return rc;
 
   static bool attr_set = false;
@@ -734,8 +731,8 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   }
   const int grid = p.num_row_tiles < num_sms() ? p.num_row_tiles : num_sms();
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (p.copy_mode) vq_assign_kernel<1><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, p);
-  else if (p.resid_mode) vq_assign_kernel<2><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, p);
-  else vq_assign_kernel<0><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, p);
+  if (p.copy_mode) vq_assign_kernel<1><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
+  else if (p.resid_mode) vq_assign_kernel<2><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
+  else vq_assign_kernel<0><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
   return static_cast<int>(cudaGetLastError());
 }
