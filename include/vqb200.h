@@ -273,6 +273,11 @@ int vqb_decode(const float* embeds, int64_t embed_stride, int Q, int K, int D, c
  * idx i64 [N][Q] (no -1 entries), embeds as for vqb_decode.  Replaces Q read-modify-write passes over (N x D). */
 int vqb_rvq_accumulate(const float* embeds, int64_t embed_stride, int Q, int K, int D, const int64_t* idx, int64_t N,
                        void* out, int dtype, void* stream);
+/* The slice plan vqb_decode / vqb_rvq_accumulate launch with — host only, no device needed.  nbooks codebooks (1 when
+ * embed_stride is 0, Q otherwise) of K x D, staged as esz-byte elements (2: vqb_rvq_accumulate in bf16; 4 otherwise), N rows,
+ * `sms` SMs.  out3 (host int[3]) = {W: column slice of every codebook in shared memory, 0 when the L2 kernel runs; slices =
+ * D / W; CTAs per slice}. */
+int vqb_debug_gather_sum_plan(int nbooks, int K, int D, int esz, int64_t N, int sms, int* out3);
 
 /* A whole ResidualVQ / GroupedResidualVQ forward in ONE call (residual_vq.py:469-568 the stage loop, :593-601 the
  * deferred codebook updates, :676-724 the groups): the ops are enqueued in order and replayed together from one cached

@@ -95,6 +95,7 @@ SIGNATURES = {
     "vqb_debug_stats_plan": (_i32, [_i64, _i32, _i32, _vp]),
     "vqb_decode": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _i64, _vp, _i32, _vp]),
     "vqb_rvq_accumulate": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _i64, _vp, _i32, _vp]),
+    "vqb_debug_gather_sum_plan": (_i32, [_i32, _i32, _i32, _i32, _i64, _i32, _vp]),
     "vqb_rvq_forward": (_i32, [_vp, _i32, _vp]),
 }
 

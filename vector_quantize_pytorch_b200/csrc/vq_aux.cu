@@ -478,6 +478,10 @@ rvq_accumulate_smem_kernel(const float* __restrict__ embeds, int64_t embed_strid
 //   out  = (e - 2 (e.w) w + 2 (e.u) q) * ||tgt|| / max(||src||, eps)          with e = src
 //   d_e  = (g - 2 (g.w) w + 2 (g.q) u) * ||tgt|| / max(||src||, eps)          (only `e` carries gradient)
 // Every scalar follows from five row reductions (||s||^2, ||t||^2, s.t, g.s, g.t): one sweep for them, one for the row.
+// The reductions and the scalars are taken in double: ||u + q||^2 = ||u||^2 + ||q||^2 + 2 u.q and e.(u + q) cancel when src
+// points almost opposite to tgt, and in fp32 their rounding noise (~1e-7) swamps ||u + q||^2 below ||u + q|| ~ 5e-4, where the
+// eps clamp could then scale the row by up to 1e6.  Products of fp32 values are exact in double, so the sums are exact to
+// about D * 2^-53.  nw and the dot products are those of the vectors the second sweep forms with the fp32 ins / int_.
 // ---------------------------------------------------------------------------------------------
 template <int DT, bool BWD>
 __global__ void rotate_kernel(const void* __restrict__ src, const void* __restrict__ tgt, const void* __restrict__ grad,
@@ -489,23 +493,25 @@ __global__ void rotate_kernel(const void* __restrict__ src, const void* __restri
   for (int64_t row = static_cast<int64_t>(blockIdx.x) * wpb + (threadIdx.x >> 5); row < N;
        row += static_cast<int64_t>(gridDim.x) * wpb) {
     const int64_t base = row * D;
-    float ss = 0.f, tt = 0.f, st = 0.f, gs = 0.f, gt = 0.f;
+    double ss = 0.0, tt = 0.0, st = 0.0, gs = 0.0, gt = 0.0;
     for (int i = lane; i < D; i += 32) {
-      const float s = E::load(src, base + i), t = E::load(tgt, base + i);
-      ss = fmaf(s, s, ss); tt = fmaf(t, t, tt); st = fmaf(s, t, st);
-      if (BWD) { const float g = E::load(grad, base + i); gs = fmaf(g, s, gs); gt = fmaf(g, t, gt); }
+      const double s = E::load(src, base + i), t = E::load(tgt, base + i);
+      ss = fma(s, s, ss); tt = fma(t, t, tt); st = fma(s, t, st);
+      if (BWD) { const double g = E::load(grad, base + i); gs = fma(g, s, gs); gt = fma(g, t, gt); }
     }
     ss = warp_sum(ss); tt = warp_sum(tt); st = warp_sum(st);
     if (BWD) { gs = warp_sum(gs); gt = warp_sum(gt); }
-    const float ns = sqrtf(ss), nt = sqrtf(tt);
+    const float ns = static_cast<float>(sqrt(ss)), nt = static_cast<float>(sqrt(tt));
     const float ins = 1.f / fmaxf(ns, eps), int_ = 1.f / fmaxf(nt, eps);        // safe_div (vqp:52-53)
+    const double dins = ins, dint = int_;
     // ||u + q||^2 = ||u||^2 + ||q||^2 + 2 u.q
-    const float nw = sqrtf(fmaxf(ss * ins * ins + tt * int_ * int_ + 2.f * st * ins * int_, 0.f));
-    const float inw = 1.f / fmaxf(nw, eps);                                      // l2norm eps (vqp:37-38)
+    const double nw = sqrt(fmax(ss * dins * dins + tt * dint * dint + 2.0 * st * dins * dint, 0.0));
+    const double dinw = 1.0 / fmax(nw, static_cast<double>(eps));                // l2norm eps (vqp:37-38)
+    const float inw = static_cast<float>(dinw);
     const float lam = nt * ins;
     // forward: a = e.w, b = e.u ; backward: a = g.w, b = g.q
-    const float a = BWD ? (gs * ins + gt * int_) * inw : (ss * ins + st * int_) * inw;
-    const float b = BWD ? gt * int_ : ss * ins;
+    const float a = static_cast<float>(BWD ? (gs * dins + gt * dint) * dinw : (ss * dins + st * dint) * dinw);
+    const float b = static_cast<float>(BWD ? gt * dint : ss * dins);
     for (int i = lane; i < D; i += 32) {
       const float s = E::load(src, base + i), t = E::load(tgt, base + i);
       const float u = s * ins, q = t * int_, w = (u + q) * inw;
@@ -636,17 +642,30 @@ extern "C" int vqb_loss_finalize(const double* loss_sum, int64_t numel, int dtyp
   return vqb::loss_finalize_launch(loss_sum, numel, nullptr, 1, dtype, weight, loss_out, stream);
 }
 
-// smem variant of the gather-sum (rounded running sum / decode): the widest power-of-two column slice W of all the codebooks
-// that fits (a row piece of at least 64 staged bytes); false when nothing fits and the caller uses the L2 kernel
+// Slice plan of the smem gather-sum for nbooks codebooks of K x D staged as esz-byte elements, N rows, `sms` SMs:
+// out3 = {W, slices = D / W, CTAs per slice}.  W is the widest power-of-two column slice of all the codebooks that fits in
+// 192 KiB with a row piece of 64..512 staged bytes (4..32 lanes x 16 bytes); W = 0 (the L2 kernel) when none fits or when
+// N < 4096, where staging the slices costs more than the rows it serves.
+static void gather_sum_plan(int nbooks, int K, int D, int esz, int64_t N, int sms, int* out3) {
+  int W = 0;
+  for (int w = 512 / esz; w * esz >= 64; w >>= 1)
+    if (D % w == 0 && static_cast<size_t>(nbooks) * K * w * esz <= 196608) { W = w; break; }
+  if (N < 4096) W = 0;
+  out3[0] = W;
+  out3[1] = W ? D / W : 0;
+  out3[2] = W ? max(1, sms / (D / W)) : 0;
+}
+
+// smem variant of the gather-sum (rounded running sum / decode); false when the plan picks the L2 kernel
 template <bool ROUNDED>
 static bool gather_sum_smem(const float* embeds, int64_t embed_stride, int Q, int K, int D, const int64_t* idx, int64_t N, void* out,
                             int dtype, cudaStream_t s) {
   const int esz = (ROUNDED && dtype == VQB_DTYPE_BF16) ? 2 : 4;
   const int nbooks = embed_stride ? Q : 1;
-  int W = 0;
-  for (int w = 512 / esz; w * esz >= 64; w >>= 1)   // at most 32 lanes x 16 bytes per row piece
-    if (D % w == 0 && static_cast<size_t>(nbooks) * K * w * esz <= 196608) { W = w; break; }
-  if (!W || N < 4096) return false;
+  int plan[3];
+  gather_sum_plan(nbooks, K, D, esz, N, num_sms(), plan);
+  const int W = plan[0], slices = plan[1], cps = plan[2];
+  if (!W) return false;
   const size_t smem = static_cast<size_t>(nbooks) * K * W * esz;
   static bool attr_set = false;
   if (!attr_set) {
@@ -654,9 +673,6 @@ static bool gather_sum_smem(const float* embeds, int64_t embed_stride, int Q, in
     cudaFuncSetAttribute(rvq_accumulate_smem_kernel<VQB_DTYPE_BF16, ROUNDED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 196608);
     attr_set = true;
   }
-  const int slices = D / W;
-  int cps = num_sms() / slices;
-  if (cps < 1) cps = 1;
   if (dtype == VQB_DTYPE_F32)
     rvq_accumulate_smem_kernel<VQB_DTYPE_F32, ROUNDED><<<slices * cps, 1024, smem, s>>>(embeds, embed_stride, nbooks, Q, K, D, W, idx, N, out, cps);
   else
@@ -692,6 +708,12 @@ extern "C" int vqb_rvq_accumulate(const float* embeds, int64_t embed_stride, int
   else
     rvq_accumulate_kernel<VQB_DTYPE_BF16, true><<<g, ROW_THREADS, 0, s>>>(embeds, embed_stride, Q, D, idx, N, out);
   return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int vqb_debug_gather_sum_plan(int nbooks, int K, int D, int esz, int64_t N, int sms, int* out3) {
+  if (!out3 || nbooks <= 0 || K <= 0 || D <= 0 || N <= 0 || sms <= 0 || (esz != 2 && esz != 4)) return VQB_E_INVALID;
+  gather_sum_plan(nbooks, K, D, esz, N, sms, out3);
+  return VQB_OK;
 }
 
 extern "C" int vqb_rotate(const void* src, const void* tgt, const void* grad_out, int64_t N, int D, int dtype, void* out,
