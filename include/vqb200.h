@@ -288,8 +288,10 @@ int vqb_debug_gather_sum_plan(int nbooks, int K, int D, int esz, int64_t N, int 
  *   VQB_RVQ_ACCUMULATE  vqb_rvq_accumulate(acc ...)       quantized_out from the indices (residual_vq.py:525)
  *   VQB_RVQ_BARRIER     vqb_peer_barrier(bar ...)         multi-GPU: every rank's statistics of this forward are in place
  *   VQB_RVQ_EMA_PEERS   vqb_ema_apply_peers(emap ...)     the EMA op with the sum over ranks taken inside (vqp:603, :607)
+ *   VQB_RVQ_SIMVQ_TAIL  vqb_rsimvq_tail(simvq ...)        one ResidualSimVQ stage tail, after that stage's search op
  * At most 62 ops, lanes 0..3; ops of one lane execute in list order. */
-enum { VQB_RVQ_STAGE = 0, VQB_RVQ_EMA = 1, VQB_RVQ_ACCUMULATE = 2, VQB_RVQ_BARRIER = 3, VQB_RVQ_EMA_PEERS = 4 };
+enum { VQB_RVQ_STAGE = 0, VQB_RVQ_EMA = 1, VQB_RVQ_ACCUMULATE = 2, VQB_RVQ_BARRIER = 3, VQB_RVQ_EMA_PEERS = 4,
+       VQB_RVQ_SIMVQ_TAIL = 5 };
 typedef struct vqb_rvq_op {
   int kind, lane;
   vqb_vq_forward_args stage;
@@ -308,8 +310,36 @@ typedef struct vqb_rvq_op {
     double decay, eps; int metric, do_normalise; void* planes; void* bext; float* bias; float* cnorm2; float* cmax; float* scratch;
     int n_lerp; int64_t slice_stride;  /* as in `ema` */
   } emap;
+  struct {  /* the arguments of vqb_rsimvq_tail, in its order */
+    const float* r; const float* codes; const int32_t* idx; int64_t N; int D, rotation; float* r_next; float* qsum; int first;
+    int64_t* idx64_out; int64_t idx_stride; double* loss_sum; float* loss_out; float input_weight, weight;
+  } simvq;
 } vqb_rvq_op;
 int vqb_rvq_forward(const vqb_rvq_op* ops, int n_ops, void* stream);
+
+/* ResidualSimVQ (residual_sim_vq.py of the reference: a stack of SimVQ layers, rsv:182-203 over sim_vq.py:100-138).  A stage
+ * is a search of the residual r (N x D fp32) against the stage's implicit codebook (vqb_codebook_prepare + a VQB_RVQ_STAGE op,
+ * update = 1 when the codebook needs a gradient: its statistics [count | sum of r] per code are the codebook gradient's input),
+ * then this tail, one warp per row (D <= 1024):
+ *   c = codes[idx[row]] (codes [K][D] fp32, idx i32 [N] from the search)
+ *   out = rotate_to(r, c) (rotation != 0, vector_quantize_pytorch.py:287-318) or (c - r) + r, in fp32
+ *   r_next = r - out (NULL for the last stage)  — the estimator's forward value, as rsv:195 subtracts it
+ *   qsum = 0 + out (first != 0) or qsum + out   — quantized_out, rsv:196
+ *   idx64_out[row * idx_stride] = idx (NULL to skip)
+ *   loss_out f32[1] = (mse + mse * input_weight) * weight with mse = mean((r - c)^2), sim_vq.py:121-124, :138; loss_sum f64[1]
+ *   is its scratch (NULL loss_out: no loss) */
+int vqb_rsimvq_tail(const float* r, const float* codes, const int32_t* idx, int64_t N, int D, int rotation, float* r_next,
+                    float* qsum, int first, int64_t* idx64_out, int64_t idx_stride, double* loss_sum, float* loss_out,
+                    float input_weight, float weight, void* stream);
+/* Backward of a whole ResidualSimVQ forward, one warp per row.  The residuals r_0 = x, r_1, ... are recomputed with the tail's
+ * own arithmetic (bit-identical to the forward's), so no residual is kept between forward and backward:
+ *   grad_x = sum_{q < n_active} [ rotate_to backward of grad_q at (r_q, c_q) (or grad_q itself without the rotation trick)
+ *                                 + grad_loss[q] * (r_q - c_q) ]
+ *   codes [Q][K][D] fp32 (the codebooks the stages searched), idx i64 [N][Q], grad_q [N][D] or NULL (zero), grad_loss f32 [Q]
+ *   or NULL (zero): dL/dloss_q already multiplied by 2 * weight * input_weight / (N * D).  Stages >= n_active were dropped.
+ * The codebook gradient 2 weight dL/dloss_q / (N D) * (count * c - sum of r) comes from the stage statistics (caller). */
+int vqb_rsimvq_backward(const float* x, const float* codes, int Q, int K, const int64_t* idx, int64_t N, int D, int n_active,
+                        int rotation, const float* grad_q, const float* grad_loss, float* grad_x, void* stream);
 
 /* Rotation-trick gradient estimator (vector_quantize_pytorch.py:287-318, default when x.requires_grad, :856, :1225-1228).
  *   grad_out == NULL: forward   out = rotate_to(src, tgt)        (numerically ~ tgt, carries d out / d src)

@@ -57,13 +57,19 @@ class RvqEmaPeersArgs(ctypes.Structure):
                 ("scratch", _vp), ("n_lerp", _i32), ("slice_stride", _i64)]
 
 
+class RvqSimvqArgs(ctypes.Structure):
+    _fields_ = [("r", _vp), ("codes", _vp), ("idx", _vp), ("N", _i64), ("D", _i32), ("rotation", _i32), ("r_next", _vp),
+                ("qsum", _vp), ("first", _i32), ("idx64_out", _vp), ("idx_stride", _i64), ("loss_sum", _vp), ("loss_out", _vp),
+                ("input_weight", _f32), ("weight", _f32)]
+
+
 class RvqOp(ctypes.Structure):
     """Mirror of `vqb_rvq_op` (include/vqb200.h)."""
     _fields_ = [("kind", _i32), ("lane", _i32), ("stage", VQForwardArgs), ("ema", RvqEmaArgs), ("acc", RvqAccArgs),
-                ("bar", RvqBarArgs), ("emap", RvqEmaPeersArgs)]
+                ("bar", RvqBarArgs), ("emap", RvqEmaPeersArgs), ("simvq", RvqSimvqArgs)]
 
 
-RVQ_STAGE, RVQ_EMA, RVQ_ACCUMULATE, RVQ_BARRIER, RVQ_EMA_PEERS = 0, 1, 2, 3, 4
+RVQ_STAGE, RVQ_EMA, RVQ_ACCUMULATE, RVQ_BARRIER, RVQ_EMA_PEERS, RVQ_SIMVQ_TAIL = 0, 1, 2, 3, 4, 5
 
 SIGNATURES = {
     "vqb_version": (_i32, []),
@@ -97,6 +103,8 @@ SIGNATURES = {
     "vqb_rvq_accumulate": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _i64, _vp, _i32, _vp]),
     "vqb_debug_gather_sum_plan": (_i32, [_i32, _i32, _i32, _i32, _i64, _i32, _vp]),
     "vqb_rvq_forward": (_i32, [_vp, _i32, _vp]),
+    "vqb_rsimvq_tail": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _i32, _vp, _i64, _vp, _vp, _f32, _f32, _vp]),
+    "vqb_rsimvq_backward": (_i32, [_vp, _vp, _i32, _i32, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
 }
 
 

@@ -367,6 +367,10 @@ int rvq_enqueue(const void* ctx, void* stream) {
                             op.emap.eps, op.emap.metric, op.emap.n_lerp > 1 ? op.emap.n_lerp : 1, op.emap.do_normalise, nullptr,
                             op.emap.planes, op.emap.bext, op.emap.bias, op.emap.cnorm2, op.emap.cmax, op.emap.scratch, os,
                             op.emap.slice_stride);
+    } else if (op.kind == VQB_RVQ_SIMVQ_TAIL) {
+      const auto& t = op.simvq;
+      rc = vqb_rsimvq_tail(t.r, t.codes, t.idx, t.N, t.D, t.rotation, t.r_next, t.qsum, t.first, t.idx64_out, t.idx_stride,
+                           t.loss_sum, t.loss_out, t.input_weight, t.weight, os);
     } else {
       rc = VQB_E_INVALID;
     }
@@ -447,6 +451,15 @@ extern "C" int vqb_rvq_forward(const vqb_rvq_op* ops, int n_ops, void* stream) {
       p1[0] = reinterpret_cast<uint64_t>(op.acc.embeds); p1[1] = reinterpret_cast<uint64_t>(op.acc.idx);
       p1[2] = reinterpret_cast<uint64_t>(op.acc.out);
       s1[0] = op.acc.embed_stride; s1[1] = op.acc.Q; s1[2] = op.acc.K; s1[3] = op.acc.D; s1[4] = op.acc.N; s1[5] = op.acc.dtype;
+    } else if (op.kind == VQB_RVQ_SIMVQ_TAIL) {
+      const auto& t = op.simvq;
+      const void* ptrs[] = {t.r, t.codes, t.idx, t.r_next, t.qsum, t.idx64_out, t.loss_sum, t.loss_out};
+      for (int j = 0; j < 8; ++j) p1[j] = reinterpret_cast<uint64_t>(ptrs[j]);
+      s1[0] = static_cast<uint64_t>(t.N); s1[1] = t.D; s1[2] = t.rotation; s1[3] = t.first; s1[4] = static_cast<uint64_t>(t.idx_stride);
+      s1[5] = t.loss_out != nullptr;   // the loss adds a memset and a kernel
+      uint32_t wb[2];
+      memcpy(&wb[0], &t.input_weight, 4); memcpy(&wb[1], &t.weight, 4);
+      s1[6] = wb[0]; s1[7] = wb[1];
     } else {
       return VQB_E_INVALID;
     }

@@ -186,6 +186,12 @@ def _workspace(key, nbytes: int, device) -> torch.Tensor:
     return buf
 
 
+def take_workspaces(ws_key, device) -> list:
+    """Remove the scratch buffers `vq_forward_args` made for `ws_key` on `device` from the shared cache and return them: the
+    caller (a cached program that points into them) owns them from now on, and they are freed together with it."""
+    return [b for b in (_WS_CACHE.pop((kind, ws_key, device.index), None) for kind in ("idx32", "fwd")) if b is not None]
+
+
 def vq_forward_args(x: torch.Tensor, ops: CodebookOperands, state: tuple, *, update: int, do_normalise: bool, decay: float,
                     eps: float, q_out=None, idx64_out=None, idx_stride: int = 1, loss_out=None, loss_weight: float = 1.0,
                     resid_out=None, qsum=None, stats=None, margin: float | None = None, already_normalised: bool = False,
@@ -317,6 +323,19 @@ class RvqProgram:
         self.ops.append(op)
         self.keep.append((embeds, indices, out))
         self.launches += 1
+
+    def simvq_tail(self, lane, r, codes, idx32, *, rotation, r_next, qsum, first, idx64_out, idx_stride, loss_sum, loss_out,
+                   input_weight, weight):
+        """One ResidualSimVQ stage tail (vqb_rsimvq_tail) after that stage's `stage` op: r (N, D) fp32, codes (K, D) fp32."""
+        N, D = r.shape
+        op = _C.RvqOp(kind=_C.RVQ_SIMVQ_TAIL, lane=lane)
+        op.simvq = _C.RvqSimvqArgs(r=_p(r), codes=_p(codes), idx=_p(idx32), N=N, D=D, rotation=int(rotation), r_next=_p(r_next),
+                                   qsum=_p(qsum), first=int(first), idx64_out=_p(idx64_out), idx_stride=int(idx_stride),
+                                   loss_sum=_p(loss_sum), loss_out=_p(loss_out), input_weight=float(input_weight),
+                                   weight=float(weight))
+        self.ops.append(op)
+        self.keep.append((r, codes, idx32, r_next, qsum, idx64_out, loss_sum, loss_out))
+        self.launches += 3 if loss_out is not None else 1
 
     def freeze(self):
         """Materialise the op array once; afterwards only `arr` is patched (cached programs: residual_vq.py)."""
@@ -456,6 +475,25 @@ def ema_apply_peers(cluster_size: torch.Tensor, embed_avg: torch.Tensor, embed: 
                                       _p(code_weight), _p(ops.planes), _p(ops.bext), _p(ops.bias), _p(ops.cnorm2), _p(ops.cmax),
                                       _p(ops.scratch), _stream()), "vqb_ema_apply_peers")
     _count(2)
+
+
+def rsimvq_backward(x: torch.Tensor, codes: torch.Tensor, indices: torch.Tensor, rotation: bool, grad_q: torch.Tensor | None,
+                    grad_loss: torch.Tensor | None) -> torch.Tensor:
+    """d loss / d x of a whole ResidualSimVQ forward (vqb_rsimvq_backward).  x (N, D) fp32; codes (n_active, K, D) fp32, the
+    codebooks of the stages that ran; indices (N, Q) int64; grad_loss (n_active,) fp32 already scaled by
+    2 * weight * input_weight / (N * D)."""
+    _require_cuda(x, codes, indices, grad_q, grad_loss)
+    N, D = x.shape
+    n_active, K, _ = codes.shape
+    Q = indices.shape[1]
+    for t in (x, codes, indices, grad_q, grad_loss):
+        assert t is None or t.is_contiguous()
+    gx = torch.empty_like(x)
+    with torch.cuda.device(x.device):
+        check(lib.vqb_rsimvq_backward(_p(x), _p(codes), Q, K, _p(indices), N, D, n_active, int(rotation), _p(grad_q),
+                                      _p(grad_loss), _p(gx), _stream()), "vqb_rsimvq_backward")
+    _count(1)
+    return gx
 
 
 def rotate(src: torch.Tensor, tgt: torch.Tensor, grad_out: torch.Tensor | None = None) -> torch.Tensor:
