@@ -64,8 +64,8 @@ typedef struct vqb_fused_outputs {
   const void* x_raw;   /* NULL = x_eff                                                         */
   void* resid_out;     /* [N][D] dtype = x_raw - q or NULL                                     */
   void* qsum;          /* [N][D] dtype += q or NULL                                            */
-  float* stats_cnt;    /* [K] cluster_size += 1 per row, or NULL (caller zeroes)                 */
-  float* stats_sum;    /* [K][D] embed_sum += x_eff row (vector RED), or NULL (caller zeroes)    */
+  float* stats_cnt;    /* reserved, must be NULL (VQB_E_UNSUPPORTED otherwise): statistics come */
+  float* stats_sum;    /* from vqb_ema_stats, the tail accumulates none                          */
   int dtype;           /* VQB_DTYPE_*                                                          */
   void* planes_out;    /* optional, fp32 rows with resid_out: the bf16 hi / lo split of the residual, [2][N][D] — the MMA
                           operand of the NEXT ResidualVQ stage, which then skips vqb_input_prepare (NULL to skip)          */
@@ -125,7 +125,7 @@ int vqb_assign(const void* a_planes, int n_a, int64_t N, int D, const void* b_pl
                int32_t* flag_count, float* dbg_best, const vqb_fused_outputs* fused /* NULL: search only */, void* stream);
 
 /* vqb_assign + the metric / ||c||^2 (cnorm2 [K]) that the in-kernel commitment loss of the COSINE metric needs.
- * When the fused tail asks for neither residual, running sum nor fused statistics, the tail degenerates to a row copy
+ * When the fused tail asks for neither residual nor running sum, the tail degenerates to a row copy
  * q <- codebook row (bf16 inputs: the bf16 hi plane) and the loss is read off the winning score. */
 int vqb_assign_ex(const void* a_planes, int n_a, int64_t N, int D, const void* b_planes, const void* bext,
                   const float* cmax, int K, float margin_rel, int n_passes, int32_t* idx, vqb_flag_entry* flagged,
@@ -235,9 +235,8 @@ typedef struct vqb_vq_forward_args {
   int32_t* idx32;           /* [N] int32 indices (always written; input of the statistics)                     */
   int update;               /* 0: none; 1: statistics only (caller all-reduces, then vqb_ema_apply); 2: + apply;
                                3: + peer barrier + apply over every rank's statistics (see peer_* below)             */
-  int stats_mode;           /* 0: statistics accumulated by the search kernel's store warps (vector RED into L2);
-                               1: separate counting-sort + segmented-sum kernels (vqb_ema_stats)                 */
-  int stats_accumulate;     /* stats_mode 0: do not zero `stats` first (chunked batches sum their statistics)   */
+  int stats_mode;           /* ignored: the statistics always come from the counting sort (vqb_ema_stats)         */
+  int stats_accumulate;     /* must be 0 when update != 0 (VQB_E_UNSUPPORTED otherwise): `stats` is overwritten    */
   int do_normalise;         /* update == 2: also embed = embed_avg / smoothed cluster_size                      */
   double decay, eps;
   float* stats;             /* [vqb_stats_floats(K, D)] (update != 0)                                          */
@@ -255,7 +254,7 @@ typedef struct vqb_vq_forward_args {
    * searched (the tiles stay dense) but gets index -1 in idx32, its q_out / idx64_out are NOT written (the caller pre-fills them:
    * zeros or the input, and -1, :1378-1396), it adds nothing to the loss (:1317-1325) or to the statistics (:599-600) and is
    * never re-scored.  n_live i64 [1] (device): the number of unmasked rows, the divisor of the loss (NULL: N).  VectorQuantize
-   * chain only (resid_out / qsum / planes_out must be NULL, stats_mode 1).  NULL = no mask. */
+   * chain only (resid_out / qsum / planes_out must be NULL).  NULL = no mask. */
   const uint8_t* row_mask; const int64_t* n_live;
 } vqb_vq_forward_args;
 size_t vqb_vq_forward_workspace(int64_t N, int D, int K, int dtype, int metric, int update);

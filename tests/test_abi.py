@@ -55,6 +55,35 @@ def test_argument_errors_are_return_codes_not_crashes():
     assert lib.vqb_ema_apply_weighted(p, p, p, p, 10, 1032, 0.8, 1e-5, 0, 1, 1, None, p, p, p, p, p, p, None) == -2
 
 
+def test_struct_layout_is_pinned():
+    """The ctypes mirrors have the layout of include/vqb200.h (the library static_asserts the same sizes); fields that no
+    longer select anything keep their place."""
+    from vector_quantize_pytorch_b200 import _C
+    assert ctypes.sizeof(_C.VQForwardArgs) == 328
+    assert ctypes.sizeof(_C.FusedOutputs) == 104
+    assert ctypes.sizeof(_C.RvqOp) == 808
+    offsets = {(_C.VQForwardArgs, "stats_mode"): 180, (_C.VQForwardArgs, "stats_accumulate"): 184,
+               (_C.VQForwardArgs, "row_mask"): 312, (_C.VQForwardArgs, "n_live"): 320,
+               (_C.FusedOutputs, "stats_cnt"): 72, (_C.FusedOutputs, "stats_sum"): 80, (_C.FusedOutputs, "planes_out"): 96}
+    for (cls, field), off in offsets.items():
+        assert getattr(cls, field).offset == off, (cls.__name__, field)
+
+
+def test_retired_statistics_options_are_rejected():
+    """Statistics always come from the counting sort: a call that asks the search tail to accumulate them, or asks
+    vqb_vq_forward to add onto `stats`, is refused before any CUDA call instead of being ignored."""
+    from vector_quantize_pytorch_b200 import _C
+    lib = _C.lib
+    p = 0x10000   # non-null, 16-byte aligned; never dereferenced
+    a = _C.VQForwardArgs(x=p, dtype=_C.DTYPE_BF16, N=1024, D=64, K=64, cluster_size=p, embed_avg=p, embed=p, planes=p,
+                         bext=p, bias=p, cnorm2=p, cmax=p, scratch=p, idx32=p, update=1, stats_mode=1,
+                         stats_accumulate=1, stats=p, workspace=p, workspace_bytes=1 << 30)
+    assert lib.vqb_vq_forward(ctypes.byref(a), None) == -2
+    for field in ("stats_cnt", "stats_sum"):
+        f = _C.FusedOutputs(x_eff=p, embed=p, q_out=p, dtype=_C.DTYPE_BF16, **{field: p})
+        assert lib.vqb_assign(p, 1, 1024, 64, p, p, p, 64, 0.0, 0, p, p, p, None, ctypes.byref(f), None) == -2
+
+
 def test_no_cpu_fallback():
     import vector_quantize_pytorch_b200 as m
     vq = m.VectorQuantize(dim=64, codebook_size=32)

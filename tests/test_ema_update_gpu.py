@@ -1,9 +1,8 @@
 """The EMA codebook update against float64 on every path it takes (run on an H100: `pytest -m gpu`).
 
 (a) Batch statistics.  The production chain (search kernel's slab histogram + provisional indices, sort on the side stream,
-    exact re-score rows added by stats_add_flagged), the fused mode (VQB_STATS_MODE=0: vector REDs from the store warps) and
-    the stand-alone chain (ops.ema_stats: hist_kernel with shared or global atomics) against float64 sums over the kernel's
-    own final indices.  Counts are exact; each embed_sum element is within (L + 2) * 2^-24 * sum|x| of the float64 sum, where
+    exact re-score rows added by stats_add_flagged) and the stand-alone chain (ops.ema_stats: hist_kernel with shared or
+    global atomics) against float64 sums over the kernel's own final indices.  Counts are exact; each embed_sum element is within (L + 2) * 2^-24 * sum|x| of the float64 sum, where
     L is the longest chain of fp32 additions the kernels give that element.
 (b) ops.ema_apply from a given statistics buffer against float64 evaluations of the same formulas, with an error bound that
     follows every fp32 rounding; the refreshed tensor-core operands bit for bit against vqb_codebook_prepare of the new
@@ -146,7 +145,7 @@ def stats_case(dt, D, K, N, cosine, skew, gen):
 
 
 @pytest.mark.parametrize("name,dt,D,K,N,cosine,skew,path", STATS_CASES, ids=[c[0] for c in STATS_CASES])
-def test_ema_statistics(monkeypatch, name, dt, D, K, N, cosine, skew, path):
+def test_counting_sort_statistics(name, dt, D, K, N, cosine, skew, path):
     from vector_quantize_pytorch_b200 import ops
     s = sms()
     if N == "cap":
@@ -190,14 +189,11 @@ def test_ema_statistics(monkeypatch, name, dt, D, K, N, cosine, skew, path):
     zero = torch.zeros_like(cnt)
     state = (torch.ones(K, device=DEV), c.clone(), c)
     worst = {}
-    for mode in (1, 0):
-        monkeypatch.setattr(ops, "STATS_MODE", mode)
-        idx32, st = ops.vq_forward(x, cb, state, update=1, do_normalise=False, decay=0.8, eps=1e-5, ws_key=("ema_stats", name))
-        torch.cuda.synchronize()
-        assert torch.equal(idx32.long(), idx), f"mode {mode}: indices differ from the search"
-        # sort: segment chains + one atomicAdd per work item and per re-scored row; fused: one RED per row
-        L = chain_sorted(cnt, n_flag, NY) if mode == 1 else cnt
-        worst[f"forward mode {mode}"] = check_stats(st, xe, idx, K, L, f"{name} vq_forward stats mode {mode}")
+    idx32, st = ops.vq_forward(x, cb, state, update=1, do_normalise=False, decay=0.8, eps=1e-5, ws_key=("ema_stats", name))
+    torch.cuda.synchronize()
+    assert torch.equal(idx32.long(), idx), "vq_forward: indices differ from the search"
+    # segment chains + one atomicAdd per work item and per re-scored row
+    worst["vq_forward"] = check_stats(st, xe, idx, K, chain_sorted(cnt, n_flag, NY), f"{name} vq_forward stats")
     st = ops.ema_stats(xe, res.idx, K)
     torch.cuda.synchronize()
     worst["ema_stats"] = check_stats(st, xe, idx, K, chain_sorted(cnt, zero, NY), f"{name} ema_stats")

@@ -335,7 +335,7 @@ class Codebook(nn.Module):
     @torch.no_grad()
     def quantize_rows(self, x: torch.Tensor, *, update: bool, q_out=None, idx64_out=None, idx_stride=1, loss_out=None,
                       loss_weight=1.0, resid_out=None, qsum=None, stats_out=None, defer_ema=False, margin=None,
-                      stats_accumulate=False, ema_update=None, ema_update_weight=None, accum_ema_update=False,
+                      ema_update=None, ema_update_weight=None, accum_ema_update=False,
                       row_mask=None, n_live=None):
         """x (N, D) contiguous fp32/bf16 — the input BEFORE the cosine l2norm (done in-kernel).
 
@@ -364,7 +364,7 @@ class Codebook(nn.Module):
         idx32, stats = ops.vq_forward(
             x, cb, self._state2d(), update=mode, do_normalise=normalise, decay=self.decay, eps=self.eps, q_out=q_out,
             idx64_out=idx64_out, idx_stride=idx_stride, loss_out=loss_out, loss_weight=loss_weight, resid_out=resid_out,
-            qsum=qsum, stats=stats_out, margin=margin, ws_key=id(self), stats_accumulate=stats_accumulate,
+            qsum=qsum, stats=stats_out, margin=margin, ws_key=id(self),
             peer=peer, peer_ptrs=peer_ptrs, row_mask=row_mask, n_live=n_live)
         if mode >= 2 and normalise:
             self._mark_operands_fresh()

@@ -19,8 +19,6 @@ struct FusedOut {  // device-side copy of vqb_fused_outputs
   const void* x_raw;
   void* resid_out;
   void* qsum;
-  float* stats_cnt;   // optional: cluster_size[k] += 1        (vqp:602)
-  float* stats_sum;   // optional: embed_sum[k][:] += x_eff[row] (vqp:605), vector RED into the L2-resident buffer
   int dtype;
   int enabled;
   uint16_t* planes_out;   // optional (fp32 rows): bf16 hi / lo split of the residual, [2][N][D]
@@ -33,6 +31,7 @@ inline int make_fused(FusedOut* o, const vqb_fused_outputs* f, int D, int64_t N 
   if (!f->x_eff || !f->embed) return VQB_E_INVALID;
   if (f->dtype != VQB_DTYPE_F32 && f->dtype != VQB_DTYPE_BF16) return VQB_E_INVALID;
   if (D % 8 != 0) return VQB_E_UNSUPPORTED;
+  if (f->stats_cnt || f->stats_sum) return VQB_E_UNSUPPORTED;   // reserved fields: the tail accumulates no statistics
   const uintptr_t all = reinterpret_cast<uintptr_t>(f->x_eff) | reinterpret_cast<uintptr_t>(f->embed) |
                         reinterpret_cast<uintptr_t>(f->q_out) | reinterpret_cast<uintptr_t>(f->x_raw) |
                         reinterpret_cast<uintptr_t>(f->resid_out) | reinterpret_cast<uintptr_t>(f->qsum);
@@ -40,25 +39,12 @@ inline int make_fused(FusedOut* o, const vqb_fused_outputs* f, int D, int64_t N 
   o->x_eff = f->x_eff; o->embed = f->embed; o->q_out = f->q_out; o->idx64_out = f->idx64_out;
   o->idx_stride = f->idx_stride; o->loss_sum = f->loss_sum; o->x_raw = f->x_raw ? f->x_raw : f->x_eff;
   o->resid_out = f->resid_out; o->qsum = f->qsum; o->dtype = f->dtype; o->enabled = 1;
-  o->stats_cnt = f->stats_cnt; o->stats_sum = f->stats_sum;
   if (f->planes_out) {  // the split rides on the fp32 residual
     if (f->dtype != VQB_DTYPE_F32 || !f->resid_out || N <= 0 || (reinterpret_cast<uintptr_t>(f->planes_out) & 15)) return VQB_E_INVALID;
     o->planes_out = static_cast<uint16_t*>(f->planes_out);
     o->planes_stride = N * D;
   }
-  if ((reinterpret_cast<uintptr_t>(f->stats_sum) & 15) != 0) return VQB_E_ALIGN;
   return VQB_OK;
-}
-
-// 16-byte vector reduction: four fp32 adds into global memory without a return value (sm_90+)
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-template <int VEC>
-__device__ __forceinline__ void stats_add(const FusedOut& o, int k, int D, int i, const float* xv) {
-  float* dst = o.stats_sum + static_cast<int64_t>(k) * D + i;
-  red_add_v4(dst, xv[0], xv[1], xv[2], xv[3]);
-  if (VEC == 8) red_add_v4(dst + 4, xv[4], xv[5], xv[6], xv[7]);
 }
 
 // bf16 hi / lo split of four fp32 values (the same arithmetic as input_prepare_kernel) -> the two operand planes
@@ -97,96 +83,43 @@ __device__ __forceinline__ uint4 pack16(const float* v) {
   return make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-// Returns this lane's partial of sum((q - x)^2) (0 if no loss is requested).  All 32 lanes must call.
-template <int DT>
-__device__ __forceinline__ float gather_row(const FusedOut& o, int64_t row, int k, int D, int lane) {
-  using E = Elem<DT>;
-  using T = typename E::T;
-  constexpr int VEC = 16 / sizeof(T);  // elements per 16-byte access: 8 (bf16) or 4 (fp32)
-  float lsum = 0.f;
-  if (o.idx64_out && lane == 0) o.idx64_out[row * o.idx_stride] = k;
-  if (o.stats_cnt && lane == 0) atomicAdd(o.stats_cnt + k, 1.f);
-  const float* c = o.embed + static_cast<int64_t>(k) * D;
-  const int64_t base = row * D;
-  for (int i = lane * VEC; i < D; i += 32 * VEC) {
-    float cv[8], xv[8], qv[8];
-#pragma unroll
-    for (int e = 0; e < VEC; e += 4) {
-      const float4 t = __ldg(reinterpret_cast<const float4*>(c + i + e));
-      cv[e] = t.x; cv[e + 1] = t.y; cv[e + 2] = t.z; cv[e + 3] = t.w;
-    }
-    unpack16<DT>(*reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(o.x_eff) + base + i), xv);
-    if (o.stats_sum) stats_add<VEC>(o, k, D, i, xv);
-#pragma unroll
-    for (int e = 0; e < VEC; ++e) {
-      qv[e] = E::round(cv[e]);
-      const float d = qv[e] - xv[e];
-      lsum += E::round(d * d);
-    }
-    if (o.q_out) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(o.q_out) + base + i) = pack16<DT>(qv);
-    if (o.resid_out) {
-      float rv[8];
-      if (o.x_raw != o.x_eff) unpack16<DT>(*reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(o.x_raw) + base + i), rv);
-      else {
-#pragma unroll
-        for (int e = 0; e < VEC; ++e) rv[e] = xv[e];
-      }
-#pragma unroll
-      for (int e = 0; e < VEC; ++e) rv[e] -= qv[e];
-      *reinterpret_cast<uint4*>(reinterpret_cast<T*>(o.resid_out) + base + i) = pack16<DT>(rv);
-      if (DT == VQB_DTYPE_F32 && o.planes_out) store_planes4(o.planes_out, o.planes_stride, base + i, rv);
-    }
-    if (o.qsum) {
-      float sv[8];
-      unpack16<DT>(*reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(o.qsum) + base + i), sv);
-#pragma unroll
-      for (int e = 0; e < VEC; ++e) sv[e] += qv[e];
-      *reinterpret_cast<uint4*>(reinterpret_cast<T*>(o.qsum) + base + i) = pack16<DT>(sv);
-    }
-  }
-  return lsum;
-}
-
-// Batched variant: B rows per call with all loads of the batch issued before any use/store, so a warp keeps
-// ~3*B independent 16-byte requests in flight (the store warps of the search kernel are latency-bound otherwise).
-// rows[b] < 0 marks an empty slot.  Returns this lane's loss partial.
+// B rows (ks[b] their codes) per call.  A batch (B > 1, the store warps of the search kernel, latency-bound otherwise) issues
+// all its loads before any use/store, so a warp keeps ~3*B independent 16-byte requests in flight; rows[b] < 0 marks an
+// empty slot.  The row kernels pass one row (rows[0] >= 0) and read x_raw / qsum where they are used: hoisting those loads
+// costs them ~14 registers, and the re-score kernels run next to the statistics sort.  All 32 lanes must call.  Returns
+// this lane's partial of sum((q - x)^2) (0 if no loss is requested).
 template <int DT, int B>
 __device__ __forceinline__ float gather_rows(const FusedOut& o, const int64_t (&rows)[B], const int (&ks)[B], int D, int lane) {
   using E = Elem<DT>;
   using T = typename E::T;
-  constexpr int VEC = 16 / sizeof(T);
+  constexpr int VEC = 16 / sizeof(T);  // elements per 16-byte access: 8 (bf16) or 4 (fp32)
+  auto ld = [](const void* p, int64_t off) { return *reinterpret_cast<const uint4*>(static_cast<const T*>(p) + off); };
   float lsum = 0.f;
   if (o.idx64_out && lane < B) {
 #pragma unroll
     for (int b = 0; b < B; ++b)
-      if (lane == b && rows[b] >= 0) o.idx64_out[rows[b] * o.idx_stride] = ks[b];
-  }
-  if (o.stats_cnt && lane < B) {
-#pragma unroll
-    for (int b = 0; b < B; ++b)
-      if (lane == b && rows[b] >= 0) atomicAdd(o.stats_cnt + ks[b], 1.f);
+      if (lane == b && (B == 1 || rows[b] >= 0)) o.idx64_out[rows[b] * o.idx_stride] = ks[b];
   }
   for (int i = lane * VEC; i < D; i += 32 * VEC) {
     float4 cq[B][VEC / 4];
     uint4 xq[B], rq[B], sq[B];
 #pragma unroll
     for (int b = 0; b < B; ++b) {
-      if (rows[b] < 0) continue;
+      if (B > 1 && rows[b] < 0) continue;
       const float* c = o.embed + static_cast<int64_t>(ks[b]) * D + i;
 #pragma unroll
       for (int e = 0; e < VEC / 4; ++e) cq[b][e] = __ldg(reinterpret_cast<const float4*>(c) + e);
       const int64_t off = rows[b] * D + i;
-      xq[b] = *reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(o.x_eff) + off);
-      if (o.resid_out && o.x_raw != o.x_eff) rq[b] = *reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(o.x_raw) + off);
-      if (o.qsum) sq[b] = *reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(o.qsum) + off);
+      xq[b] = ld(o.x_eff, off);
+      if (B > 1 && o.resid_out && o.x_raw != o.x_eff) rq[b] = ld(o.x_raw, off);
+      if (B > 1 && o.qsum) sq[b] = ld(o.qsum, off);
     }
 #pragma unroll
     for (int b = 0; b < B; ++b) {
-      if (rows[b] < 0) continue;
+      if (B > 1 && rows[b] < 0) continue;
       const int64_t off = rows[b] * D + i;
       float xv[8], qv[8];
       unpack16<DT>(xq[b], xv);
-      if (o.stats_sum) stats_add<VEC>(o, ks[b], D, i, xv);
 #pragma unroll
       for (int e = 0; e < VEC / 4; ++e) {
         qv[4 * e] = E::round(cq[b][e].x); qv[4 * e + 1] = E::round(cq[b][e].y);
@@ -200,7 +133,7 @@ __device__ __forceinline__ float gather_rows(const FusedOut& o, const int64_t (&
       if (o.q_out) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(o.q_out) + off) = pack16<DT>(qv);
       if (o.resid_out) {
         float rv[8];
-        if (o.x_raw != o.x_eff) unpack16<DT>(rq[b], rv);
+        if (o.x_raw != o.x_eff) unpack16<DT>(B > 1 ? rq[b] : ld(o.x_raw, off), rv);
         else {
 #pragma unroll
           for (int e = 0; e < VEC; ++e) rv[e] = xv[e];
@@ -212,7 +145,7 @@ __device__ __forceinline__ float gather_rows(const FusedOut& o, const int64_t (&
       }
       if (o.qsum) {
         float sv[8];
-        unpack16<DT>(sq[b], sv);
+        unpack16<DT>(B > 1 ? sq[b] : ld(o.qsum, off), sv);
 #pragma unroll
         for (int e = 0; e < VEC; ++e) sv[e] += qv[e];
         *reinterpret_cast<uint4*>(reinterpret_cast<T*>(o.qsum) + off) = pack16<DT>(sv);

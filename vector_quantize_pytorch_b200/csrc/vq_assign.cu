@@ -91,8 +91,8 @@ struct Ctrl {  // lives at the start of dynamic smem
 };
 static_assert(sizeof(Ctrl) <= SMEM_CTRL_BYTES, "control block too large");
 
-// Generic fused tail of one batch of rows (needs x again: residual / running sum / fused statistics).  Kept out of
-// line so that its register appetite does not set the allocation of the whole persistent kernel.
+// Generic fused tail of one batch of rows (needs x again: running sum / cosine residual).  Kept out of line so that
+// its register appetite does not set the allocation of the whole persistent kernel.
 template <int GB>
 __device__ __forceinline__ float tail_rows(const FusedOut& fo, const int64_t (&rows)[GB], const int (&ks)[GB], int D, int lane) {
   if (fo.dtype == VQB_DTYPE_BF16) return gather_rows<VQB_DTYPE_BF16, GB>(fo, rows, ks, D, lane);
@@ -120,7 +120,7 @@ __device__ __forceinline__ float sq_diff16(const uint4& xa, const uint4& ca, boo
 }
 
 // TAIL selects the work of the store warps at compile time (one instantiation each: the variants do not share a register
-// budget): 0 = none / generic (x re-read: running sum, fused statistics, cosine residual), 1 = copy mode, 2 = resid mode.
+// budget): 0 = none / generic (x re-read: running sum, cosine residual), 1 = copy mode, 2 = resid mode.
 template <int TAIL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -681,10 +681,12 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   if (N > (static_cast<int64_t>(1) << 31) - BM) return VQB_E_UNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(a_planes) | reinterpret_cast<uintptr_t>(b_planes) | reinterpret_cast<uintptr_t>(bext)) & 15)
     return VQB_E_ALIGN;
+  AssignParams p;
+  rc = make_fused(&p.fo, fused, D, N);
+  if (rc) return rc;
   rc = check_device();
   if (rc) return rc;
 
-  AssignParams p;
   p.N = N; p.D = D; p.K = K;
   p.Kpad = vqb_padded_codes(K);
   p.n_a = n_a; p.n_passes = n_passes; p.KB = plan.KB;
@@ -695,17 +697,15 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   p.row_mask = row_mask;
   p.prof = g_prof;
   p.tagmask = 0xFFFFFFF0u; p.mul1 = 1u; p.mulm1 = 0xFFFFFFFFu;
-  rc = make_fused(&p.fo, fused, D, N);
-  if (rc) return rc;
   p.metric = metric;
   p.cnorm2 = cnorm2;
   p.b_hi = static_cast<const uint16_t*>(b_planes);   // plane 0: bf16(c) == the quantized row for bf16 inputs
   p.bext = static_cast<const uint16_t*>(bext);
-  // pure-copy tail: nothing needs x again (no residual / running sum / fused statistics); the cosine loss needs ||c||^2
-  p.copy_mode = p.fo.enabled && !p.fo.resid_out && !p.fo.qsum && !p.fo.stats_sum &&
+  // pure-copy tail: nothing needs x again (no residual / running sum); the cosine loss needs ||c||^2
+  p.copy_mode = p.fo.enabled && !p.fo.resid_out && !p.fo.qsum &&
                 !(metric == VQB_METRIC_COSINE && p.fo.loss_sum && !cnorm2);
   // residual-only tail of a ResidualVQ stage on the raw rows (Euclidean, or inputs that were already unit vectors)
-  p.resid_mode = p.fo.enabled && p.fo.resid_out && !p.fo.q_out && !p.fo.qsum && !p.fo.stats_sum &&
+  p.resid_mode = p.fo.enabled && p.fo.resid_out && !p.fo.q_out && !p.fo.qsum &&
                  (!p.fo.x_raw || p.fo.x_raw == p.fo.x_eff) && !(metric == VQB_METRIC_COSINE && p.fo.loss_sum && !cnorm2);
   p.stream_a = plan.stream_a;
   p.a_global = static_cast<const uint16_t*>(a_planes);

@@ -95,11 +95,12 @@ __global__ void input_prepare_kernel(const void* __restrict__ x, int64_t N, int 
 // ---------------------------------------------------------------------------------------------
 // exact re-score of flagged rows (reference formula and tie rule)
 // ---------------------------------------------------------------------------------------------
+// Six CTAs per SM (40 registers): the kernel runs next to the statistics sort of vqb_vq_forward's side stream.
 template <int DT>
-__global__ void fix_flagged_kernel(const void* __restrict__ x, int64_t N, int D, const float* __restrict__ embed,
-                                   const float* __restrict__ cnorm2, int K, int metric,
-                                   vqb_flag_entry* __restrict__ flagged, const int32_t* __restrict__ flag_count,
-                                   int32_t* idx, const FusedOut fo) {
+__global__ void __launch_bounds__(ROW_THREADS, 6)
+fix_flagged_kernel(const void* __restrict__ x, int64_t N, int D, const float* __restrict__ embed,
+                   const float* __restrict__ cnorm2, int K, int metric, vqb_flag_entry* __restrict__ flagged,
+                   const int32_t* __restrict__ flag_count, int32_t* idx, const FusedOut fo) {
   using E = Elem<DT>;
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
@@ -142,7 +143,7 @@ __global__ void fix_flagged_kernel(const void* __restrict__ x, int64_t N, int D,
     }
     if (lane == 0) idx[fe.row] = best_k;
     if (fo.enabled) {  // finish the row the search kernel left to us: gather / loss / residual
-      const double l = warp_sum(static_cast<double>(gather_row<DT>(fo, fe.row, best_k, D, lane)));
+      const double l = warp_sum(static_cast<double>(gather_rows<DT, 1>(fo, {int64_t{fe.row}}, {best_k}, D, lane)));
       if (fo.loss_sum && lane == 0) atomicAdd(fo.loss_sum, l);
     }
   }
@@ -257,7 +258,7 @@ __global__ void fix_finish_kernel(int64_t N, int D, const vqb_flag_entry* __rest
     const int k = static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(key & 0xFFFFFFFFull));
     if (lane == 0) idx[fe.row] = k;
     if (fo.enabled) {
-      const double l = warp_sum(static_cast<double>(gather_row<DT>(fo, fe.row, k, D, lane)));
+      const double l = warp_sum(static_cast<double>(gather_rows<DT, 1>(fo, {int64_t{fe.row}}, {k}, D, lane)));
       if (fo.loss_sum && lane == 0) atomicAdd(fo.loss_sum, l);
     }
   }
@@ -273,7 +274,7 @@ __global__ void gather_kernel(int64_t N, int D, const int32_t* __restrict__ idx,
   float lsum = 0.f;
   for (int64_t row = static_cast<int64_t>(blockIdx.x) * wpb + (threadIdx.x >> 5); row < N;
        row += static_cast<int64_t>(gridDim.x) * wpb)
-    lsum += gather_row<DT>(fo, row, idx[row], D, lane);
+    lsum += gather_rows<DT, 1>(fo, {row}, {idx[row]}, D, lane);
   if (fo.loss_sum) {
     __shared__ double part[32];
     const double w = warp_sum(static_cast<double>(lsum));
@@ -619,7 +620,6 @@ extern "C" int vqb_gather(const void* x_eff, int dtype, int64_t N, int D, const 
   vqb_fused_outputs f = {};
   f.x_eff = x_eff; f.embed = embed; f.q_out = q_out; f.idx64_out = idx64_out; f.idx_stride = idx_stride;
   f.loss_sum = loss_sum; f.x_raw = x_raw; f.resid_out = resid_out; f.qsum = qsum; f.dtype = dtype;
-  f.stats_cnt = nullptr; f.stats_sum = nullptr;
   FusedOut fo;
   const int rc = make_fused(&fo, &f, D);
   if (rc) return rc;

@@ -12,6 +12,12 @@
 
 using namespace vqb;
 
+// Callers mirror these structs field for field (the ctypes stub of INTEGRATION.md, _C.py): their layout is part of the
+// ABI and must not move.  Sizes on x86-64.
+static_assert(sizeof(vqb_vq_forward_args) == 328, "vqb_vq_forward_args layout changed");
+static_assert(sizeof(vqb_fused_outputs) == 104, "vqb_fused_outputs layout changed");
+static_assert(sizeof(vqb_rvq_op) == 808, "vqb_rvq_op layout changed");
+
 extern "C" int vqb_debug_active(void);  // vq_assign.cu: diagnostics (profile buffer / debug mode) are armed
 
 namespace {
@@ -111,7 +117,7 @@ void make_keys(const vqb_vq_forward_args* a, void* stream, uint64_t* sk, uint64_
   P(a->peer_epoch);
   for (int r = 0; r < a->peer_world && r < 16; ++r) { P(a->peer_stats ? a->peer_stats[r] : nullptr); P(a->peer_flags ? a->peer_flags[r] : nullptr); }
   I(a->dtype); I(a->metric); I(a->N); I(a->D); I(a->K); I(a->already_normalised); I(a->idx_stride); F(a->loss_weight);
-  I(a->update); I(a->stats_mode); I(a->stats_accumulate); I(a->do_normalise); F(a->decay); F(a->eps); F(a->margin_rel);
+  I(a->update); I(a->do_normalise); F(a->decay); F(a->eps); F(a->margin_rel);
   I(static_cast<long long>(a->workspace_bytes)); I(reinterpret_cast<long long>(stream)); I(static_cast<long long>(present));
   I(a->peer_rank); I(a->peer_world); I(a->peer_slice_offset);
   while (si < kKeyWords) sk[si++] = 0;
@@ -398,6 +404,8 @@ uint64_t hash_words(const uint64_t* w, int n, uint64_t seed) {
 
 extern "C" int vqb_vq_forward(const vqb_vq_forward_args* a, void* stream) {
   if (!a) return VQB_E_INVALID;
+  // the statistics always come from the counting sort, which writes `stats` whole: nothing accumulates onto it
+  if (a->update && a->stats_accumulate) return VQB_E_UNSUPPORTED;
   std::lock_guard<std::mutex> lock(g_cache_mutex);
   if (a->ev_search_begin || a->ev_search_end || !graphs_usable(static_cast<cudaStream_t>(stream)))
     return vq_forward_enqueue(a, stream);
@@ -411,8 +419,11 @@ extern "C" int vqb_rvq_forward(const vqb_rvq_op* ops, int n_ops, void* stream) {
   std::lock_guard<std::mutex> lock(g_cache_mutex);
   RvqCtx ctx{ops, n_ops};
   bool events = false;
-  for (int i = 0; i < n_ops; ++i)
-    events |= ops[i].kind == VQB_RVQ_STAGE && (ops[i].stage.ev_search_begin || ops[i].stage.ev_search_end);
+  for (int i = 0; i < n_ops; ++i) {
+    if (ops[i].kind != VQB_RVQ_STAGE) continue;
+    if (ops[i].stage.update && ops[i].stage.stats_accumulate) return VQB_E_UNSUPPORTED;   // as in vqb_vq_forward
+    events |= ops[i].stage.ev_search_begin || ops[i].stage.ev_search_end;
+  }
   if (events || !graphs_usable(static_cast<cudaStream_t>(stream))) return rvq_enqueue(&ctx, stream);
   // one key word per op: hashes of its structural words and of its pointers
   uint64_t sk[kKeyWords], pk[kKeyWords];
@@ -532,27 +543,17 @@ static int vq_forward_enqueue(const vqb_vq_forward_args* a, void* stream, int la
   f.x_raw = (x_eff != a->x) ? a->x : nullptr;
   f.resid_out = a->resid_out; f.qsum = a->qsum; f.dtype = a->dtype;
   f.planes_out = (a->dtype == VQB_DTYPE_F32 && a->resid_out && !l2) ? a->planes_out : nullptr;
-  const bool fused_stats = a->update && a->stats_mode == 0;
-  f.stats_cnt = nullptr; f.stats_sum = nullptr;
-  if (fused_stats) {  // statistics ride on the store warps: zero the packed buffer, accumulate with vector REDs
-    if (!a->stats_accumulate) {
-      e = cudaMemsetAsync(a->stats, 0, sizeof(float) * static_cast<size_t>(vqb_stats_floats(a->K, a->D)), s);
-      if (e != cudaSuccess) return static_cast<int>(e);
-    }
-    f.stats_cnt = a->stats;
-    f.stats_sum = a->stats + vqb_stats_offset(a->K);
-  }
   // A ResidualVQ stage that also keeps the running sum (qsum: read-modify-write of one more (N x D) tensor from HBM)
   // throttles the search kernel when its four store warps run that tail (measured +0.3 ms per stage at config 3), so
   // it runs as the stand-alone gather kernel after the re-score.  The residual-only tail (x row from L2 — the TMA just
   // read it —, code row from L2, one (N x D) write) stays fused: ResidualVQ rebuilds the running sum from the indices
   // at the end (vqb_rvq_accumulate).  The VectorQuantize tail (row copy + loss from the scores) is always fused.
-  const bool split_tail = a->qsum && !fused_stats;
+  const bool split_tail = a->qsum;
   if (a->planes_out && (split_tail || a->dtype != VQB_DTYPE_F32 || !a->resid_out || l2)) return VQB_E_UNSUPPORTED;
-  const bool want_tail = !split_tail && (a->q_out || a->idx64_out || a->loss_out || fused_stats);
+  const bool want_tail = !split_tail && (a->q_out || a->idx64_out || a->loss_out);
   // Masked batch (row_mask): padding rows keep their pre-filled outputs and leave loss and statistics alone (vq_assign.cu,
-  // merge step).  Supported on the VectorQuantize chain: no ResidualVQ recurrence outputs, statistics by the sort.
-  if (a->row_mask && (split_tail || fused_stats || a->resid_out || a->qsum || a->planes_out)) return VQB_E_UNSUPPORTED;
+  // merge step).  Supported on the VectorQuantize chain: no ResidualVQ recurrence outputs.
+  if (a->row_mask && (split_tail || a->resid_out || a->qsum || a->planes_out)) return VQB_E_UNSUPPORTED;
   if (a->n_live && !a->row_mask) return VQB_E_INVALID;
   vqb_flag_entry* flagged = reinterpret_cast<vqb_flag_entry*>(ws + w.flagged);
   // The EMA sort (histogram -> scans -> scatter -> segmented sums) only needs the indices, and all but ~0.1 % of them
@@ -563,7 +564,7 @@ static int vq_forward_enqueue(const vqb_vq_forward_args* a, void* stream, int la
   // sizes, and the cluster-size half of the EMA follows them there.  Only the row half of the EMA waits for the segmented
   // sums.  Critical path after the search: scan -> scatter -> sums -> EMA rows (was: hist -> colscan -> scan -> scatter ->
   // sums -> re-scored rows -> EMA sizes -> EMA rows).
-  SideStream* side = (a->update && !fused_stats) ? side_stream(lane) : nullptr;
+  SideStream* side = a->update ? side_stream(lane) : nullptr;
   int32_t* idx_prov = side ? reinterpret_cast<int32_t*>(ws + w.idx_prov) : nullptr;
   const size_t stats_ws_bytes = a->update ? vqb_ema_stats_workspace(a->N, a->K) : 0;
   int32_t* hist = nullptr;
@@ -638,7 +639,7 @@ static int vq_forward_enqueue(const vqb_vq_forward_args* a, void* stream, int la
       if (rc) return rc;
     }
     if (cudaStreamWaitEvent(s, side->join, 0) != cudaSuccess) return static_cast<int>(cudaGetLastError());
-  } else if (a->update && !fused_stats) {
+  } else if (a->update) {  // no side stream for this lane: the whole sort on the caller's stream
     rc = vqb_ema_stats(x_eff, a->dtype, a->N, a->D, a->idx32, a->K, a->stats, ws + w.stats_ws, stats_ws_bytes, stream);
     if (rc) return rc;
   }

@@ -171,8 +171,6 @@ def search(x: torch.Tensor, ops: CodebookOperands, embed: torch.Tensor, *, margi
     return SearchResult(idx, x_eff, count[:1], flagged, best, count[1:])
 
 
-# 0: EMA statistics accumulated inside the search kernel (vector RED into L2); 1: separate sort + segmented sums
-STATS_MODE = int(__import__("os").environ.get("VQB_STATS_MODE", "1"))
 _WS_CACHE: dict = {}
 
 
@@ -195,7 +193,7 @@ def take_workspaces(ws_key, device) -> list:
 def vq_forward_args(x: torch.Tensor, ops: CodebookOperands, state: tuple, *, update: int, do_normalise: bool, decay: float,
                     eps: float, q_out=None, idx64_out=None, idx_stride: int = 1, loss_out=None, loss_weight: float = 1.0,
                     resid_out=None, qsum=None, stats=None, margin: float | None = None, already_normalised: bool = False,
-                    ws_key=None, stats_accumulate: bool = False, peer=None, peer_ptrs=None, peer_slice_offset: int = 0,
+                    ws_key=None, peer=None, peer_ptrs=None, peer_slice_offset: int = 0,
                     a_planes_in=None, planes_out=None, row_mask=None, n_live=None):
     """The argument block of one vqb_vq_forward call (also one VQB_RVQ_STAGE op of vqb_rvq_forward).
     row_mask (N,) uint8 / n_live (1,) int64 on the device: a masked batch (vqp:1116-1119) — padding rows (0) keep the values
@@ -222,7 +220,7 @@ def vq_forward_args(x: torch.Tensor, ops: CodebookOperands, state: tuple, *, upd
         cluster_size=_p(cs), embed_avg=_p(ea), embed=_p(emb), planes=_p(ops.planes), bext=_p(ops.bext), bias=_p(ops.bias),
         cnorm2=_p(ops.cnorm2), cmax=_p(ops.cmax), scratch=_p(ops.scratch), q_out=_p(q_out), idx64_out=_p(idx64_out),
         idx_stride=int(idx_stride), loss_out=_p(loss_out), loss_weight=float(loss_weight), resid_out=_p(resid_out),
-        qsum=_p(qsum), idx32=_p(idx32), update=int(update), stats_mode=STATS_MODE, stats_accumulate=int(stats_accumulate), do_normalise=int(do_normalise), decay=float(decay),
+        qsum=_p(qsum), idx32=_p(idx32), update=int(update), stats_mode=1, do_normalise=int(do_normalise), decay=float(decay),
         eps=float(eps), stats=_p(stats), margin_rel=float(DEFAULT_MARGIN if margin is None else margin),
         workspace=_p(ws), workspace_bytes=nbytes, ev_search_begin=None, ev_search_end=None,
         a_planes_in=_p(a_planes_in), planes_out=_p(planes_out), row_mask=_p(row_mask), n_live=_p(n_live))

@@ -322,12 +322,11 @@ class VectorQuantize(nn.Module):
             n = r1 - r0
             weights.append(n / N)
             cur.wait_event(ev_up[c])
-            in_place = ops.STATS_MODE == 0  # fused statistics accumulate straight into the running total
             cbk.quantize_rows(st["x"][r0:r1], update=do_update, q_out=st["q"][r0:r1], idx64_out=st["i"][r0:r1],
                               loss_out=st["loss"][c:c + 1] if want_loss else None, loss_weight=self.commitment_weight,
-                              stats_out=(st["stats"] if (in_place or c == 0) else st["stats_chunk"]) if do_update else None,
-                              defer_ema=True, stats_accumulate=in_place and c > 0)
-            if do_update and not in_place and c > 0:
+                              stats_out=(st["stats"] if c == 0 else st["stats_chunk"]) if do_update else None,
+                              defer_ema=True)
+            if do_update and c > 0:
                 st["stats"].add_(st["stats_chunk"])
             e = torch.cuda.Event(); e.record(cur)
             with torch.cuda.stream(down):
@@ -370,7 +369,7 @@ class VectorQuantize(nn.Module):
         B, N, D = x.shape
         flat = x.detach().reshape(-1, D)
         do_update = training and not freeze_codebook and (ema_update or cbk.has_dead_code_replacement)
-        if (ops.STATS_MODE == 1 and not self.use_cosine_sim and cbk._initted_host and x.dtype in (torch.float32, torch.bfloat16)
+        if (not self.use_cosine_sim and cbk._initted_host and x.dtype in (torch.float32, torch.bfloat16)
                 and not (do_update and cbk.has_dead_code_replacement)):
             # in-kernel mask: every row is searched (like the reference), the merge step of the search kernel drops the padding
             # rows — index -1, outputs left as pre-filled here, no loss term, no statistics — and the loss is divided by the
