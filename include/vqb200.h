@@ -63,7 +63,8 @@ typedef struct vqb_fused_outputs {
   double* loss_sum;    /* f64[1] += sum((q-x)^2) or NULL                                       */
   const void* x_raw;   /* NULL = x_eff                                                         */
   void* resid_out;     /* [N][D] dtype = x_raw - q or NULL                                     */
-  void* qsum;          /* [N][D] dtype += q or NULL                                            */
+  void* qsum;          /* reserved, must be NULL (VQB_E_UNSUPPORTED otherwise): ResidualVQ rebuilds */
+                       /* its running sum from the indices (vqb_rvq_accumulate)                  */
   float* stats_cnt;    /* reserved, must be NULL (VQB_E_UNSUPPORTED otherwise): statistics come */
   float* stats_sum;    /* from vqb_ema_stats, the tail accumulates none                          */
   int dtype;           /* VQB_DTYPE_*                                                          */
@@ -125,7 +126,7 @@ int vqb_assign(const void* a_planes, int n_a, int64_t N, int D, const void* b_pl
                int32_t* flag_count, float* dbg_best, const vqb_fused_outputs* fused /* NULL: search only */, void* stream);
 
 /* vqb_assign + the metric / ||c||^2 (cnorm2 [K]) that the in-kernel commitment loss of the COSINE metric needs.
- * When the fused tail asks for neither residual nor running sum, the tail degenerates to a row copy
+ * When the fused tail asks for no residual, the tail degenerates to a row copy
  * q <- codebook row (bf16 inputs: the bf16 hi plane) and the loss is read off the winning score. */
 int vqb_assign_ex(const void* a_planes, int n_a, int64_t N, int D, const void* b_planes, const void* bext,
                   const float* cmax, int K, float margin_rel, int n_passes, int32_t* idx, vqb_flag_entry* flagged,
@@ -160,7 +161,8 @@ int vqb_fix_flagged(const void* x_eff, int dtype, int64_t N, int D, const float*
  *   loss_sum  f64[1] += sum((q - x)^2)  (bf16: each square rounded to bf16 as torch does) (:1327)
  *   x_raw     [N][D] dtype : the stage input before l2norm (cosine); NULL = x_eff
  *   resid_out [N][D] dtype = x_raw - q   (NULL to skip)                               (residual_vq.py:524)
- *   qsum      [N][D] dtype += q      (NULL to skip)                                   (residual_vq.py:525) */
+ *   qsum      reserved, must be NULL (VQB_E_UNSUPPORTED otherwise): ResidualVQ's running sum (residual_vq.py:525)
+ *             is rebuilt from the indices by vqb_rvq_accumulate */
 int vqb_gather(const void* x_eff, int dtype, int64_t N, int D, const float* embed, const int32_t* idx, void* q_out,
                int64_t* idx64_out, int64_t idx_stride, double* loss_sum, const void* x_raw, void* resid_out, void* qsum,
                void* stream);
@@ -231,7 +233,9 @@ typedef struct vqb_vq_forward_args {
   void* q_out;              /* [N][D] dtype or NULL                                                            */
   int64_t* idx64_out; int64_t idx_stride;   /* int64 indices (NULL to skip)                                    */
   float* loss_out; float loss_weight;       /* f32[1] = weight * mse (NULL to skip)                            */
-  void* resid_out; void* qsum;              /* ResidualVQ recurrence (NULL to skip)                            */
+  void* resid_out;                          /* ResidualVQ recurrence: x - q (NULL to skip)                     */
+  void* qsum;                               /* reserved, must be NULL (VQB_E_UNSUPPORTED otherwise): the running
+                                               sum is rebuilt from the indices (vqb_rvq_accumulate)             */
   int32_t* idx32;           /* [N] int32 indices (always written; input of the statistics)                     */
   int update;               /* 0: none; 1: statistics only (caller all-reduces, then vqb_ema_apply); 2: + apply;
                                3: + peer barrier + apply over every rank's statistics (see peer_* below)             */
@@ -254,7 +258,7 @@ typedef struct vqb_vq_forward_args {
    * searched (the tiles stay dense) but gets index -1 in idx32, its q_out / idx64_out are NOT written (the caller pre-fills them:
    * zeros or the input, and -1, :1378-1396), it adds nothing to the loss (:1317-1325) or to the statistics (:599-600) and is
    * never re-scored.  n_live i64 [1] (device): the number of unmasked rows, the divisor of the loss (NULL: N).  VectorQuantize
-   * chain only (resid_out / qsum / planes_out must be NULL).  NULL = no mask. */
+   * chain only (resid_out / planes_out must be NULL).  NULL = no mask. */
   const uint8_t* row_mask; const int64_t* n_live;
 } vqb_vq_forward_args;
 size_t vqb_vq_forward_workspace(int64_t N, int D, int K, int dtype, int metric, int update);

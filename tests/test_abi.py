@@ -63,8 +63,8 @@ def test_struct_layout_is_pinned():
     assert ctypes.sizeof(_C.FusedOutputs) == 104
     assert ctypes.sizeof(_C.RvqOp) == 808
     offsets = {(_C.VQForwardArgs, "stats_mode"): 180, (_C.VQForwardArgs, "stats_accumulate"): 184,
-               (_C.VQForwardArgs, "row_mask"): 312, (_C.VQForwardArgs, "n_live"): 320,
-               (_C.FusedOutputs, "stats_cnt"): 72, (_C.FusedOutputs, "stats_sum"): 80, (_C.FusedOutputs, "planes_out"): 96}
+               (_C.VQForwardArgs, "row_mask"): 312, (_C.VQForwardArgs, "n_live"): 320, (_C.VQForwardArgs, "qsum"): 160,
+               (_C.FusedOutputs, "qsum"): 64, (_C.FusedOutputs, "stats_cnt"): 72, (_C.FusedOutputs, "stats_sum"): 80, (_C.FusedOutputs, "planes_out"): 96}
     for (cls, field), off in offsets.items():
         assert getattr(cls, field).offset == off, (cls.__name__, field)
 
@@ -82,6 +82,24 @@ def test_retired_statistics_options_are_rejected():
     for field in ("stats_cnt", "stats_sum"):
         f = _C.FusedOutputs(x_eff=p, embed=p, q_out=p, dtype=_C.DTYPE_BF16, **{field: p})
         assert lib.vqb_assign(p, 1, 1024, 64, p, p, p, 64, 0.0, 0, p, p, p, None, ctypes.byref(f), None) == -2
+
+
+def test_retired_running_sum_is_rejected():
+    """ResidualVQ rebuilds quantized_out from the indices (vqb_rvq_accumulate): a non-NULL `qsum` — the running sum the
+    stage tail used to add into — is refused before any CUDA call by every entry point that takes one."""
+    from vector_quantize_pytorch_b200 import _C
+    lib = _C.lib
+    p = 0x10000   # non-null, 16-byte aligned; never dereferenced
+    a = _C.VQForwardArgs(x=p, dtype=_C.DTYPE_BF16, N=1024, D=64, K=64, embed=p, planes=p, bext=p, bias=p, cnorm2=p, cmax=p,
+                         scratch=p, idx64_out=p, idx_stride=1, resid_out=p, qsum=p, idx32=p, workspace=p,
+                         workspace_bytes=1 << 30)
+    assert lib.vqb_vq_forward(ctypes.byref(a), None) == -2
+    op = _C.RvqOp(kind=_C.RVQ_STAGE, lane=0)
+    op.stage = a
+    assert lib.vqb_rvq_forward(ctypes.byref(op), 1, None) == -2
+    f = _C.FusedOutputs(x_eff=p, embed=p, resid_out=p, qsum=p, dtype=_C.DTYPE_BF16)
+    assert lib.vqb_assign(p, 1, 1024, 64, p, p, p, 64, 0.0, 0, p, p, p, None, ctypes.byref(f), None) == -2
+    assert lib.vqb_gather(p, _C.DTYPE_BF16, 1024, 64, p, p, None, p, 1, None, None, p, p, None) == -2
 
 
 def test_no_cpu_fallback():

@@ -198,33 +198,54 @@ def test_row_threshold_kernels_agree(kind, dt):
 # ------------------------------------------------------------------------------------------------ (c): the modules
 @pytest.mark.parametrize("program", ["1", "0"], ids=["program", "stagewise"])
 @pytest.mark.parametrize("dt", ["bf16", "fp32"])
-@pytest.mark.parametrize("kind", ["rvq_shared", "rvq_separate", "grvq"])
+@pytest.mark.parametrize("kind", ["rvq_shared", "rvq_separate", "grvq", "rvq_dropout", "rvq_mixed"])
 def test_module_running_sum_and_decode(kind, dt, program, monkeypatch):
     """`quantized` of a training forward is the recurrence (a) on the module's own indices and the codebooks the stages
-    searched (before the deferred EMA update); get_output_from_indices is the decode (b) on the updated codebooks."""
+    searched (before the deferred EMA update); get_output_from_indices is the decode (b) on the updated codebooks.
+    rvq_dropout: quantize dropout at a fixed seed that runs 2 of the 4 stages (the dropped columns are -1); rvq_mixed:
+    codebooks of different sizes.  Both always run stage-wise."""
     m = vqb()
     monkeypatch.setenv("VQB_RVQ_PROGRAM", program)
     torch.manual_seed(3)
+    kw, n_run = {}, None
     if kind == "grvq":
         mod = m.GroupedResidualVQ(dim=256, groups=2, num_quantizers=3, codebook_size=128).to(DEV)
         rvqs, dim = list(mod.rvqs), 256
+    elif kind == "rvq_dropout":
+        mod = m.ResidualVQ(dim=128, num_quantizers=4, codebook_size=256, quantize_dropout=True).to(DEV)
+        rvqs, dim = [mod], 128
+        kw, n_run = dict(rand_quantize_dropout_fixed_seed=1), 2   # random.Random(1).randrange(0, 4) == 1
+    elif kind == "rvq_mixed":
+        mod = m.ResidualVQ(dim=128, codebook_size=(256, 128, 512)).to(DEV)
+        rvqs, dim = [mod], 128
     else:
         shared = kind == "rvq_shared"
         mod = m.ResidualVQ(dim=128, num_quantizers=4, codebook_size=512 if shared else 256, shared_codebook=shared).to(DEV)
         rvqs, dim = [mod], 128
+
+    def books(r):   # (Q, K, D), codebooks of different sizes zero-padded to the largest
+        return torch.nn.utils.rnn.pad_sequence([layer._codebook.embed[0] for layer in r.layers], batch_first=True)
+
     for step in range(2):   # step 0 initialises the codebooks (stage-wise); step 1 runs the cached program when allowed
-        pre = [torch.stack([layer._codebook.embed[0] for layer in r.layers]).clone() for r in rvqs]
+        pre = [books(r).clone() for r in rvqs]
         x = torch.randn(2, 4096, dim, device=DEV).to(TDT[dt])
-        q, ind, _ = mod(x)
+        q, ind, _ = mod(x, **kw)
         torch.cuda.synchronize()
         inds = ind if kind == "grvq" else ind[None]
         Q = inds.shape[-1]
-        ref = torch.cat([running_sum_ref(E, i.reshape(-1, Q), TDT[dt]) for E, i in zip(pre, inds)], -1)
+        n = Q if n_run is None else n_run
+        if n < Q:
+            assert (inds[..., n:] == -1).all() and (inds[..., :n] >= 0).all(), f"step {step}: dropped stages"
+        ref = torch.cat([running_sum_ref(E[:n], i.reshape(-1, Q)[:, :n], TDT[dt]) for E, i in zip(pre, inds)], -1)
         assert torch.equal(q.reshape(-1, dim), ref), f"step {step}: quantized is not the rounded running sum"
-        post = [torch.stack([layer._codebook.embed[0] for layer in r.layers]) for r in rvqs]
-        dec = torch.cat([decode_ref(E, i.reshape(-1, Q), torch.float32) for E, i in zip(post, inds)], -1)
+        post = [books(r) for r in rvqs]
+        if kind == "rvq_mixed":   # get_output_from_indices sums get_codes_from_indices with torch
+            i = ind.reshape(-1, Q)
+            dec = torch.stack([post[0][s][i[:, s]] for s in range(Q)]).sum(dim=0)
+        else:
+            dec = torch.cat([decode_ref(E, i.reshape(-1, Q), torch.float32) for E, i in zip(post, inds)], -1)
         assert torch.equal(mod.get_output_from_indices(ind).reshape(-1, dim), dec), f"step {step}: decode differs"
-    assert (len(mod.__dict__.get("_plans", {})) >= 1) == (program == "1")
+    assert (len(mod.__dict__.get("_plans", {})) >= 1) == (program == "1" and kind not in ("rvq_dropout", "rvq_mixed"))
 
 
 # ------------------------------------------------------------------------------------------------ (d): rotation trick

@@ -96,12 +96,9 @@ def bits(t):
     return t.view(torch.int16) if t.element_size() == 2 else t.view(torch.int32)
 
 
-def guarded(N, D, dt, fill=None):
-    """(N + GUARD, D) buffer; rows >= N hold the sentinel (rows < N the sentinel too, or `fill`)."""
-    buf = torch.full((N + GUARD, D), SENT_F, dtype=TDT[dt], device=DEV)
-    if fill is not None:
-        buf[:N] = fill
-    return buf
+def guarded(N, D, dt):
+    """(N + GUARD, D) buffer holding the sentinel; rows >= N must keep it."""
+    return torch.full((N + GUARD, D), SENT_F, dtype=TDT[dt], device=DEV)
 
 
 def assert_guard(buf, N, what):
@@ -132,7 +129,7 @@ def plant_ties(N, D, K, cosine, gen):
 
 
 @pytest.mark.parametrize("dt,D,K,cosine,r", PLAN_CASES)
-def test_search_plan_multi_wave(dt, D, K, cosine, r):
+def test_search_plan_fused_tails(dt, D, K, cosine, r):
     from vector_quantize_pytorch_b200 import ops
     N = 128 * (2 * sms() + 1) + r
     gen = torch.Generator().manual_seed(D * 7919 + K * 31 + r)
@@ -208,22 +205,29 @@ def test_search_plan_multi_wave(dt, D, K, cosine, r):
         assert (p_buf[2 * N * D:] == SENT_P).all(), "residual tail: planes_out guard written"
     assert_loss_sum(l_res.item(), l_ref, dt, cosine, "residual tail: loss")   # cosine: the generic tail
 
-    # ---- generic tail: running sum qsum += q, q_out, int64 indices at a stride of 2, loss from x
-    qs0 = torch.randn(N, D, generator=gen).to(TDT[dt]).to(DEV)
-    s_buf = guarded(N, D, dt, fill=qs0)
+    # ---- generic tail (q_out and resid_out together): q_out, r <- x - q, int64 indices at a stride of 2, loss from x
     q2_buf = guarded(N, D, dt)
+    r2_buf = guarded(N, D, dt)
     i2_buf = torch.full(((N + GUARD) * 2,), SENT_I, dtype=torch.int64, device=DEV)
     l_gen = torch.zeros(1, dtype=torch.float64, device=DEV)
-    res3 = ops.search(x, cb, c, fused=dict(q_out=q2_buf[:N], qsum=s_buf[:N], idx64_out=i2_buf, idx_stride=2, loss_sum=l_gen))
+    res3 = ops.search(x, cb, c, fused=dict(q_out=q2_buf[:N], resid_out=r2_buf[:N], idx64_out=i2_buf, idx_stride=2, loss_sum=l_gen))
     torch.cuda.synchronize()
     assert torch.equal(res3.idx, res.idx)
-    assert torch.equal(bits(s_buf[:N]), bits((qs0.float() + q_ref.float()).to(TDT[dt]))), "generic tail: qsum"
-    assert_guard(s_buf, N, "generic tail: qsum")
+    assert torch.equal(bits(r2_buf[:N]), bits(r_ref)), "generic tail: resid_out"
+    assert_guard(r2_buf, N, "generic tail: resid_out")
     assert torch.equal(bits(q2_buf[:N]), bits(q_ref)), "generic tail: q_out"
     assert_guard(q2_buf, N, "generic tail: q_out")
     iv2 = i2_buf.view(N + GUARD, 2)
     assert torch.equal(iv2[:N, 0], idx) and (iv2[:N, 1] == SENT_I).all() and (iv2[N:] == SENT_I).all(), "generic tail: idx64_out"
     assert_loss_sum(l_gen.item(), l_ref, dt, True, "generic tail: loss")
+
+    # the running-sum output (qsum) is retired: asking for it is refused before the search kernel runs, not ignored
+    from vector_quantize_pytorch_b200._C import VQBError
+    s_buf = guarded(N, D, dt)
+    with pytest.raises(VQBError, match="vqb_assign"):
+        ops.search(x, cb, c, fused=dict(q_out=s_buf[:N], qsum=s_buf[:N]))
+    torch.cuda.synchronize()
+    assert (bits(s_buf) == bits(guarded(N, D, dt))).all(), "refused running sum: a buffer was written"
 
     # ---- EMA statistics of this batch
     st = ops.ema_stats(res.x_eff, res.idx, K)

@@ -334,13 +334,13 @@ class Codebook(nn.Module):
     # ------------------------------------------------------------------ the hot path
     @torch.no_grad()
     def quantize_rows(self, x: torch.Tensor, *, update: bool, q_out=None, idx64_out=None, idx_stride=1, loss_out=None,
-                      loss_weight=1.0, resid_out=None, qsum=None, stats_out=None, defer_ema=False, margin=None,
+                      loss_weight=1.0, resid_out=None, stats_out=None, defer_ema=False, margin=None,
                       ema_update=None, ema_update_weight=None, accum_ema_update=False,
                       row_mask=None, n_live=None):
         """x (N, D) contiguous fp32/bf16 — the input BEFORE the cosine l2norm (done in-kernel).
 
         One C call: search (pre-update codebook, vqp:743-747) with the fused gather / loss / residual tail
-        (vqp:766, :1178, :1327; rvq:524-525) -> batch statistics (vqp:602-607) -> EMA apply (vqp:616-617, :576-584).
+        (vqp:766, :1178, :1327; rvq:524) -> batch statistics (vqp:602-607) -> EMA apply (vqp:616-617, :576-584).
         With defer_ema (or when the statistics must be all-reduced first) the EMA apply is left to the caller.
         row_mask (N,) uint8 + n_live (1,) int64: in-kernel padding mask (vqp:1116-1119; ops.vq_forward_args) — the caller has made
         sure that neither k-means init nor dead-code expiry (both sample from `x[mask]`) can run in this call.
@@ -364,7 +364,7 @@ class Codebook(nn.Module):
         idx32, stats = ops.vq_forward(
             x, cb, self._state2d(), update=mode, do_normalise=normalise, decay=self.decay, eps=self.eps, q_out=q_out,
             idx64_out=idx64_out, idx_stride=idx_stride, loss_out=loss_out, loss_weight=loss_weight, resid_out=resid_out,
-            qsum=qsum, stats=stats_out, margin=margin, ws_key=id(self),
+            stats=stats_out, margin=margin, ws_key=id(self),
             peer=peer, peer_ptrs=peer_ptrs, row_mask=row_mask, n_live=n_live)
         if mode >= 2 and normalise:
             self._mark_operands_fresh()

@@ -1,7 +1,8 @@
 // Per-row tail of VectorQuantize.forward / one ResidualVQ stage, executed by ONE WARP for one row:
 //   q = embed[k].type(dtype)                      vqp:766/:779-781, :1178
 //   loss partial += sum((q - x)^2) in dtype        vqp:1327
-//   residual = x_raw - q ; quantized_out += q      rvq:524-525
+//   residual = x_raw - q                           rvq:524
+// (ResidualVQ's quantized_out += q, rvq:525, is rebuilt from the indices afterwards: vqb_rvq_accumulate.)
 // Shared by the stand-alone gather kernel, the store warps of the fused search kernel and the exact
 // re-score kernels (which finish the rows the search kernel could not certify).
 #pragma once
@@ -18,7 +19,6 @@ struct FusedOut {  // device-side copy of vqb_fused_outputs
   double* loss_sum;
   const void* x_raw;
   void* resid_out;
-  void* qsum;
   int dtype;
   int enabled;
   uint16_t* planes_out;   // optional (fp32 rows): bf16 hi / lo split of the residual, [2][N][D]
@@ -31,14 +31,15 @@ inline int make_fused(FusedOut* o, const vqb_fused_outputs* f, int D, int64_t N 
   if (!f->x_eff || !f->embed) return VQB_E_INVALID;
   if (f->dtype != VQB_DTYPE_F32 && f->dtype != VQB_DTYPE_BF16) return VQB_E_INVALID;
   if (D % 8 != 0) return VQB_E_UNSUPPORTED;
-  if (f->stats_cnt || f->stats_sum) return VQB_E_UNSUPPORTED;   // reserved fields: the tail accumulates no statistics
+  // reserved fields: the tail accumulates no statistics and no running sum
+  if (f->stats_cnt || f->stats_sum || f->qsum) return VQB_E_UNSUPPORTED;
   const uintptr_t all = reinterpret_cast<uintptr_t>(f->x_eff) | reinterpret_cast<uintptr_t>(f->embed) |
                         reinterpret_cast<uintptr_t>(f->q_out) | reinterpret_cast<uintptr_t>(f->x_raw) |
-                        reinterpret_cast<uintptr_t>(f->resid_out) | reinterpret_cast<uintptr_t>(f->qsum);
+                        reinterpret_cast<uintptr_t>(f->resid_out);
   if (all & 15) return VQB_E_ALIGN;
   o->x_eff = f->x_eff; o->embed = f->embed; o->q_out = f->q_out; o->idx64_out = f->idx64_out;
   o->idx_stride = f->idx_stride; o->loss_sum = f->loss_sum; o->x_raw = f->x_raw ? f->x_raw : f->x_eff;
-  o->resid_out = f->resid_out; o->qsum = f->qsum; o->dtype = f->dtype; o->enabled = 1;
+  o->resid_out = f->resid_out; o->dtype = f->dtype; o->enabled = 1;
   if (f->planes_out) {  // the split rides on the fp32 residual
     if (f->dtype != VQB_DTYPE_F32 || !f->resid_out || N <= 0 || (reinterpret_cast<uintptr_t>(f->planes_out) & 15)) return VQB_E_INVALID;
     o->planes_out = static_cast<uint16_t*>(f->planes_out);
@@ -85,8 +86,8 @@ __device__ __forceinline__ uint4 pack16(const float* v) {
 
 // B rows (ks[b] their codes) per call.  A batch (B > 1, the store warps of the search kernel, latency-bound otherwise) issues
 // all its loads before any use/store, so a warp keeps ~3*B independent 16-byte requests in flight; rows[b] < 0 marks an
-// empty slot.  The row kernels pass one row (rows[0] >= 0) and read x_raw / qsum where they are used: hoisting those loads
-// costs them ~14 registers, and the re-score kernels run next to the statistics sort.  All 32 lanes must call.  Returns
+// empty slot.  The row kernels pass one row (rows[0] >= 0) and read x_raw where it is used: hoisting that load costs them
+// registers, and the re-score kernels run next to the statistics sort.  All 32 lanes must call.  Returns
 // this lane's partial of sum((q - x)^2) (0 if no loss is requested).
 template <int DT, int B>
 __device__ __forceinline__ float gather_rows(const FusedOut& o, const int64_t (&rows)[B], const int (&ks)[B], int D, int lane) {
@@ -102,7 +103,7 @@ __device__ __forceinline__ float gather_rows(const FusedOut& o, const int64_t (&
   }
   for (int i = lane * VEC; i < D; i += 32 * VEC) {
     float4 cq[B][VEC / 4];
-    uint4 xq[B], rq[B], sq[B];
+    uint4 xq[B], rq[B];
 #pragma unroll
     for (int b = 0; b < B; ++b) {
       if (B > 1 && rows[b] < 0) continue;
@@ -112,7 +113,6 @@ __device__ __forceinline__ float gather_rows(const FusedOut& o, const int64_t (&
       const int64_t off = rows[b] * D + i;
       xq[b] = ld(o.x_eff, off);
       if (B > 1 && o.resid_out && o.x_raw != o.x_eff) rq[b] = ld(o.x_raw, off);
-      if (B > 1 && o.qsum) sq[b] = ld(o.qsum, off);
     }
 #pragma unroll
     for (int b = 0; b < B; ++b) {
@@ -142,13 +142,6 @@ __device__ __forceinline__ float gather_rows(const FusedOut& o, const int64_t (&
         for (int e = 0; e < VEC; ++e) rv[e] -= qv[e];
         *reinterpret_cast<uint4*>(reinterpret_cast<T*>(o.resid_out) + off) = pack16<DT>(rv);
         if (DT == VQB_DTYPE_F32 && o.planes_out) store_planes4(o.planes_out, o.planes_stride, off, rv);
-      }
-      if (o.qsum) {
-        float sv[8];
-        unpack16<DT>(B > 1 ? sq[b] : ld(o.qsum, off), sv);
-#pragma unroll
-        for (int e = 0; e < VEC; ++e) sv[e] += qv[e];
-        *reinterpret_cast<uint4*>(reinterpret_cast<T*>(o.qsum) + off) = pack16<DT>(sv);
       }
     }
   }

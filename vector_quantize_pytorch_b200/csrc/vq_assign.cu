@@ -701,11 +701,10 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   p.cnorm2 = cnorm2;
   p.b_hi = static_cast<const uint16_t*>(b_planes);   // plane 0: bf16(c) == the quantized row for bf16 inputs
   p.bext = static_cast<const uint16_t*>(bext);
-  // pure-copy tail: nothing needs x again (no residual / running sum); the cosine loss needs ||c||^2
-  p.copy_mode = p.fo.enabled && !p.fo.resid_out && !p.fo.qsum &&
-                !(metric == VQB_METRIC_COSINE && p.fo.loss_sum && !cnorm2);
+  // pure-copy tail: nothing needs x again (no residual); the cosine loss needs ||c||^2
+  p.copy_mode = p.fo.enabled && !p.fo.resid_out && !(metric == VQB_METRIC_COSINE && p.fo.loss_sum && !cnorm2);
   // residual-only tail of a ResidualVQ stage on the raw rows (Euclidean, or inputs that were already unit vectors)
-  p.resid_mode = p.fo.enabled && p.fo.resid_out && !p.fo.q_out && !p.fo.qsum &&
+  p.resid_mode = p.fo.enabled && p.fo.resid_out && !p.fo.q_out &&
                  (!p.fo.x_raw || p.fo.x_raw == p.fo.x_eff) && !(metric == VQB_METRIC_COSINE && p.fo.loss_sum && !cnorm2);
   p.stream_a = plan.stream_a;
   p.a_global = static_cast<const uint16_t*>(a_planes);

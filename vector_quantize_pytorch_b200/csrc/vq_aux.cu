@@ -243,9 +243,11 @@ fix_overflow_kernel(const void* __restrict__ x, int64_t N, int D, const float* _
   }
 }
 
+// Five CTAs per SM (at most 48 registers): like fix_flagged_kernel, it runs next to the statistics sort.
 template <int DT>
-__global__ void fix_finish_kernel(int64_t N, int D, const vqb_flag_entry* __restrict__ flagged,
-                                  const int32_t* __restrict__ flag_count, int32_t* idx, const FusedOut fo) {
+__global__ void __launch_bounds__(ROW_THREADS, 5)
+fix_finish_kernel(int64_t N, int D, const vqb_flag_entry* __restrict__ flagged, const int32_t* __restrict__ flag_count,
+                  int32_t* idx, const FusedOut fo) {
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
   int64_t cnt = flag_count[1];

@@ -112,7 +112,7 @@ void make_keys(const vqb_vq_forward_args* a, void* stream, uint64_t* sk, uint64_
   auto I = [&](long long v) { sk[si++] = static_cast<uint64_t>(v); };
   auto F = [&](double v) { uint64_t u; memcpy(&u, &v, 8); sk[si++] = u; };
   P(a->x); P(a->cluster_size); P(a->embed_avg); P(a->embed); P(a->planes); P(a->bext); P(a->bias); P(a->cnorm2); P(a->cmax);
-  P(a->scratch); P(a->q_out); P(a->idx64_out); P(a->loss_out); P(a->resid_out); P(a->qsum); P(a->idx32); P(a->stats);
+  P(a->scratch); P(a->q_out); P(a->idx64_out); P(a->loss_out); P(a->resid_out); P(a->idx32); P(a->stats);
   P(a->workspace); P(a->a_planes_in); P(a->planes_out); P(a->row_mask); P(a->n_live);
   P(a->peer_epoch);
   for (int r = 0; r < a->peer_world && r < 16; ++r) { P(a->peer_stats ? a->peer_stats[r] : nullptr); P(a->peer_flags ? a->peer_flags[r] : nullptr); }
@@ -406,6 +406,8 @@ extern "C" int vqb_vq_forward(const vqb_vq_forward_args* a, void* stream) {
   if (!a) return VQB_E_INVALID;
   // the statistics always come from the counting sort, which writes `stats` whole: nothing accumulates onto it
   if (a->update && a->stats_accumulate) return VQB_E_UNSUPPORTED;
+  // reserved: ResidualVQ rebuilds quantized_out from the indices (vqb_rvq_accumulate), the tail keeps no running sum
+  if (a->qsum) return VQB_E_UNSUPPORTED;
   std::lock_guard<std::mutex> lock(g_cache_mutex);
   if (a->ev_search_begin || a->ev_search_end || !graphs_usable(static_cast<cudaStream_t>(stream)))
     return vq_forward_enqueue(a, stream);
@@ -422,6 +424,7 @@ extern "C" int vqb_rvq_forward(const vqb_rvq_op* ops, int n_ops, void* stream) {
   for (int i = 0; i < n_ops; ++i) {
     if (ops[i].kind != VQB_RVQ_STAGE) continue;
     if (ops[i].stage.update && ops[i].stage.stats_accumulate) return VQB_E_UNSUPPORTED;   // as in vqb_vq_forward
+    if (ops[i].stage.qsum) return VQB_E_UNSUPPORTED;
     events |= ops[i].stage.ev_search_begin || ops[i].stage.ev_search_end;
   }
   if (events || !graphs_usable(static_cast<cudaStream_t>(stream))) return rvq_enqueue(&ctx, stream);
@@ -541,19 +544,13 @@ static int vq_forward_enqueue(const vqb_vq_forward_args* a, void* stream, int la
   f.x_eff = x_eff; f.embed = a->embed; f.q_out = a->q_out; f.idx64_out = a->idx64_out; f.idx_stride = a->idx_stride;
   f.loss_sum = a->loss_out ? loss_sum : nullptr;
   f.x_raw = (x_eff != a->x) ? a->x : nullptr;
-  f.resid_out = a->resid_out; f.qsum = a->qsum; f.dtype = a->dtype;
+  f.resid_out = a->resid_out; f.dtype = a->dtype;
   f.planes_out = (a->dtype == VQB_DTYPE_F32 && a->resid_out && !l2) ? a->planes_out : nullptr;
-  // A ResidualVQ stage that also keeps the running sum (qsum: read-modify-write of one more (N x D) tensor from HBM)
-  // throttles the search kernel when its four store warps run that tail (measured +0.3 ms per stage at config 3), so
-  // it runs as the stand-alone gather kernel after the re-score.  The residual-only tail (x row from L2 — the TMA just
-  // read it —, code row from L2, one (N x D) write) stays fused: ResidualVQ rebuilds the running sum from the indices
-  // at the end (vqb_rvq_accumulate).  The VectorQuantize tail (row copy + loss from the scores) is always fused.
-  const bool split_tail = a->qsum;
-  if (a->planes_out && (split_tail || a->dtype != VQB_DTYPE_F32 || !a->resid_out || l2)) return VQB_E_UNSUPPORTED;
-  const bool want_tail = !split_tail && (a->q_out || a->idx64_out || a->loss_out);
+  if (a->planes_out && (a->dtype != VQB_DTYPE_F32 || !a->resid_out || l2)) return VQB_E_UNSUPPORTED;
+  const bool want_tail = a->q_out || a->idx64_out || a->loss_out;
   // Masked batch (row_mask): padding rows keep their pre-filled outputs and leave loss and statistics alone (vq_assign.cu,
   // merge step).  Supported on the VectorQuantize chain: no ResidualVQ recurrence outputs.
-  if (a->row_mask && (split_tail || a->resid_out || a->qsum || a->planes_out)) return VQB_E_UNSUPPORTED;
+  if (a->row_mask && (a->resid_out || a->planes_out)) return VQB_E_UNSUPPORTED;
   if (a->n_live && !a->row_mask) return VQB_E_INVALID;
   vqb_flag_entry* flagged = reinterpret_cast<vqb_flag_entry*>(ws + w.flagged);
   // The EMA sort (histogram -> scans -> scatter -> segmented sums) only needs the indices, and all but ~0.1 % of them
@@ -603,11 +600,6 @@ static int vq_forward_enqueue(const vqb_vq_forward_args* a, void* stream, int la
   rc = vqb_fix_flagged(x_eff, a->dtype, a->N, a->D, a->embed, a->cnorm2, a->K, a->metric, flagged, flag_count, a->idx32,
                        want_tail ? &f : nullptr, stream);
   if (rc) return rc;
-  if (split_tail) {
-    rc = vqb_gather(x_eff, a->dtype, a->N, a->D, a->embed, a->idx32, a->q_out, a->idx64_out, a->idx_stride,
-                    a->loss_out ? loss_sum : nullptr, f.x_raw, a->resid_out, a->qsum, stream);
-    if (rc) return rc;
-  }
   if (a->loss_out) {
     rc = loss_finalize_launch(loss_sum, a->N * a->D, a->row_mask ? a->n_live : nullptr, a->D, a->dtype, a->loss_weight, a->loss_out,
                               stream);

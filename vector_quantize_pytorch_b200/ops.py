@@ -112,7 +112,7 @@ def search(x: torch.Tensor, ops: CodebookOperands, embed: torch.Tensor, *, margi
            debug_best: bool = False, fix: bool = True, normalise: bool = True, fused: dict | None = None) -> SearchResult:
     """Nearest code of every row of x (N, D).  Replaces cdist/einsum + argmax (vqp:58-62, :741-747, :130-145).
 
-    fused: optional dict(q_out=, idx64_out=, idx_stride=, loss_sum=, resid_out=, qsum=, planes_out=) of output tensors — the
+    fused: optional dict(q_out=, idx64_out=, idx_stride=, loss_sum=, resid_out=, planes_out=) of output tensors — the
     gather / commitment-loss / residual tail (see `gather`) then runs INSIDE the search kernel (store warps) and
     the re-score kernels, and no separate gather launch is needed.  planes_out (fp32 rows with resid_out): 2-byte
     [2][N][D], the bf16 hi / lo split of the residual (the next ResidualVQ stage's A operand)."""
@@ -151,8 +151,9 @@ def search(x: torch.Tensor, ops: CodebookOperands, embed: torch.Tensor, *, margi
             fo = _C.FusedOutputs(x_eff=_p(x_eff), embed=_p(embed), q_out=_p(fused.get("q_out")),
                                  idx64_out=_p(fused.get("idx64_out")), idx_stride=int(fused.get("idx_stride", 1)),
                                  loss_sum=_p(fused.get("loss_sum")), x_raw=_p(x) if x_eff is not x else None,
-                                 resid_out=_p(fused.get("resid_out")), qsum=_p(fused.get("qsum")), stats_cnt=None, stats_sum=None, dtype=dt,
-                                 planes_out=_p(fused.get("planes_out")))
+                                 resid_out=_p(fused.get("resid_out")), stats_cnt=None, stats_sum=None, dtype=dt,
+                                 planes_out=_p(fused.get("planes_out")),
+                                 qsum=_p(fused.get("qsum")))   # reserved: vqb_assign refuses a running sum, not ignores it
         fo_ref = ctypes.byref(fo) if fo is not None else None
         prof = PROFILE_EVENTS
         if prof is not None:
@@ -192,7 +193,7 @@ def take_workspaces(ws_key, device) -> list:
 
 def vq_forward_args(x: torch.Tensor, ops: CodebookOperands, state: tuple, *, update: int, do_normalise: bool, decay: float,
                     eps: float, q_out=None, idx64_out=None, idx_stride: int = 1, loss_out=None, loss_weight: float = 1.0,
-                    resid_out=None, qsum=None, stats=None, margin: float | None = None, already_normalised: bool = False,
+                    resid_out=None, stats=None, margin: float | None = None, already_normalised: bool = False,
                     ws_key=None, peer=None, peer_ptrs=None, peer_slice_offset: int = 0,
                     a_planes_in=None, planes_out=None, row_mask=None, n_live=None):
     """The argument block of one vqb_vq_forward call (also one VQB_RVQ_STAGE op of vqb_rvq_forward).
@@ -220,7 +221,7 @@ def vq_forward_args(x: torch.Tensor, ops: CodebookOperands, state: tuple, *, upd
         cluster_size=_p(cs), embed_avg=_p(ea), embed=_p(emb), planes=_p(ops.planes), bext=_p(ops.bext), bias=_p(ops.bias),
         cnorm2=_p(ops.cnorm2), cmax=_p(ops.cmax), scratch=_p(ops.scratch), q_out=_p(q_out), idx64_out=_p(idx64_out),
         idx_stride=int(idx_stride), loss_out=_p(loss_out), loss_weight=float(loss_weight), resid_out=_p(resid_out),
-        qsum=_p(qsum), idx32=_p(idx32), update=int(update), stats_mode=1, do_normalise=int(do_normalise), decay=float(decay),
+        idx32=_p(idx32), update=int(update), stats_mode=1, do_normalise=int(do_normalise), decay=float(decay),
         eps=float(eps), stats=_p(stats), margin_rel=float(DEFAULT_MARGIN if margin is None else margin),
         workspace=_p(ws), workspace_bytes=nbytes, ev_search_begin=None, ev_search_end=None,
         a_planes_in=_p(a_planes_in), planes_out=_p(planes_out), row_mask=_p(row_mask), n_live=_p(n_live))
@@ -355,15 +356,14 @@ class RvqProgram:
 
 def gather(x_eff: torch.Tensor, embed: torch.Tensor, idx: torch.Tensor, *, q_out: torch.Tensor | None = None,
            idx64_out: torch.Tensor | None = None, idx_stride: int = 1, loss_sum: torch.Tensor | None = None,
-           x_raw: torch.Tensor | None = None, resid_out: torch.Tensor | None = None,
-           qsum: torch.Tensor | None = None) -> None:
+           x_raw: torch.Tensor | None = None, resid_out: torch.Tensor | None = None) -> None:
     """quantize = embed[idx].type(x.dtype) (vqp:766/:779-781, :1178) fused with the mse partial sum (vqp:1327)
-    and, for ResidualVQ, residual -= q ; quantized_out += q (rvq:524-525)."""
+    and, for ResidualVQ, residual -= q (rvq:524)."""
     _require_cuda(x_eff, embed, idx)
     N, D = x_eff.shape
     with torch.cuda.device(x_eff.device):
         check(lib.vqb_gather(_p(x_eff), _dtype_code(x_eff), N, D, _p(embed), _p(idx), _p(q_out), _p(idx64_out),
-                             int(idx_stride), _p(loss_sum), _p(x_raw), _p(resid_out), _p(qsum), _stream()), "vqb_gather")
+                             int(idx_stride), _p(loss_sum), _p(x_raw), _p(resid_out), None, _stream()), "vqb_gather")
     _count(1)
 
 

@@ -1,11 +1,11 @@
 """`ResidualVQ` / `GroupedResidualVQ` — drop-ins for residual_vq.py:166-630 and :634-724 of the reference
 (no beam search, no implicit neural codebook; quantize dropout and masks run on the stage-wise path).
 
-The Q-stage recurrence  residual -= q ; quantized_out += q  (rvq:524-525) runs inside the gather
-kernel of every stage (rounded to the input dtype exactly where the reference rounds), indices are
-written straight into the (..., Q) int64 result, and the EMA statistics of ALL stages (and, for the
-grouped module, all groups) are packed into one buffer so that multi-GPU training needs ONE all-reduce
-per forward instead of the reference's 2 per codebook per stage.
+Every stage's search writes the next residual (residual -= q, rvq:524) from its fused tail and its indices
+straight into the (..., Q) int64 result; quantized_out += q (rvq:525) is rebuilt from those indices in one
+pass after the last stage (rounded to the input dtype exactly where the reference rounds).  The EMA
+statistics of ALL stages (and, for the grouped module, all groups) are packed into one buffer so that
+multi-GPU training needs ONE all-reduce per forward instead of the reference's 2 per codebook per stage.
 """
 from __future__ import annotations
 
@@ -340,7 +340,6 @@ class ResidualVQ(nn.Module):
         # update_codebook ends with expire_codes_, vqp:641, on the one aliased Codebook): such stages cannot be deferred.
         inline = [u and self.shared_codebook and b.has_dead_code_replacement for b, u in zip(books, do_update)]
         stat_sizes = [ops.stats_floats(b.codebook_size, D) if (u and not i) else 0 for b, u, i in zip(books, do_update, inline)]
-        running_sum = torch.zeros_like(flat) if (any(inline) or not self.uniform_codebook_size or n_run < Q) else None  # rvq:410
         packed, peer_ptrs = None, None
         if sum(stat_sizes):
             peer = self._peer_reducer(sum(stat_sizes), dev) if any(b.use_ddp for b in books) else None
@@ -351,26 +350,34 @@ class ResidualVQ(nn.Module):
                 packed = torch.empty((sum(stat_sizes),), dtype=torch.float32, device=dev)
         offs = [sum(stat_sizes[:i]) for i in range(Q)]
 
+        inline_embeds = []   # the shared codebook as each inline stage searched it
         for q, book in enumerate(books[:n_run]):  # rvq:469
             nxt = (bufs[q] if keep_inputs else bufs[q & 1]) if q + 1 < n_run else None
             if keep_inputs:
                 stage_inputs.append(residual)
+            if inline[q]:
+                if not book._initted_host:   # k-means init precedes the search (quantize_rows would run it next)
+                    book.init_embed_(book.transform_input(residual).float())
+                inline_embeds.append(book.embed[0].clone())
             want_loss = training and self.layers[q].has_commitment_loss
             book.quantize_rows(
                 residual, update=do_update[q], idx64_out=all_idx[:, q], idx_stride=Q,
                 loss_out=losses[q:q + 1] if want_loss else None, loss_weight=self.layers[q].commitment_weight,
-                resid_out=nxt, qsum=running_sum,
-                stats_out=packed[offs[q]:offs[q] + stat_sizes[q]] if stat_sizes[q] else None, defer_ema=not inline[q])
+                resid_out=nxt, stats_out=packed[offs[q]:offs[q] + stat_sizes[q]] if stat_sizes[q] else None,
+                defer_ema=not inline[q])
             residual = nxt
 
-        # quantized_out (rvq:410, :525): rebuilt from the indices in one pass over the codebooks the stages searched (their
-        # update is deferred to _finish_update below) instead of a read-modify-write of (N x D) in every stage.  Only when
-        # the codebooks cannot be stacked, or a shared codebook is modified between stages, the stages keep the sum.
-        if running_sum is None:
-            embeds = books[0].embed[0] if self.shared_codebook else torch.stack([b.embed[0] for b in books])
-            quantized_out = ops.rvq_accumulate(embeds, all_idx, dtype)
+        # quantized_out (rvq:410, :525): rebuilt from the indices of the stages that ran, in one pass over the codebooks they
+        # searched, instead of a read-modify-write of (N x D) in every stage.  Only inline stages change a codebook between
+        # stages; every other update is deferred to _finish_update below.  Codebooks of different sizes are zero-padded to
+        # the largest: every index of a stage is below its own size.
+        if inline_embeds:
+            searched = torch.stack(inline_embeds)
+        elif self.shared_codebook:
+            searched = books[0].embed[0]
         else:
-            quantized_out = running_sum
+            searched = torch.nn.utils.rnn.pad_sequence([b.embed[0] for b in books[:n_run]], batch_first=True)
+        quantized_out = ops.rvq_accumulate(searched, all_idx[:, :n_run].contiguous(), dtype)
 
         if packed is not None or any(inline):
             if _stats_sink is not None:  # GroupedResidualVQ gathers every group's statistics into one collective
