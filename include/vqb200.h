@@ -350,6 +350,15 @@ int vqb_rsimvq_backward(const float* x, const float* codes, int Q, int K, const 
  * src, tgt, grad_out, out: [N][D] in `dtype` (arithmetic in fp32, rounded once on store). */
 int vqb_rotate(const void* src, const void* tgt, const void* grad_out, int64_t N, int D, int dtype, void* out, void* stream);
 
+/* DiVeQ, the directional reparameterization estimator (vector_quantize_pytorch.py:323-330), one warp per row (D <= 1024):
+ *   e = q - x,  u = l2norm(e + noise_scale * noise) (detached),  out = x + u * ||e||
+ *   grad_out == NULL: forward   out = x + u ||e||                                  (dtype)
+ *   grad_out != NULL: backward  out = dx = g - (g.u) e / ||e||, grad_q = (g.u) e / ||e||   (0 where ||e|| = 0)
+ * x, q, noise (the raw N(0, 1) draw), grad_out, out: [N][D] in `dtype`; grad_q: f32 [N][D] (values rounded to `dtype`).
+ * Every step is rounded to `dtype` where torch rounds the reference's expression; the backward recomputes e, u and ||e||. */
+int vqb_diveq(const void* x, const void* q, const void* noise, const void* grad_out, int64_t N, int D, int dtype,
+              float noise_scale, void* out, float* grad_q, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

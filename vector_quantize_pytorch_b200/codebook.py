@@ -27,6 +27,41 @@ def _unsupported(what):
     raise NotImplementedError(f"vqb200: {what} is outside the accelerated hot path (SURVEY.md §8) and is not implemented")
 
 
+class _LearnableCodebook(torch.autograd.Function):
+    """Makes the kernels' `quantize` (and the commitment loss) differentiable w.r.t. a learnable `embed` (1, K, D).
+
+    The reference's `quantize = onehot @ embed` (vqp:766) — and its gathers from `embed` (vqp:779-781, :998-1018) — send every
+    row's upstream gradient to its code: d embed[k] = sum of the gradient rows n with idx(n) = k, taken by the statistics chain
+    (ops.ema_stats) on those rows.  `valid` (bool per row, optional): rows whose index was -1 (zeros, no code) send nothing.
+    The commitment loss `mse(quantize, x)` (vqp:1214-1216, :1327) adds scale * (count_k c_k - sum_{n -> k} x_n) per code, where
+    `commit_rows` is that K x D difference, formed from the search's own statistics before any codebook change."""
+
+    @staticmethod
+    def forward(ctx, embed, q, loss, idx32, commit_rows, commit_scale, valid=None):
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(idx32, commit_rows, valid)
+        ctx.commit_scale = commit_scale
+        ctx.embed_shape = embed.shape
+        return q, loss
+
+    @staticmethod
+    def backward(ctx, g_q, g_loss):
+        idx32, rows, valid = ctx.saved_tensors
+        H, K, D = ctx.embed_shape
+        grad = None
+        if g_q is not None:
+            g = g_q.reshape(-1, D)
+            if valid is not None:
+                g = g.masked_fill(~valid[:, None], 0)
+            stats = ops.ema_stats(g.contiguous(), idx32, K)
+            off = ops.stats_offset(K)
+            grad = stats[off:off + K * D].view(K, D)
+        if rows is not None and g_loss is not None:
+            part = rows * (g_loss.float() * ctx.commit_scale)
+            grad = part if grad is None else grad + part
+        return (None if grad is None else grad.view(H, K, D)), None, g_loss, None, None, None, None
+
+
 class Codebook(nn.Module):
     def __init__(
         self,
@@ -58,8 +93,12 @@ class Codebook(nn.Module):
             raise ValueError("num_codebooks must be >= 1")
         if kmeans_init and use_ddp and sync_kmeans:
             _unsupported("kmeans_init with distributed sampling (use_ddp + sync_kmeans, vqp:211-229)")
-        if learnable_codebook:
-            _unsupported("learnable_codebook")
+        if learnable_codebook and ema_update:
+            _unsupported("learnable_codebook with ema_update (the reference rejects the combination, vqp:908)")
+        if learnable_codebook and use_cosine_sim:
+            _unsupported("learnable_codebook with use_cosine_sim (the reference rejects the combination, vqp:884)")
+        if learnable_codebook and num_codebooks > 1:
+            _unsupported("learnable_codebook with num_codebooks > 1 (separate codebooks per head)")
         if affine_param:
             _unsupported("affine_param")
         if vq_bridge is not None:
@@ -82,7 +121,7 @@ class Codebook(nn.Module):
         self.sample_codebook_temp = sample_codebook_temp
         self.use_ddp = use_ddp
         self.sync_kmeans = sync_kmeans
-        self.learnable_codebook = False
+        self.learnable_codebook = learnable_codebook
         self.use_cosine_sim = use_cosine_sim
 
         self.kmeans_iters = kmeans_iters
@@ -97,7 +136,10 @@ class Codebook(nn.Module):
         self.register_buffer("initted", torch.tensor(not kmeans_init))  # vqp:415
         self.register_buffer("cluster_size", torch.ones(num_codebooks, codebook_size))  # vqp:416
         self.register_buffer("embed_avg", embed.clone())  # vqp:417
-        self.register_buffer("embed", embed)  # vqp:423
+        if learnable_codebook:  # vqp:419-421: same state_dict key and shape, trained by the caller's optimizer
+            self.embed = nn.Parameter(embed)
+        else:
+            self.register_buffer("embed", embed)  # vqp:423
 
         # num_codebooks > 1 (VectorQuantize(separate_codebook_per_head=True), vqp:1044-1049): every head is served by a light
         # view of this module (`head(i)`): same buffers, own slot, own operand cache
@@ -140,15 +182,31 @@ class Codebook(nn.Module):
         if embed.dtype != torch.float32 or not embed.is_contiguous():
             raise RuntimeError("vqb200: the `embed` buffer must be contiguous float32")
         key = (embed.data_ptr(), embed._version, embed.device)
-        if self._operands is None or self._operands_key != key:
+        # a learnable codebook is written by the caller's optimizer, and not every optimizer step bumps `embed._version` (the
+        # fused Adam kernels do not): its operands are rebuilt for every search
+        if self._operands is None or self._operands_key != key or embed.requires_grad:
             reuse = self._operands if (self._operands is not None and self._operands.planes.device == embed.device) else None
-            self._operands = ops.prepare_codebook(embed[self._slot], self.use_cosine_sim, out=reuse)
+            self._operands = ops.prepare_codebook(embed.detach()[self._slot], self.use_cosine_sim, out=reuse)
             self._operands_key = key
         return self._operands
 
     def _mark_operands_fresh(self):
         e = self.embed
         self._operands_key = (e.data_ptr(), e._version, e.device)
+
+    def learns(self) -> bool:
+        """True when this forward must carry a gradient to `embed` (learnable codebook, grad enabled)."""
+        return torch.is_grad_enabled() and self.embed.requires_grad
+
+    def decode(self, indices: torch.Tensor) -> torch.Tensor:
+        """embed[slot][indices] (int64, -1 -> zeros) in fp32, shape indices.shape + (D,): the vqb_decode gather, differentiable
+        w.r.t. a learnable `embed` like the reference's gather from the parameter (vqp:998-1018)."""
+        codes = ops.decode(self.embed.detach()[self._slot], indices.unsqueeze(-1).contiguous())
+        if self.learns():
+            idx = indices.reshape(-1)
+            codes, _ = _LearnableCodebook.apply(self.embed, codes, None, idx.clamp_min(0).to(torch.int32).contiguous(), None, 0.,
+                                                idx >= 0)
+        return codes
 
     # ------------------------------------------------------------------ reference surface
     def transform_input(self, t):  # vqp:376
@@ -336,7 +394,7 @@ class Codebook(nn.Module):
     def quantize_rows(self, x: torch.Tensor, *, update: bool, q_out=None, idx64_out=None, idx_stride=1, loss_out=None,
                       loss_weight=1.0, resid_out=None, stats_out=None, defer_ema=False, margin=None,
                       ema_update=None, ema_update_weight=None, accum_ema_update=False,
-                      row_mask=None, n_live=None):
+                      row_mask=None, n_live=None, on_stats=None):
         """x (N, D) contiguous fp32/bf16 — the input BEFORE the cosine l2norm (done in-kernel).
 
         One C call: search (pre-update codebook, vqp:743-747) with the fused gather / loss / residual tail
@@ -344,6 +402,8 @@ class Codebook(nn.Module):
         With defer_ema (or when the statistics must be all-reduced first) the EMA apply is left to the caller.
         row_mask (N,) uint8 + n_live (1,) int64: in-kernel padding mask (vqp:1116-1119; ops.vq_forward_args) — the caller has made
         sure that neither k-means init nor dead-code expiry (both sample from `x[mask]`) can run in this call.
+        on_stats: called with this batch's statistics [count | sum of rows] right after the search, before any all-reduce or
+        codebook change (the commitment gradient of a learnable codebook); the search then always produces them.
         Returns (idx32, stats or None).
         """
         if not self._initted_host:
@@ -352,11 +412,11 @@ class Codebook(nn.Module):
         ema_update = self.ema_update if ema_update is None else ema_update   # per-call override (vqp:628)
         custom = ema_update_weight is not None or accum_ema_update or any(
             b.grad is not None for b in (self.cluster_size, self.embed_avg))
-        apply_here = update and not defer_ema and not self.use_ddp and not custom
-        mode = 0 if not update else (2 if apply_here else 1)
+        apply_here = update and not defer_ema and not self.use_ddp and not custom and on_stats is None
+        mode = 0 if not (update or on_stats is not None) else (2 if apply_here else 1)
         normalise = ema_update and not self.manual_ema_update
         peer = peer_ptrs = None
-        if update and not defer_ema and self.use_ddp and not custom and stats_out is None:
+        if update and not defer_ema and self.use_ddp and not custom and stats_out is None and on_stats is None:
             peer = self.peer_reducer()
             if peer is not None:   # multi-GPU step in ONE chain: statistics -> peer barrier -> reduce + EMA (vq_peer.cu)
                 mode = 3
@@ -368,6 +428,8 @@ class Codebook(nn.Module):
             peer=peer, peer_ptrs=peer_ptrs, row_mask=row_mask, n_live=n_live)
         if mode >= 2 and normalise:
             self._mark_operands_fresh()
+        if on_stats is not None:
+            on_stats(stats)
         if update and not defer_ema:
             applied = True
             if mode == 1:
@@ -402,7 +464,7 @@ class Codebook(nn.Module):
         if not self._initted_host:
             self.init_embed_(flat.float())   # vqp:703
         cb = self.operands()
-        embed2d = self.embed[self._slot]
+        embed2d = self.embed.detach()[self._slot]
         with torch.no_grad():
             res = ops.search(flat, cb, embed2d, normalise=False)  # the caller already applied transform_input
             q = torch.empty((flat.shape[0], shape[-1]), dtype=torch.float32, device=flat.device)
@@ -415,6 +477,8 @@ class Codebook(nn.Module):
                 if self.lerp_stats(stats, normalise=ema_update and not self.manual_ema_update,
                                    ema_update_weight=ema_update_weight, accum_ema_update=accum_ema_update):
                     self.expire_codes_(res.x_eff.float())
+        if self.learns():   # vqp:710, :766: `quantize` carries each row's gradient to its code
+            q, _ = _LearnableCodebook.apply(self.embed, q, None, res.idx.clone(), None, 0.)
         return q.reshape(shape), idx64.reshape(shape[:-1]), None
 
 

@@ -507,3 +507,23 @@ def rotate(src: torch.Tensor, tgt: torch.Tensor, grad_out: torch.Tensor | None =
         check(lib.vqb_rotate(_p(s2), _p(t2), _p(g2), s2.shape[0], s2.shape[1], _dtype_code(s2), _p(out), _stream()), "vqb_rotate")
     _count(1)
     return out.reshape(shape)
+
+
+def diveq(x: torch.Tensor, q: torch.Tensor, noise: torch.Tensor, noise_scale: float, grad_out: torch.Tensor | None = None):
+    """DiVeQ estimator (vqp:323-330, vqb_diveq): the forward value x + l2norm(q - x + noise_scale * noise) * ||q - x|| when
+    grad_out is None, else (dx in x.dtype, dq fp32).  x, q, noise, grad_out: (..., D) in one dtype."""
+    _require_cuda(x, q, noise, grad_out)
+    shape = x.shape
+    D = shape[-1]
+    rows = [t.reshape(-1, D).contiguous() if t is not None else None for t in (x, q, noise, grad_out)]
+    assert all(t is None or t.dtype == x.dtype for t in rows)
+    x2, q2, z2, g2 = rows
+    out = torch.empty_like(x2)
+    dq = torch.empty(x2.shape, dtype=torch.float32, device=x2.device) if g2 is not None else None
+    with torch.cuda.device(x2.device):
+        check(lib.vqb_diveq(_p(x2), _p(q2), _p(z2), _p(g2), x2.shape[0], D, _dtype_code(x2), float(noise_scale), _p(out), _p(dq),
+                            _stream()), "vqb_diveq")
+    _count(1)
+    if g2 is None:
+        return out.reshape(shape)
+    return out.reshape(shape), dq.reshape(shape)

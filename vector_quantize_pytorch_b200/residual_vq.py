@@ -20,7 +20,7 @@ from torch import nn
 from . import ops
 from .codebook import _unsupported
 from .dist import allreduce_packed, PeerReducer
-from .vector_quantize import VectorQuantize
+from .vector_quantize import VectorQuantize, directional_reparam
 
 
 class _PlanCache(dict):
@@ -185,8 +185,8 @@ class ResidualVQ(nn.Module):
         super().__init__()
         assert heads == 1, "residual vq is not compatible with multi-headed codes"  # rvq:191
         assert num_quantizers is not None or isinstance(codebook_size, tuple)  # rvq:192
-        if diveq or implicit_neural_codebook:
-            _unsupported("diveq / implicit_neural_codebook")
+        if implicit_neural_codebook:
+            _unsupported("implicit_neural_codebook")
         if (beam_size is not None and beam_size > 1) or (eval_beam_size is not None and eval_beam_size > 1):
             _unsupported("beam search")
         if accept_image_fmap:
@@ -204,6 +204,9 @@ class ResidualVQ(nn.Module):
 
         if shared_codebook:  # rvq:213-217
             vq_kwargs.update(manual_ema_update=True)
+        self.diveq = diveq
+        if diveq:  # rvq:222-232: the codebooks learn from the DiVeQ gradient of quantized_out alone
+            vq_kwargs.update(ema_update=False, learnable_codebook=True, route_gradients_to_input=False, commitment_weight=0.)
 
         codebook_sizes = codebook_size if isinstance(codebook_size, tuple) else (codebook_size,) * num_quantizers
         num_quantizers = len(codebook_sizes) if num_quantizers is None else num_quantizers
@@ -220,7 +223,8 @@ class ResidualVQ(nn.Module):
         self.quantize_dropout_cutoff_index = quantize_dropout_cutoff_index
         self.quantize_dropout_multiple_of = quantize_dropout_multiple_of  # rvq:258
         self.vq_is_ema_updating = self.layers[0].ema_update
-        self.quant_grad_frac = 0.
+        # rvq:268: 1 under DiVeQ; the residual then only feeds the searches, so no gradient flows through it either way
+        self.quant_grad_frac = 1. if diveq else 0.
         self.shared_codebook = shared_codebook
         if shared_codebook:  # rvq:295-306: every layer aliases ONE Codebook
             assert self.uniform_codebook_size
@@ -248,18 +252,14 @@ class ResidualVQ(nn.Module):
 
     def get_codes_from_indices(self, indices):  # rvq:324-376
         indices = self._pad_dropped(indices)
-        if self.uniform_codebook_size:
-            q_idx = indices.reshape(-1, self.num_quantizers)
-            codes = [ops.decode(self.layers[q]._codebook.embed[0], q_idx[:, q:q + 1].contiguous()) for q in range(self.num_quantizers)]
-        else:
-            q_idx = indices.reshape(-1, self.num_quantizers)
-            codes = [ops.decode(self.layers[q]._codebook.embed[0], q_idx[:, q:q + 1].contiguous()) for q in range(self.num_quantizers)]
+        q_idx = indices.reshape(-1, self.num_quantizers)
+        codes = [self.layers[q]._codebook.decode(q_idx[:, q]) for q in range(self.num_quantizers)]
         return torch.stack(codes).reshape(self.num_quantizers, *indices.shape[:-1], self.codebook_dim)
 
     def get_output_from_indices(self, indices):  # rvq:378-382: sum over quantizers in ONE gather kernel
         indices = self._pad_dropped(indices)
-        if self.uniform_codebook_size:
-            out = ops.decode(self.codebooks.contiguous(), indices)
+        if self.uniform_codebook_size and not (torch.is_grad_enabled() and self._codebooks_need_grad()):
+            out = ops.decode(self.codebooks.detach().contiguous(), indices)
         else:
             out = self.get_codes_from_indices(indices).sum(dim=0)
         return self.project_out(out)
@@ -288,9 +288,9 @@ class ResidualVQ(nn.Module):
             return self._forward_masked(x, mask, return_all_codes, freeze_codebook, rand_quantize_dropout_fixed_seed)
         if not _projected:   # _projected: the masked path hands in compacted rows that went through project_in already
             x = self.project_in(x)
-        if x.requires_grad and torch.is_grad_enabled():
-            # gradients (to the input or to project_in, rvq:406) need the per-stage straight-through / rotation glue of
-            # VectorQuantize: take the layered path
+        if torch.is_grad_enabled() and (x.requires_grad or self._codebooks_need_grad()):
+            # gradients (to the input or to project_in, rvq:406, or to learnable codebooks) need the per-stage
+            # straight-through / rotation / codebook-gradient glue of VectorQuantize: take the layered path
             return self._forward_layered(x, freeze_codebook, return_all_codes,
                                          self._active_layers(rand_quantize_dropout_fixed_seed, x.device))
         shape, dtype = x.shape, x.dtype
@@ -322,7 +322,10 @@ class ResidualVQ(nn.Module):
             prog, part = plan
             bound = part.bind(prog.arr, flat)
             prog.run()
-            return part.finish(bound, shape, return_all_codes)
+            if not self.diveq:
+                return part.finish(bound, shape, return_all_codes)
+            out, *rest = part.finish(bound, shape, return_all_codes, project=False)
+            return (self.project_out(directional_reparam(x, out)), *rest)   # rvq:603-606, in every mode
 
         if n_run < Q:   # rvq:473-476: the skipped layers report index -1 and loss 0
             all_idx = torch.full((N, Q), -1, dtype=torch.int64, device=dev)
@@ -386,6 +389,8 @@ class ResidualVQ(nn.Module):
                 self._finish_update(packed, offs, stat_sizes, do_update, (stage_inputs, shape, peer_ptrs), synced=False)
 
         quantized_out = quantized_out.reshape(shape)
+        if self.diveq:   # rvq:603-606, in every mode
+            quantized_out = directional_reparam(x, quantized_out)
         if not _projected:
             quantized_out = self.project_out(quantized_out)  # rvq:610
         ret = (quantized_out, all_idx.reshape(*shape[:-1], Q), losses.clone())
@@ -418,6 +423,8 @@ class ResidualVQ(nn.Module):
         with zeros / -1 scattered around it — which is what runs here (stage-wise path: the compacted row count changes from call
         to call, a cached program per count would not pay).  project_in / project_out see every row (rvq:406, :610)."""
         books = self._stage_plan()
+        if any(b.learnable_codebook for b in books):
+            _unsupported("ResidualVQ.forward(mask=) with learnable codebooks")
         if any(b.use_cosine_sim for b in books):
             _unsupported("ResidualVQ.forward(mask=) with use_cosine_sim (the masked loss is taken against the un-normalised input, vqp:1319)")
         if any(not vq.return_zeros_for_masked_padding for vq in self.layers):
@@ -445,6 +452,9 @@ class ResidualVQ(nn.Module):
         if return_all_codes:
             ret = (*ret, self.get_codes_from_indices(ret[1]))
         return ret
+
+    def _codebooks_need_grad(self):
+        return any(vq._codebook.embed.requires_grad for vq in self.layers)
 
     def _program_ok(self, books, do_update):
         """One-call path (ops.RvqProgram): every stage deferred, no collective, no dead-code expiry, nothing parked on `.grad`
@@ -543,6 +553,8 @@ class ResidualVQ(nn.Module):
             all_losses.append(loss)
         if self.training and self.shared_codebook and self.vq_is_ema_updating and not freeze_codebook:
             self.layers[0]._codebook.update_ema()
+        if self.diveq:   # rvq:603-606: every stage's codebook gets the DiVeQ gradient of quantized_out
+            quantized_out = directional_reparam(x, quantized_out)
         ret = (self.project_out(quantized_out), torch.stack(all_idx, dim=-1), torch.stack(all_losses))
         if return_all_codes:
             ret = (*ret, self.get_codes_from_indices(ret[1]))
@@ -576,7 +588,9 @@ class GroupedResidualVQ(nn.Module):
 
     def _program_ok(self, chunks, freeze_codebook):
         """All groups in one ops.RvqProgram: every group qualifies (ResidualVQ._program_ok), no gradient path, and the op list fits."""
-        if torch.is_grad_enabled() and any(c.requires_grad for c in chunks):
+        if torch.is_grad_enabled() and (any(c.requires_grad for c in chunks) or any(r._codebooks_need_grad() for r in self.rvqs)):
+            return False
+        if any(rvq.diveq for rvq in self.rvqs):
             return False
         total = 0
         for rvq, c in zip(self.rvqs, chunks):

@@ -7,6 +7,7 @@ loss and EMA run in the sm_90a kernels.  Unsupported constructor / forward optio
 """
 from __future__ import annotations
 
+import math
 from collections import namedtuple
 
 import torch
@@ -14,7 +15,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
-from .codebook import Codebook, _unsupported
+from .codebook import Codebook, _LearnableCodebook, _unsupported
 
 LossBreakdown = namedtuple("LossBreakdown", ["commitment", "codebook_diversity", "orthogonal_reg", "inplace_optimize"])
 
@@ -50,6 +51,34 @@ class _RotateTo(torch.autograd.Function):
 
 def rotate_to(src, tgt):
     return _RotateTo.apply(src, tgt)
+
+
+def diveq_noise(like):
+    """The N(0, 1) draw of DiVeQ (`torch.randn_like(error_dir)`, vqp:327), in `like`'s shape and dtype.  Every DiVeQ forward
+    of this package draws through this one function."""
+    return torch.randn_like(like)
+
+
+class _DiVeQ(torch.autograd.Function):
+    """DiVeQ estimator (vqp:323-330) on the vqb_diveq kernel: x + l2norm(q - x + s z) ||q - x|| with the direction detached.
+    The backward recomputes the row scalars from (x, q, z)."""
+
+    @staticmethod
+    def forward(ctx, src, tgt, noise, scale):
+        ctx.save_for_backward(src, tgt, noise)
+        ctx.scale = scale
+        return ops.diveq(src.detach(), tgt.detach(), noise, scale)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        src, tgt, noise = ctx.saved_tensors
+        dx, dq = ops.diveq(src.detach(), tgt.detach(), noise, ctx.scale, grad_out.to(src.dtype))
+        return dx, dq.to(tgt.dtype), None, None
+
+
+def directional_reparam(src, tgt, noise_variance=5e-3):
+    """vqp:323-330; src and tgt in one dtype (the noise is drawn in it, after the codebook forward like the reference's)."""
+    return _DiVeQ.apply(src, tgt, diveq_noise(tgt), math.sqrt(noise_variance))
 
 
 def host_chunk_bounds(N: int, n_chunks: int):
@@ -122,8 +151,8 @@ class VectorQuantize(nn.Module):
         super().__init__()
         # ---- options outside the accelerated path fail loudly
 
-        if directional_reparam or vq_bridge is not None or learnable_codebook:
-            _unsupported("directional_reparam / vq_bridge / learnable_codebook")
+        if vq_bridge is not None:
+            _unsupported("vq_bridge")
         if in_place_codebook_optimizer is not None:
             _unsupported("in_place_codebook_optimizer")
         if affine_param:
@@ -132,13 +161,22 @@ class VectorQuantize(nn.Module):
             _unsupported("stochastic_sample_codes / gumbel straight_through")
         if commitment_use_cross_entropy_loss or orthogonal_reg_weight > 0 or codebook_diversity_loss_weight > 0:
             _unsupported("cross-entropy / orthogonal / diversity losses (they need the N x K distance matrix)")
-        if sync_update_v > 0:
-            _unsupported("sync_update_v")
-        ema_update = True if ema_update is None else ema_update  # vqp:854
-        if not ema_update:
-            # a frozen, non-learnable codebook is still a valid use of the search kernels
-            pass
-        rotation_trick = (dim > 1) if rotation_trick is None else rotation_trick  # vqp:856
+        ema_update = (not directional_reparam) if ema_update is None else ema_update  # vqp:854
+        learnable_codebook = directional_reparam if learnable_codebook is None else bool(learnable_codebook)  # vqp:855
+        rotation_trick = (not directional_reparam and dim > 1) if rotation_trick is None else rotation_trick  # vqp:856
+        # combinations the reference rejects (vqp:884, :908, :913)
+        if learnable_codebook and ema_update:
+            _unsupported("learnable_codebook together with ema_update")
+        if learnable_codebook and use_cosine_sim:
+            _unsupported("learnable_codebook together with use_cosine_sim")
+        if sync_update_v > 0 and not learnable_codebook:
+            _unsupported("sync_update_v without learnable_codebook")
+        if learnable_codebook and separate_codebook_per_head and heads > 1:
+            _unsupported("learnable_codebook with separate_codebook_per_head")
+        assert 0 <= sync_update_v <= 1.  # vqp:912
+        assert not (rotation_trick and directional_reparam)  # vqp:898
+        assert not (directional_reparam and threshold_ema_dead_code == 0), \
+            "periodic dead code replacement should be enabled when differential reparam method is turned on"  # vqp:901
 
         self.dim = dim
         self.heads = heads
@@ -158,10 +196,13 @@ class VectorQuantize(nn.Module):
         self.has_projections = requires_projection
 
         self.eps = eps
-        self.has_commitment_loss = commitment_weight > 0.
+        self.has_commitment_loss = commitment_weight > 0. and not directional_reparam  # vqp:880
         self.commitment_weight = commitment_weight
-        self.learnable_codebook = False
+        self.learnable_codebook = learnable_codebook
         self.rotation_trick = rotation_trick
+        self.directional_reparam = directional_reparam
+        self.directional_reparam_variance = directional_reparam_variance
+        self.sync_update_v = sync_update_v
         self.route_gradients_to_input = route_gradients_to_input
 
         if sync_codebook is None:  # vqp:925-926
@@ -183,6 +224,7 @@ class VectorQuantize(nn.Module):
             ema_update=ema_update,
             manual_ema_update=manual_ema_update,
             use_cosine_sim=use_cosine_sim,
+            learnable_codebook=learnable_codebook,
         )
         self.codebook_size = codebook_size
         self.accept_image_fmap = accept_image_fmap
@@ -204,6 +246,7 @@ class VectorQuantize(nn.Module):
         return self._codebook.embed[0]
 
     @codebook.setter
+    @torch.no_grad()
     def codebook(self, codes):  # vqp:991-996
         self._codebook.embed.copy_(codes if self.separate_codebook_per_head else codes.unsqueeze(0))
 
@@ -211,7 +254,7 @@ class VectorQuantize(nn.Module):
         if self.separate_codebook_per_head:   # 'b * h' indices -> every head gathers from its own codebook -> 'b * (h d)'
             codes = torch.cat([ops.decode(self._codebook.embed[h], indices[..., h:h + 1].contiguous()) for h in range(self.heads)], dim=-1)
         else:
-            codes = ops.decode(self.codebook, indices.unsqueeze(-1))
+            codes = self._codebook.decode(indices)
         if not self.channel_last or self.accept_image_fmap or self.accept_3d_fmap:
             codes = codes.movedim(-1, 1)
         return codes
@@ -504,6 +547,8 @@ class VectorQuantize(nn.Module):
         if lens is not None:  # vqp:1118-1119, :99-101
             mask = torch.arange(x.shape[1], device=lens.device) < lens[:, None]
         if mask is not None:
+            if self.learnable_codebook:
+                _unsupported("mask / lens with a learnable codebook")
             return self._forward_masked(x, mask, freeze_codebook, ema_update, return_loss_breakdown)
         if topk is not None or codebook_transform_fn is not None:
             _unsupported("topk / codebook_transform_fn")
@@ -545,9 +590,20 @@ class VectorQuantize(nn.Module):
         loss_buf = self._loss_scratch(flat.device) if fused_loss else None
         # LossBreakdown.commitment is the UNweighted mse (vqp:1327-1329): ask the kernel for weight 1 then
         split_weight = fused_loss and return_loss_breakdown and self.commitment_weight != 1.
-        cbk.quantize_rows(flat, update=do_update, q_out=q, idx64_out=idx64, loss_out=loss_buf,
-                          loss_weight=1. if split_weight else self.commitment_weight, ema_update=ema_update,
-                          ema_update_weight=ema_update_weight, accum_ema_update=accum_ema_update)
+        # a learnable codebook (vqp:710) gets the gradient of `quantize` and, in training, of the commitment loss (vqp:1214-1216)
+        learn = cbk.learns()
+        commit_grad = learn and training and self.has_commitment_loss and not freeze_codebook
+        commit_rows = []
+
+        def take_commit_rows(stats):   # count_k c_k - sum_{n -> k} x_n, with the codebook the rows were searched in
+            # the reference differentiates mse(quantize.type(dtype), x) (vqp:1178, :1327): the code as rounded to x's dtype
+            count, sums = cbk._stat_views(stats)
+            commit_rows.append(count[0, :, None] * cbk.embed.detach()[0].to(dtype).float() - sums[0])
+
+        idx32, _ = cbk.quantize_rows(flat, update=do_update, q_out=q, idx64_out=idx64, loss_out=loss_buf,
+                                     loss_weight=1. if split_weight else self.commitment_weight, ema_update=ema_update,
+                                     ema_update_weight=ema_update_weight, accum_ema_update=accum_ema_update,
+                                     on_stats=take_commit_rows if commit_grad else None)
         commit_loss = loss_buf.clone().reshape(()) if fused_loss else self.zero
         weighted = commit_loss
         if split_weight:  # commit_loss * weight in the input dtype, promoted by the fp32 accumulator (vqp:1329, :1282)
@@ -561,17 +617,32 @@ class VectorQuantize(nn.Module):
             loss = weighted.requires_grad_(torch.is_grad_enabled())
         else:
             loss = torch.tensor(0., device=flat.device, requires_grad=training and torch.is_grad_enabled())  # vqp:1282
+        if training and self.has_commitment_loss and not fused_loss:
+            # differentiable w.r.t. the input: PyTorch glue on the kernel's outputs
+            commit_loss = F.mse_loss(quantize.detach(), cbk.transform_input(x))
+        if learn:
+            idx32 = idx32.clone()   # the search's index buffer is reused by the next forward
+            if not commit_rows:
+                quantize, _ = _LearnableCodebook.apply(cbk.embed, quantize, None, idx32, None, 0.)
+            elif fused_loss:   # `loss` is already weight * mse
+                quantize, loss = _LearnableCodebook.apply(cbk.embed, quantize, loss, idx32, commit_rows[0],
+                                                          2. * self.commitment_weight / flat.numel())
+            else:
+                quantize, commit_loss = _LearnableCodebook.apply(cbk.embed, quantize, commit_loss, idx32, commit_rows[0],
+                                                                 2. / flat.numel())
         if training:
-            if self.has_commitment_loss:
-                if fused_loss:
-                    pass
-                else:  # differentiable w.r.t. the input: PyTorch glue on the kernel's outputs
-                    x_t = cbk.transform_input(x)
-                    commit_loss = F.mse_loss(quantize.detach(), x_t)
-                    loss = loss + commit_loss * self.commitment_weight
+            if self.has_commitment_loss and not fused_loss:
+                loss = loss + commit_loss * self.commitment_weight
             if input_requires_grad and self.route_gradients_to_input:  # vqp:1225-1233
                 x_t = cbk.transform_input(x)
-                quantize = rotate_to(x_t, quantize) if self.rotation_trick else straight_through(x_t, quantize)
+                if self.rotation_trick:
+                    quantize = rotate_to(x_t, quantize)
+                elif self.directional_reparam:
+                    quantize = directional_reparam(x_t, quantize, self.directional_reparam_variance)
+                else:
+                    quantize = straight_through(x_t, quantize)
+            if self.sync_update_v > 0.:  # vqp:1235-1237
+                quantize = quantize + self.sync_update_v * (quantize - quantize.detach())
 
         if heads > 1:  # vqp:1354-1358 '1 (b h) n d -> b n (h d)', :1266-1270 '1 (b h) n -> b n h'
             n = quantize.shape[1]
