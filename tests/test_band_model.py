@@ -99,13 +99,55 @@ def split_bf16(a):
     return hi, lo
 
 
+FLOOR = 1e-8   # the band's clamp-floor term (Euclid): the reference's d^2 clamp, vqp:58-62
+
+
 def kernel_band(x2, xlo_norm, cmax, cres, caux, euclid):
     """W of vq_assign.cu (`sc.init`), float64 evaluation."""
     xn = np.sqrt(x2)
     xc = xn * cmax
     e = 1.0 if euclid else 0.0
     return (2.0 * (xn * cres + xlo_norm * caux + MARGIN * xc + e * 2.0 ** -21 * cmax * cmax)
-            + 2.0 ** -18 * (xc + e * 0.5 * cmax * cmax) + e * 2.0 ** -22 * (x2 + cmax * cmax))
+            + 2.0 ** -18 * (xc + e * 0.5 * cmax * cmax) + e * (2.0 ** -22 * (x2 + cmax * cmax) + FLOOR))
+
+
+def _floor_case(kind, rng):
+    """(rows, codebook) of the clamp-floor regime.  The reference clamps d^2 at 1e-8, so every code within 1e-4 of a row
+    scores exactly -1e-4 and the LOWEST such index wins, even when a higher index is strictly closer."""
+    K, D = 1024, 256
+    if kind == "zero_rows":   # a ResidualVQ stage after an exact match: zero residuals, two codes of norm below 1e-4
+        e = (rng.standard_normal((K, D)) * 3e-3 / np.sqrt(D)).astype(np.float32)
+        e[1] = (rng.standard_normal(D) * 5e-5 / np.sqrt(D)).astype(np.float32)
+        e[3] = (rng.standard_normal(D) * 1e-6 / np.sqrt(D)).astype(np.float32)
+        return np.zeros((8, D), np.float32), e
+    scale = {"pair_3e-3": 3e-3, "pair_1e-2": 1e-2}[kind]   # small-norm codebook, a pair 5e-5 apart, rows on the higher index
+    e = (rng.standard_normal((K, D)) * scale / np.sqrt(D)).astype(np.float32)
+    e[700] = e[5] + (rng.standard_normal(D) * 5e-5 / np.sqrt(D)).astype(np.float32)
+    x = (e[700] + rng.standard_normal((64, D)) * 1e-6 / np.sqrt(D)).astype(np.float32)
+    return x, e
+
+
+@pytest.mark.parametrize("kind", ["zero_rows", "pair_3e-3", "pair_1e-2"])
+def test_clamp_floor_departures_lie_inside_the_band(kind):
+    """At the clamp floor the reference's winner departs from the exact arg-max on every row of these cases (the departure
+    is asserted, so the case keeps testing the floor); the exact score gap between the two must still lie inside W, or
+    the kernel would certify the exact winner instead of the reference's.  Without the band's FLOOR term the zero rows
+    (gap ~30 W) and the pair at max||c|| ~ 3e-3 (~5 W) would be certified with the exact winner; at ~1e-2 the norm-scaled
+    terms alone still cover the floor."""
+    x, e = _floor_case(kind, np.random.default_rng(1))
+    ref = O.argmax_first(O.neg_cdist(x, e))
+    x64, e64 = x.astype(np.float64), e.astype(np.float64)
+    s = x64 @ e64.T - 0.5 * (e64 * e64).sum(-1)[None]
+    best = s.argmax(-1)
+    assert (ref != best).all() and (ref < best).all()
+    ar = np.arange(len(x))
+    gap = s[ar, best] - s[ar, ref]
+    x2 = (x64 * x64).sum(-1)
+    cmax = float(np.sqrt((e64 * e64).sum(-1).max()))
+    c_hi, c_lo = split_bf16(e)
+    cres = float(np.sqrt(((e64 - c_hi.astype(np.float64) - c_lo.astype(np.float64)) ** 2).sum(-1)).max())
+    W = kernel_band(x2, np.zeros_like(x2), cmax, cres, 0.0, True)   # bf16 rows: no x_lo term
+    assert (gap * 1.5 <= W).all(), f"worst gap / W = {np.max(gap / W):.3f}"
 
 
 @pytest.mark.parametrize("dtype", ["bf16", "fp32"])

@@ -17,9 +17,10 @@
 //
 // Exactness: the tensor-core score of a (row, code) pair differs from the exact fp32 value by at most
 // tau = margin_rel * ||x|| * max||c||, and the epilogue's 4-bit column tag perturbs it by < 16 ulp.  A row is
-// certified when its best (tagged) score leads every other score by more than W = 2*tau + 2*(tag slack);
+// certified when its best (tagged) score leads every other score by more than W = 2*tau + 2*(tag slack) + the widths
+// over which the reference's own fp32 formula ties distinct codes (its sqrt collapse and, Euclid, its 1e-8 clamp floor);
 // otherwise (row, two best candidates, candidate count) goes to `flagged` and vqb_fix_flagged re-scores it with
-// the reference's exact formula (count >= 3: whole-row rescan).  Conservative: may over-flag, never under-flag.
+// the reference's exact formula (count > 3: whole-row rescan).  Conservative: may over-flag, never under-flag.
 #include "ptx.cuh"
 #include "vqb_common.cuh"
 #include "gather_row.cuh"
@@ -445,12 +446,17 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             // 2 * |score error|: what the passes leave out of the codebook (||x|| * cres) and of the row (xaux * caux), both by
             // Cauchy-Schwarz on exact norms; the fp32 accumulation in the tensor core (margin_rel relative to ||x|| max||c||,
             // 2^-20 relative to the bias the bias MMA sums); then the tag slack and the sqrt-collapse width.
+            // Last (Euclid), the clamp floor: the reference clamps d^2 at 1e-8 before the sqrt (vqp:58-62), so every code with
+            // fp32 d^2 <= 1e-8 scores -1e-4 and the lowest such index wins, although their exact scores differ by up to
+            // (1e-8 + the d^2 rounding) / 2.  The norm-scaled terms above are narrower than that once ||x|| and max||c|| fall
+            // to ~1e-2 (late ResidualVQ stages, zero residuals); 1e-8 keeps those codes inside the band, and the band of a
+            // normal-norm codebook (~1e-5 and up) does not notice it.
             const float xn = sqrtf(x2[h]);
             const float xc = xn * cmax;
             xlo[h] = p.n_a == 2 ? sqrtf(xlo[h]) * 1.0001f : 0.f;
             sc[h].init(2.f * (xn * cres + xlo[h] * caux + p.margin_rel * xc + (euclid ? 0x1p-21f * cmax * cmax : 0.f)) +
                        0x1p-18f * (xc + (euclid ? 0.5f * cmax * cmax : 0.f)) +
-                       (euclid ? 0x1p-22f * (x2[h] + cmax * cmax) : 0.f) + 1e-30f);
+                       (euclid ? 0x1p-22f * (x2[h] + cmax * cmax) + 1e-8f : 1e-30f));
           }
         } else {
 #pragma unroll
