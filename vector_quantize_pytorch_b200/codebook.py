@@ -277,6 +277,22 @@ class Codebook(nn.Module):
             self._mark_operands_fresh()
         return True
 
+    def updates(self, training: bool, freeze_codebook: bool, ema_update=None) -> bool:
+        """Whether a forward changes this codebook: in training, not frozen, with an EMA update or dead-code replacement to do
+        (vqp:628-641).  `ema_update` None: the module's setting."""
+        ema_update = self.ema_update if ema_update is None else ema_update
+        return training and not freeze_codebook and (ema_update or self.has_dead_code_replacement)
+
+    def apply_stats(self, stats: torch.Tensor, samples, ema_update=None, ema_update_weight=None, accum_ema_update: bool = False):
+        """One EMA step from a batch's packed statistics: all-reduce, lerp (`lerp_stats`), then dead-code expiry (vqp:641) unless
+        the statistics were only parked by `accum_ema_update`.  `samples()` gives expiry its rows; it is called only when codes
+        can expire, so the fp32 copy of the batch is made only then."""
+        ema_update = self.ema_update if ema_update is None else ema_update
+        self.sync_stats(stats)
+        if (self.lerp_stats(stats, normalise=ema_update and not self.manual_ema_update, ema_update_weight=ema_update_weight,
+                            accum_ema_update=accum_ema_update) and self.has_dead_code_replacement):
+            self.expire_codes_(samples())
+
     def update_ema(self):  # vqp:576-584
         cs, ea, emb = self._state2d()
         cb = self.operands()
@@ -363,10 +379,8 @@ class Codebook(nn.Module):
             flat = flat.float()
         flat = flat.contiguous()
         idx = embed_ind.reshape(-1).to(torch.int32).clamp_min(0).contiguous()
-        stats = self.sync_stats(ops.ema_stats(flat, idx, self.codebook_size))
-        if self.lerp_stats(stats, normalise=ema_update and not self.manual_ema_update,
-                           ema_update_weight=ema_update_weight, accum_ema_update=accum_ema_update):
-            self.expire_codes_(flat.float())
+        self.apply_stats(ops.ema_stats(flat, idx, self.codebook_size), flat.float, ema_update, ema_update_weight,
+                         accum_ema_update)
 
     @torch.no_grad()
     def update_codebook(self, flatten, embed_onehot, mask=None, ema_update_weight=None, accum_ema_update=False,
@@ -431,12 +445,10 @@ class Codebook(nn.Module):
         if on_stats is not None:
             on_stats(stats)
         if update and not defer_ema:
-            applied = True
             if mode == 1:
-                self.sync_stats(stats)
-                applied = self.lerp_stats(stats, normalise=normalise, ema_update_weight=ema_update_weight,
-                                          accum_ema_update=accum_ema_update)
-            if applied and self.has_dead_code_replacement:
+                self.apply_stats(stats, lambda: self.transform_input(x).float(), ema_update, ema_update_weight,
+                                 accum_ema_update)
+            elif self.has_dead_code_replacement:
                 self.expire_codes_(self.transform_input(x).float())  # vqp:692: `flatten` is fp32
         return idx32, stats
 
@@ -455,7 +467,6 @@ class Codebook(nn.Module):
             _unsupported("topk")
         if self.num_codebooks > 1 and self._head_views is None and self._slot == 0 and x.ndim == 4:
             _unsupported("Codebook.forward on (h, b, n, d) inputs: go through VectorQuantize(separate_codebook_per_head=True)")
-        ema_update = self.ema_update if ema_update is None else ema_update
         shape = x.shape
         flat = x.reshape(-1, shape[-1])
         if flat.dtype not in (torch.float32, torch.bfloat16):
@@ -471,12 +482,9 @@ class Codebook(nn.Module):
             idx64 = torch.empty((flat.shape[0],), dtype=torch.int64, device=flat.device)
             x32 = res.x_eff if res.x_eff.dtype == torch.float32 else res.x_eff.float()
             ops.gather(x32, embed2d, res.idx, q_out=q, idx64_out=idx64)
-            do_update = self.training and update_usage and not freeze_codebook and (ema_update or self.has_dead_code_replacement)
-            if do_update:
-                stats = self.sync_stats(ops.ema_stats(res.x_eff, res.idx, self.codebook_size))
-                if self.lerp_stats(stats, normalise=ema_update and not self.manual_ema_update,
-                                   ema_update_weight=ema_update_weight, accum_ema_update=accum_ema_update):
-                    self.expire_codes_(res.x_eff.float())
+            if self.updates(self.training and update_usage, freeze_codebook, ema_update):
+                self.apply_stats(ops.ema_stats(res.x_eff, res.idx, self.codebook_size), res.x_eff.float, ema_update,
+                                 ema_update_weight, accum_ema_update)
         if self.learns():   # vqp:710, :766: `quantize` carries each row's gradient to its code
             q, _ = _LearnableCodebook.apply(self.embed, q, None, res.idx.clone(), None, 0.)
         return q.reshape(shape), idx64.reshape(shape[:-1]), None

@@ -305,8 +305,7 @@ class ResidualVQ(nn.Module):
 
         losses = self._ensure_loss_buf(dev)
         n_run = self._active_layers(rand_quantize_dropout_fixed_seed, dev)   # < Q: quantize dropout skips the layers after it
-        do_update = [training and not freeze_codebook and q < n_run and (b.ema_update or b.has_dead_code_replacement)
-                     for q, b in enumerate(books)]
+        do_update = [q < n_run and b.updates(training, freeze_codebook) for q, b in enumerate(books)]
         if not _projected and n_run == Q and self._program_ok(books, do_update):
             # the whole forward — stages, running sum, deferred EMA updates — as ONE vqb_rvq_forward call / one CUDA graph,
             # from a cached op list in which only the per-call pointers (input, indices, output) are patched
@@ -599,7 +598,7 @@ class GroupedResidualVQ(nn.Module):
             if torch.is_grad_enabled() and any(p.requires_grad for p in rvq.project_in.parameters()):
                 return False
             books = rvq._stage_plan()
-            upd = [rvq.training and not freeze_codebook and (b.ema_update or b.has_dead_code_replacement) for b in books]
+            upd = [b.updates(rvq.training, freeze_codebook) for b in books]
             if not rvq._program_ok(books, upd):
                 return False
             total += len(books) + 1 + sum(upd) + 2
@@ -631,7 +630,7 @@ class GroupedResidualVQ(nn.Module):
                 xin = rvq.project_in(c).detach()
                 flat = xin.reshape(-1, xin.shape[-1])     # a strided view of the group's columns: copied into the plan's buffer
                 books = rvq._stage_plan()
-                upd = [rvq.training and not freeze_codebook and (b.ema_update or b.has_dead_code_replacement) for b in books]
+                upd = [b.updates(rvq.training, freeze_codebook) for b in books]
                 rvq._ensure_loss_buf(flat.device)
                 flats.append((flat, xin.shape, books, upd))
                 keys.append(rvq._part_key(flat, books, upd))

@@ -277,10 +277,12 @@ class VectorQuantize(nn.Module):
 
     update_ema_indices = update_indices
 
-    def _loss_scratch(self, device):
+    def _loss_scratch(self, device, n=1):
+        """The persistent (n,) buffer the kernels write the commitment loss to (stable pointers for the graph cache); callers
+        get a copy."""
         buf = getattr(self, "_loss_buf", None)
-        if buf is None or buf.device != device:
-            buf = torch.zeros((1,), dtype=torch.float32, device=device)
+        if buf is None or buf.device != device or buf.numel() != n:
+            buf = torch.zeros((n,), dtype=torch.float32, device=device)
             self._loss_buf = buf
         return buf
 
@@ -326,7 +328,7 @@ class VectorQuantize(nn.Module):
         xf = x_host.reshape(-1, D)
         N = xf.shape[0]
         training = self.training
-        do_update = training and not self.freeze_codebook and (cbk.ema_update or cbk.has_dead_code_replacement)
+        do_update = cbk.updates(training, self.freeze_codebook)
         want_loss = training and self.has_commitment_loss
         if out is None:
             out = (torch.empty(shape, dtype=x_host.dtype).pin_memory(), torch.empty(shape[:-1], dtype=torch.int64).pin_memory(),
@@ -376,11 +378,8 @@ class VectorQuantize(nn.Module):
                 down.wait_event(e)
                 qf[r0:r1].copy_(st["q"][r0:r1], non_blocking=True)
                 idf[r0:r1].copy_(st["i"][r0:r1], non_blocking=True)
-        if do_update:
-            cbk.sync_stats(st["stats"])
-            cbk.lerp_stats(st["stats"], normalise=cbk.ema_update and not cbk.manual_ema_update)
-            if cbk.has_dead_code_replacement:   # vqp:641, over the whole batch (resident in st["x"])
-                cbk.expire_codes_(cbk.transform_input(st["x"]).float())
+        if do_update:   # dead-code expiry samples the whole batch, resident in st["x"] (vqp:641)
+            cbk.apply_stats(st["stats"], lambda: cbk.transform_input(st["x"]).float())
         if want_loss:
             w = torch.tensor(weights, dtype=torch.float32, device=dev)
             loss = (st["loss"][:n_chunks] * w).sum()
@@ -392,99 +391,42 @@ class VectorQuantize(nn.Module):
         cur.wait_stream(down)
         return q_host, i_host, l_host
 
-    # ------------------------------------------------------------------ variable-length sequences (vqp:599-600, :1317-1325, :1378-1396)
-    def _forward_masked(self, x, mask, freeze_codebook, ema_update, return_loss_breakdown):
-        """mask (B, N) bool.  Masked positions take no part in the statistics or the loss (the reference zeroes their one-hot
-        rows, vqp:599-600, and averages the loss over the unmasked elements against the ORIGINAL input, vqp:1317-1325) and come
-        back as zeros / index -1.  Euclidean codebooks: the search kernel takes the mask (row_mask of vqb_vq_forward).  Cosine
-        codebooks, pending k-means init, dead-code expiry: the kernels run on the compacted unmasked rows."""
-        if self.has_projections or self.accept_image_fmap or self.accept_3d_fmap or not self.channel_last or self.heads > 1:
-            _unsupported("mask / lens together with projections, feature-map layouts or heads > 1")
-        if x.requires_grad and torch.is_grad_enabled():
-            _unsupported("mask / lens on inputs that require grad")
-        if not x.is_cuda:
-            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
-        assert x.ndim == 3 and mask.shape == x.shape[:2]
-        freeze_codebook = self.freeze_codebook if freeze_codebook is None else freeze_codebook
-        cbk = self._codebook
-        ema_update = cbk.ema_update if ema_update is None else ema_update
-        training = self.training
-        B, N, D = x.shape
-        flat = x.detach().reshape(-1, D)
-        do_update = training and not freeze_codebook and (ema_update or cbk.has_dead_code_replacement)
-        if (not self.use_cosine_sim and cbk._initted_host and x.dtype in (torch.float32, torch.bfloat16)
-                and not (do_update and cbk.has_dead_code_replacement)):
-            # in-kernel mask: every row is searched (like the reference), the merge step of the search kernel drops the padding
-            # rows — index -1, outputs left as pre-filled here, no loss term, no statistics — and the loss is divided by the
-            # unmasked element count on the device: no host sync, no compaction pass.  (Cosine: the masked loss is taken
-            # against the UN-normalised input, vqp:1319; k-means init / expiry sample from x[mask]: those take the path below.)
-            flat = flat.contiguous()
-            row_mask = mask.reshape(-1).contiguous().view(torch.uint8)
-            n_live = row_mask.sum(dtype=torch.int64).reshape(1)
-            quantize = torch.zeros_like(flat) if self.return_zeros_for_masked_padding else flat.clone()
-            embed_ind = torch.full((B * N,), -1, dtype=torch.int64, device=x.device)
-            want_loss = training and self.has_commitment_loss
-            commit = torch.zeros((), dtype=torch.float32, device=x.device) if want_loss else None
-            cbk.quantize_rows(flat, update=do_update, q_out=quantize, idx64_out=embed_ind, loss_out=commit,
-                              loss_weight=self.commitment_weight, ema_update=ema_update, row_mask=row_mask, n_live=n_live)
-            if want_loss:
-                loss = commit.requires_grad_(torch.is_grad_enabled())
-                commit_loss = commit
-            else:
-                loss = torch.tensor(0., device=x.device, requires_grad=training and torch.is_grad_enabled())
-                commit_loss = self.zero
-            quantize, embed_ind = quantize.reshape(B, N, D), embed_ind.reshape(B, N)
-            if not return_loss_breakdown:
-                return quantize, embed_ind, loss
-            return quantize, embed_ind, loss, LossBreakdown(commit_loss, self.zero, self.zero, self.zero)
-        rows = mask.reshape(-1).nonzero(as_tuple=True)[0]  # host sync (the reference's masked path syncs as well)
-        quantize = torch.zeros_like(flat) if self.return_zeros_for_masked_padding else flat.clone()
-        embed_ind = torch.full((B * N,), -1, dtype=torch.int64, device=x.device)
-        loss = torch.tensor(0., device=x.device, requires_grad=training and torch.is_grad_enabled())
-        commit_loss = self.zero
-        if rows.numel() > 0:
-            xc = flat[rows].contiguous()
-            qc = torch.empty_like(xc)
-            ic = torch.empty((xc.shape[0],), dtype=torch.int64, device=x.device)
-            fused = training and self.has_commitment_loss and not self.use_cosine_sim
-            commit = torch.empty((), dtype=torch.float32, device=x.device) if fused else None
-            cbk.quantize_rows(xc, update=do_update, q_out=qc, idx64_out=ic, loss_out=commit,
-                              loss_weight=self.commitment_weight, ema_update=ema_update)
-            quantize[rows] = qc
-            embed_ind[rows] = ic
-            if training and self.has_commitment_loss:
-                if fused:  # euclid: the original input IS what the codebook saw
-                    commit_loss = commit
-                    loss = commit.requires_grad_(torch.is_grad_enabled())
-                else:      # cosine: mse against the un-normalised original input (vqp:1319)
-                    commit_loss = F.mse_loss(qc, xc)
-                    loss = loss + commit_loss * self.commitment_weight
-        quantize = quantize.reshape(B, N, D)
-        embed_ind = embed_ind.reshape(B, N)
-        if not return_loss_breakdown:
-            return quantize, embed_ind, loss
-        return quantize, embed_ind, loss, LossBreakdown(commit_loss, self.zero, self.zero, self.zero)
+    # ------------------------------------------------------------------ the codebook call of each forward variant
+    # Each returns (quantize, embed_ind, commit, glue, learn): the quantized rows and int64 indices in the layout of its input
+    # rows, the kernels' commitment loss (None: taken by the glue below), the glue loss's (quantize, target) when that is not
+    # (quantize, transform_input(x)), and what _LearnableCodebook needs (idx32, commit_rows) for a learnable codebook.
+    def _quantize_shared(self, x, update, ema_update, loss_weight, fused_loss, commit_grad, ema_update_weight, accum_ema_update):
+        """One search over all rows; with shared heads every head's sub-vector is a row (vqp:1044-1049)."""
+        cbk, shape = self._codebook, x.shape
+        flat = x.detach().reshape(-1, shape[-1]).contiguous()
+        q = torch.empty_like(flat)
+        idx64 = torch.empty((flat.shape[0],), dtype=torch.int64, device=flat.device)
+        loss_buf = self._loss_scratch(flat.device) if fused_loss else None
+        # a learnable codebook (vqp:710) gets the gradient of `quantize` and, in training, of the commitment loss (vqp:1214-1216)
+        learns = cbk.learns()
+        commit_rows = []
 
-    def _forward_separate_heads(self, x, restore, only_one, freeze_codebook, ema_update, return_loss_breakdown,
-                                ema_update_weight, accum_ema_update):
-        """separate_codebook_per_head (vqp:1044-1049 'b n (h d) -> h b n d', Codebook(num_codebooks=h), :1266-1268, :1354-1356):
-        head i searches / updates codebook i of the (h, K, d) buffers — h independent chains on the same kernels, in head
-        order (k-means init and dead-code expiry draw from the RNG head by head, like the reference's batched_sample_vectors)."""
-        heads = self.heads
-        b, n, hd = x.shape
-        d = hd // heads
-        dtype = x.dtype
-        if dtype not in (torch.float32, torch.bfloat16):
-            raise TypeError(f"vqb200 supports float32 and bfloat16 inputs, got {dtype}")
-        if accum_ema_update or ema_update_weight is not None:
-            _unsupported("ema_update_weight / accum_ema_update with separate_codebook_per_head")
-        input_requires_grad = x.requires_grad and torch.is_grad_enabled()
-        cbk = self._codebook
-        training = self.training
-        do_update = training and not freeze_codebook and (ema_update or cbk.has_dead_code_replacement)
-        fused_loss = training and self.has_commitment_loss and not input_requires_grad
+        def take_commit_rows(stats):   # count_k c_k - sum_{n -> k} x_n, with the codebook the rows were searched in
+            # the reference differentiates mse(quantize.type(dtype), x) (vqp:1178, :1327): the code as rounded to x's dtype
+            count, sums = cbk._stat_views(stats)
+            commit_rows.append(count[0, :, None] * cbk.embed.detach()[0].to(x.dtype).float() - sums[0])
+
+        idx32, _ = cbk.quantize_rows(flat, update=update, q_out=q, idx64_out=idx64, loss_out=loss_buf, loss_weight=loss_weight,
+                                     ema_update=ema_update, ema_update_weight=ema_update_weight,
+                                     accum_ema_update=accum_ema_update,
+                                     on_stats=take_commit_rows if learns and commit_grad else None)
+        commit = loss_buf.clone().reshape(()) if fused_loss else None
+        # the search's index buffer is reused by the next forward
+        learn = (idx32.clone(), commit_rows[0] if commit_rows else None) if learns else None
+        return q.reshape(shape), idx64.reshape(shape[:-1]), commit, None, learn
+
+    def _quantize_heads(self, x, update, ema_update, loss_weight, fused_loss):
+        """separate_codebook_per_head, x (b, n, h, d) (vqp:1044-1049 'b n (h d) -> h b n d', Codebook(num_codebooks=h)): head i
+        searches / updates codebook i of the (h, K, d) buffers — h independent chains on the same kernels, in head order (k-means
+        init and dead-code expiry draw from the RNG head by head, like the reference's batched_sample_vectors)."""
+        cbk, heads, d = self._codebook, self.heads, x.shape[-1]
         views = [cbk.head(i) for i in range(heads)]
-        xs = [x[..., i * d:(i + 1) * d].detach().reshape(-1, d).contiguous() for i in range(heads)]
+        xs = [x[..., i, :].detach().reshape(-1, d).contiguous() for i in range(heads)]
         if not cbk._initted_host:   # vqp:703: every head's k-means on the first batch, then ONE `initted` flag
             if not bool(cbk.initted):
                 for v, xi in zip(views, xs):
@@ -493,53 +435,65 @@ class VectorQuantize(nn.Module):
             cbk._initted_host = True
         for v in views:
             v._initted_host = True
-        loss_buf = getattr(self, "_head_loss_buf", None)
-        if loss_buf is None or loss_buf.device != x.device or loss_buf.numel() != heads:
-            loss_buf = self._head_loss_buf = torch.zeros((heads,), dtype=torch.float32, device=x.device)
-        qs, inds = [], []
+        loss_buf = self._loss_scratch(x.device, heads) if fused_loss else None
+        embed_ind = torch.empty(x.shape[:-1], dtype=torch.int64, device=x.device)   # 'h b n -> b n h' (vqp:1266-1268)
+        qs = []
         for i, (v, xi) in enumerate(zip(views, xs)):
             q = torch.empty_like(xi)
-            idx64 = torch.empty((xi.shape[0],), dtype=torch.int64, device=xi.device)
-            v.quantize_rows(xi, update=do_update, q_out=q, idx64_out=idx64, loss_out=loss_buf[i:i + 1] if fused_loss else None,
-                            loss_weight=self.commitment_weight, ema_update=ema_update)
-            qs.append(q.reshape(b, n, d))
-            inds.append(idx64.reshape(b, n))
-        quantize = torch.stack(qs, dim=2)            # (b, n, h, d)
-        embed_ind = torch.stack(inds, dim=-1)        # 'h b n -> b n h'  (vqp:1266-1268)
-        commit_loss = self.zero
-        if training and fused_loss:
-            # one mse over all heads (vqp:1327) == the mean of the heads' (equal-sized) means
-            commit_loss = loss_buf.mean()
-            loss = commit_loss.clone().requires_grad_(torch.is_grad_enabled())
+            v.quantize_rows(xi, update=update, q_out=q, idx64_out=embed_ind[..., i], idx_stride=heads,
+                            loss_out=loss_buf[i:i + 1] if fused_loss else None, loss_weight=loss_weight, ema_update=ema_update)
+            qs.append(q.reshape(x.shape[:-2] + (d,)))
+        # one mse over all heads (vqp:1327) == the mean of the heads' (equal-sized) means
+        commit = loss_buf.mean() if fused_loss else None
+        return torch.stack(qs, dim=2), embed_ind, commit, None, None
+
+    def _quantize_masked(self, x, mask, update, ema_update, loss_weight, want_loss):
+        """mask (B, N) bool (vqp:599-600, :1317-1325, :1378-1396).  Masked positions take no part in the statistics or the loss
+        (the reference zeroes their one-hot rows, vqp:599-600, and averages the loss over the unmasked elements against the
+        ORIGINAL input, vqp:1317-1325) and come back as zeros / index -1.  Euclidean codebooks: the search kernel takes the mask
+        (row_mask of vqb_vq_forward).  Cosine codebooks, pending k-means init, dead-code expiry: the kernels run on the
+        compacted unmasked rows."""
+        cbk = self._codebook
+        B, N, D = x.shape
+        flat = x.detach().reshape(-1, D).contiguous()
+        quantize = torch.zeros_like(flat) if self.return_zeros_for_masked_padding else flat.clone()
+        embed_ind = torch.full((B * N,), -1, dtype=torch.int64, device=x.device)
+        loss_buf = commit = glue = None
+        if not self.use_cosine_sim and cbk._initted_host and not (update and cbk.has_dead_code_replacement):
+            # in-kernel mask: every row is searched (like the reference), the merge step of the search kernel drops the padding
+            # rows — index -1, outputs left as pre-filled here, no loss term, no statistics — and the loss is divided by the
+            # unmasked element count on the device: no host sync, no compaction pass.  (Cosine: the masked loss is taken
+            # against the UN-normalised input, vqp:1319; k-means init / expiry sample from x[mask]: those take the path below.)
+            row_mask = mask.reshape(-1).contiguous().view(torch.uint8)
+            n_live = row_mask.sum(dtype=torch.int64).reshape(1)
+            loss_buf = self._loss_scratch(x.device) if want_loss else None
+            cbk.quantize_rows(flat, update=update, q_out=quantize, idx64_out=embed_ind, loss_out=loss_buf, loss_weight=loss_weight,
+                              ema_update=ema_update, row_mask=row_mask, n_live=n_live)
         else:
-            loss = torch.tensor(0., device=x.device, requires_grad=training and torch.is_grad_enabled())  # vqp:1282
-        if training:
-            x_h = x.reshape(b, n, heads, d)
-            if self.has_commitment_loss and not fused_loss:
-                commit_loss = F.mse_loss(quantize.detach(), cbk.transform_input(x_h))
-                loss = loss + commit_loss * self.commitment_weight
-            if input_requires_grad and self.route_gradients_to_input:  # vqp:1225-1233
-                x_t = cbk.transform_input(x_h)
-                quantize = rotate_to(x_t, quantize) if self.rotation_trick else straight_through(x_t, quantize)
-        quantize = self.project_out(quantize.reshape(b, n, hd))   # vqp:1354-1360
-        if restore is not None:
-            kind, dims = restore
-            if kind == "transpose":
-                quantize = quantize.transpose(1, 2)
-            else:
-                quantize = quantize.reshape(b, *dims, quantize.shape[-1]).movedim(-1, 1)
-                embed_ind = embed_ind.reshape(b, *dims, heads)
-        if only_one:
-            quantize = quantize.squeeze(1)
-            embed_ind = embed_ind.squeeze(1)
-        if not return_loss_breakdown:
-            return quantize, embed_ind, loss
-        return quantize, embed_ind, loss, LossBreakdown(commit_loss if self.commitment_weight == 1. or not fused_loss else commit_loss / self.commitment_weight,
-                                                       self.zero, self.zero, self.zero)
+            rows = mask.reshape(-1).nonzero(as_tuple=True)[0]  # host sync (the reference's masked path syncs as well)
+            if rows.numel() > 0:
+                xc = flat[rows].contiguous()
+                qc = torch.empty_like(xc)
+                ic = torch.empty((xc.shape[0],), dtype=torch.int64, device=x.device)
+                # euclid: the original input IS what the codebook saw; cosine: the glue takes the un-normalised input (vqp:1319)
+                loss_buf = self._loss_scratch(x.device) if want_loss and not self.use_cosine_sim else None
+                cbk.quantize_rows(xc, update=update, q_out=qc, idx64_out=ic, loss_out=loss_buf, loss_weight=loss_weight,
+                                  ema_update=ema_update)
+                quantize[rows] = qc
+                embed_ind[rows] = ic
+                glue = (qc, xc)
+            elif want_loss:   # no unmasked row: no loss term
+                commit = torch.zeros((), dtype=torch.float32, device=x.device)
+        if loss_buf is not None:
+            commit = loss_buf.clone().reshape(())
+        return quantize.reshape(B, N, D), embed_ind.reshape(B, N), commit, glue, None
 
     def forward(self, x, indices=None, mask=None, lens=None, topk=None, sample_codebook_temp=None, freeze_codebook=None,
                 return_loss_breakdown=False, codebook_transform_fn=None, ema_update_weight=None, accum_ema_update=False,
                 ema_update=None):
+        """vqp:1093-1403 as one pipeline: the input as rows (layout, project_in, heads), the codebook call of the variant (all
+        rows, one search per separate head, or a masked batch), then one tail: commitment loss, codebook gradient, gradient
+        estimator and the rows back in the input's layout."""
         if indices is not None:
             _unsupported("forward(indices=...) cross-entropy loss")
         if mask is not None and lens is not None:
@@ -549,91 +503,87 @@ class VectorQuantize(nn.Module):
         if mask is not None:
             if self.learnable_codebook:
                 _unsupported("mask / lens with a learnable codebook")
-            return self._forward_masked(x, mask, freeze_codebook, ema_update, return_loss_breakdown)
-        if topk is not None or codebook_transform_fn is not None:
+            if self.has_projections or self.accept_image_fmap or self.accept_3d_fmap or not self.channel_last or self.heads > 1:
+                _unsupported("mask / lens together with projections, feature-map layouts or heads > 1")
+            if x.requires_grad and torch.is_grad_enabled():
+                _unsupported("mask / lens on inputs that require grad")
+        elif topk is not None or codebook_transform_fn is not None:
             _unsupported("topk / codebook_transform_fn")
         if not x.is_cuda:
             raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
+        if mask is not None:
+            assert x.ndim == 3 and mask.shape == x.shape[:2]
 
         freeze_codebook = self.freeze_codebook if freeze_codebook is None else freeze_codebook
-        ema_update = self._codebook.ema_update if ema_update is None else ema_update
+        cbk = self._codebook
+        ema_update = cbk.ema_update if ema_update is None else ema_update
+        training = self.training
 
+        # ---- rows in (vqp:1136-1151)
         only_one = x.ndim == 2
         if only_one:
             x = x.unsqueeze(1)
         x, restore = self._to_rows_layout(x)
         x = self.project_in(x)  # vqp:1151
-        heads, batch = self.heads, x.shape[0]
-        if heads > 1 and self.separate_codebook_per_head:
-            return self._forward_separate_heads(x, restore, only_one, freeze_codebook, ema_update, return_loss_breakdown,
-                                                ema_update_weight, accum_ema_update)
-        if heads > 1:  # vqp:1044-1049: 'b n (h d) -> 1 (b h) n d' — every head's sub-vector is a row for the ONE codebook
-            x = x.reshape(batch, x.shape[1], heads, -1).transpose(1, 2).reshape(batch * heads, x.shape[1], -1)
+        heads, batch, n = self.heads, x.shape[0], x.shape[1]
+        separate = heads > 1 and self.separate_codebook_per_head
+        if separate:     # 'b n (h d) -> b n h d': head i is searched in codebook i
+            x = x.reshape(batch, n, heads, -1)
+        elif heads > 1:  # vqp:1044-1049: 'b n (h d) -> 1 (b h) n d' — every head's sub-vector is a row for the ONE codebook
+            x = x.reshape(batch, n, heads, -1).transpose(1, 2).reshape(batch * heads, n, -1)
         # decided AFTER project_in: with a projection the commitment loss must stay differentiable w.r.t. its weights
         # even when the raw input carries no grad (vqp:1151, :1327)
         input_requires_grad = x.requires_grad and torch.is_grad_enabled()
-        shape, dtype = x.shape, x.dtype
+        dtype = x.dtype
         if dtype not in (torch.float32, torch.bfloat16):
             raise TypeError(f"vqb200 supports float32 and bfloat16 inputs, got {dtype}")
 
-        flat = x.detach().reshape(-1, shape[-1]).contiguous()
-        N, D = flat.shape
-        cbk = self._codebook
-        training = self.training
-        do_update = training and not freeze_codebook and (ema_update or cbk.has_dead_code_replacement)
-        fused_loss = training and self.has_commitment_loss and not input_requires_grad
-
-        q = torch.empty_like(flat)
-        idx64 = torch.empty((N,), dtype=torch.int64, device=flat.device)
-        # the kernel returns weight * mse already rounded like F.mse_loss in x.dtype (vqp:1327-1329)
-        # the loss lands in a persistent scalar (stable pointer for the graph cache) and is cloned out
-        loss_buf = self._loss_scratch(flat.device) if fused_loss else None
-        # LossBreakdown.commitment is the UNweighted mse (vqp:1327-1329): ask the kernel for weight 1 then
+        # ---- the codebook call
+        want_loss = training and self.has_commitment_loss
+        fused_loss = want_loss and not input_requires_grad
+        # the kernels return weight * mse already rounded like F.mse_loss in x.dtype (vqp:1327-1329); LossBreakdown.commitment
+        # is the UNweighted mse: ask them for weight 1 then
         split_weight = fused_loss and return_loss_breakdown and self.commitment_weight != 1.
-        # a learnable codebook (vqp:710) gets the gradient of `quantize` and, in training, of the commitment loss (vqp:1214-1216)
-        learn = cbk.learns()
-        commit_grad = learn and training and self.has_commitment_loss and not freeze_codebook
-        commit_rows = []
+        update = cbk.updates(training, freeze_codebook, ema_update)
+        loss_weight = 1. if split_weight else self.commitment_weight
+        if mask is not None:
+            quantize, embed_ind, commit, glue, learn = self._quantize_masked(x, mask, update, ema_update, loss_weight, want_loss)
+        elif separate:
+            if accum_ema_update or ema_update_weight is not None:
+                _unsupported("ema_update_weight / accum_ema_update with separate_codebook_per_head")
+            quantize, embed_ind, commit, glue, learn = self._quantize_heads(x, update, ema_update, loss_weight, fused_loss)
+        else:
+            quantize, embed_ind, commit, glue, learn = self._quantize_shared(
+                x, update, ema_update, loss_weight, fused_loss, want_loss and not freeze_codebook, ema_update_weight,
+                accum_ema_update)
 
-        def take_commit_rows(stats):   # count_k c_k - sum_{n -> k} x_n, with the codebook the rows were searched in
-            # the reference differentiates mse(quantize.type(dtype), x) (vqp:1178, :1327): the code as rounded to x's dtype
-            count, sums = cbk._stat_views(stats)
-            commit_rows.append(count[0, :, None] * cbk.embed.detach()[0].to(dtype).float() - sums[0])
-
-        idx32, _ = cbk.quantize_rows(flat, update=do_update, q_out=q, idx64_out=idx64, loss_out=loss_buf,
-                                     loss_weight=1. if split_weight else self.commitment_weight, ema_update=ema_update,
-                                     ema_update_weight=ema_update_weight, accum_ema_update=accum_ema_update,
-                                     on_stats=take_commit_rows if commit_grad else None)
-        commit_loss = loss_buf.clone().reshape(()) if fused_loss else self.zero
-        weighted = commit_loss
-        if split_weight:  # commit_loss * weight in the input dtype, promoted by the fp32 accumulator (vqp:1329, :1282)
-            weighted = (commit_loss.to(dtype) * self.commitment_weight).float()
-
-        quantize = q.reshape(shape)
-        embed_ind = idx64.reshape(shape[:-1])
-
-        if training and fused_loss:
+        # ---- commitment loss (vqp:1282, :1317-1329)
+        fused = commit is not None
+        if fused:
+            weighted = commit
+            if split_weight:  # commit * weight in the input dtype, promoted by the fp32 accumulator (vqp:1329, :1282)
+                weighted = (commit.to(dtype) * self.commitment_weight).float()
             # vqp:1282: `loss` is a fresh fp32 scalar that requires grad in training mode
             loss = weighted.requires_grad_(torch.is_grad_enabled())
         else:
-            loss = torch.tensor(0., device=flat.device, requires_grad=training and torch.is_grad_enabled())  # vqp:1282
-        if training and self.has_commitment_loss and not fused_loss:
-            # differentiable w.r.t. the input: PyTorch glue on the kernel's outputs
-            commit_loss = F.mse_loss(quantize.detach(), cbk.transform_input(x))
-        if learn:
-            idx32 = idx32.clone()   # the search's index buffer is reused by the next forward
-            if not commit_rows:
+            loss = torch.tensor(0., device=x.device, requires_grad=training and torch.is_grad_enabled())  # vqp:1282
+            if want_loss:   # differentiable w.r.t. the input: PyTorch glue on the kernel's outputs
+                q_rows, target = glue or (quantize, cbk.transform_input(x))
+                commit = F.mse_loss(q_rows.detach(), target)
+        if learn is not None:
+            idx32, commit_rows = learn
+            if commit_rows is None:
                 quantize, _ = _LearnableCodebook.apply(cbk.embed, quantize, None, idx32, None, 0.)
-            elif fused_loss:   # `loss` is already weight * mse
-                quantize, loss = _LearnableCodebook.apply(cbk.embed, quantize, loss, idx32, commit_rows[0],
-                                                          2. * self.commitment_weight / flat.numel())
+            elif fused:   # `loss` is already weight * mse
+                quantize, loss = _LearnableCodebook.apply(cbk.embed, quantize, loss, idx32, commit_rows,
+                                                          2. * self.commitment_weight / x.numel())
             else:
-                quantize, commit_loss = _LearnableCodebook.apply(cbk.embed, quantize, commit_loss, idx32, commit_rows[0],
-                                                                 2. / flat.numel())
+                quantize, commit = _LearnableCodebook.apply(cbk.embed, quantize, commit, idx32, commit_rows, 2. / x.numel())
         if training:
-            if self.has_commitment_loss and not fused_loss:
-                loss = loss + commit_loss * self.commitment_weight
-            if input_requires_grad and self.route_gradients_to_input:  # vqp:1225-1233
+            if want_loss and not fused:
+                loss = loss + commit * self.commitment_weight
+            # ---- gradient estimator (vqp:1225-1237)
+            if input_requires_grad and self.route_gradients_to_input:
                 x_t = cbk.transform_input(x)
                 if self.rotation_trick:
                     quantize = rotate_to(x_t, quantize)
@@ -641,26 +591,27 @@ class VectorQuantize(nn.Module):
                     quantize = directional_reparam(x_t, quantize, self.directional_reparam_variance)
                 else:
                     quantize = straight_through(x_t, quantize)
-            if self.sync_update_v > 0.:  # vqp:1235-1237
+            if self.sync_update_v > 0.:
                 quantize = quantize + self.sync_update_v * (quantize - quantize.detach())
 
-        if heads > 1:  # vqp:1354-1358 '1 (b h) n d -> b n (h d)', :1266-1270 '1 (b h) n -> b n h'
-            n = quantize.shape[1]
+        # ---- rows out (vqp:1354-1373, :1265-1275)
+        if separate:     # 'b n h d -> b n (h d)'
+            quantize = quantize.reshape(batch, n, -1)
+        elif heads > 1:  # '1 (b h) n d -> b n (h d)', '1 (b h) n -> b n h'
             quantize = quantize.reshape(batch, heads, n, -1).transpose(1, 2).reshape(batch, n, -1)
             embed_ind = embed_ind.reshape(batch, heads, n).transpose(1, 2)
         quantize = self.project_out(quantize)  # vqp:1360
-        if restore is not None:  # vqp:1364-1373, :1265-1275
+        if restore is not None:
             kind, dims = restore
             if kind == "transpose":
                 quantize = quantize.transpose(1, 2)
             else:
-                b = quantize.shape[0]
-                quantize = quantize.reshape(b, *dims, quantize.shape[-1]).movedim(-1, 1)
-                embed_ind = embed_ind.reshape(b, *dims, *embed_ind.shape[2:])
+                quantize = quantize.reshape(batch, *dims, quantize.shape[-1]).movedim(-1, 1)
+                embed_ind = embed_ind.reshape(batch, *dims, *embed_ind.shape[2:])
         if only_one:
             quantize = quantize.squeeze(1)
             embed_ind = embed_ind.squeeze(1)
 
         if not return_loss_breakdown:
             return quantize, embed_ind, loss
-        return quantize, embed_ind, loss, LossBreakdown(commit_loss, self.zero, self.zero, self.zero)
+        return quantize, embed_ind, loss, LossBreakdown(self.zero if commit is None else commit, self.zero, self.zero, self.zero)
