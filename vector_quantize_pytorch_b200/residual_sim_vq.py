@@ -87,12 +87,7 @@ class _ResidualSimVQFunction(torch.autograd.Function):
         key = (dev, N, D, K, n_active, want_stats,
                tuple((bool(layer.rotation_trick), float(layer.input_to_quantize_commit_loss_weight), float(layer.commitment_weight))
                      for layer in mod.layers[:n_active]))
-        plans = mod.__dict__.setdefault("_plans", _PlanCache())
-        plan = plans.get(key)
-        if plan is None:
-            if len(plans) >= 8:
-                plans.clear()
-            plan = plans[key] = _Plan(mod, N, D, K, n_active, want_stats, dev)
+        plan = _PlanCache.get_or_build(mod, key, lambda: _Plan(mod, N, D, K, n_active, want_stats, dev))
         out = torch.empty_like(x)
         if n_active < Q:   # rsv:153-187: the dropped stages report index -1 and a zero loss
             indices = torch.full((N, Q), -1, dtype=torch.int64, device=dev)

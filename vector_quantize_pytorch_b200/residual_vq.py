@@ -1,11 +1,13 @@
 """`ResidualVQ` / `GroupedResidualVQ` — drop-ins for residual_vq.py:166-630 and :634-724 of the reference
 (no beam search, no implicit neural codebook; quantize dropout and masks run on the stage-wise path).
 
-Every stage's search writes the next residual (residual -= q, rvq:524) from its fused tail and its indices
-straight into the (..., Q) int64 result; quantized_out += q (rvq:525) is rebuilt from those indices in one
-pass after the last stage (rounded to the input dtype exactly where the reference rounds).  The EMA
-statistics of ALL stages (and, for the grouped module, all groups) are packed into one buffer so that
-multi-GPU training needs ONE all-reduce per forward instead of the reference's 2 per codebook per stage.
+`ResidualVQ.forward` is one row pipeline: rows in, compaction of a masked batch, ONE row quantizer — layered (gradients), the
+cached one-call program or stage-wise — and one tail.  Every stage's search writes the next residual (residual -= q, rvq:524)
+from its fused tail and its indices straight into the (..., Q) int64 result; quantized_out += q (rvq:525) is rebuilt from those
+indices in one pass after the last stage (rounded to the input dtype exactly where the reference rounds).  The codebook updates
+after the searches are described once (`_CodebookUpdates`), recorded into the program or applied eagerly.  The EMA statistics
+of ALL stages (and, for the grouped module, all groups) are packed into one buffer so that multi-GPU training needs ONE
+all-reduce per forward instead of the reference's 2 per codebook per stage.
 """
 from __future__ import annotations
 
@@ -22,6 +24,8 @@ from .codebook import _unsupported
 from .dist import allreduce_packed, PeerReducer
 from .vector_quantize import VectorQuantize, directional_reparam
 
+_DTYPES = (torch.float32, torch.bfloat16)
+
 
 class _PlanCache(dict):
     """Cached op lists of a module (raw device pointers inside): never copied or pickled along with the module."""
@@ -32,10 +36,156 @@ class _PlanCache(dict):
     def __reduce__(self):
         return (_PlanCache, ())
 
+    @staticmethod
+    def get_or_build(module, key, build):
+        """The module's cached plan for `key`, made by `build()` when missing.  At most 8 are kept: a full cache is emptied."""
+        plans = module.__dict__.setdefault("_plans", _PlanCache())
+        plan = plans.get(key)
+        if plan is None:
+            if len(plans) >= 8:
+                plans.clear()
+            plan = plans[key] = build()
+        return plan
+
+
+def _sync_seed(device):
+    """get_maybe_sync_seed (rvq:96-103): torch.randint on the device, all-reduced over the ranks."""
+    seed = torch.randint(0, 10_000, (), device=device)
+    if distributed.is_available() and distributed.is_initialized() and distributed.get_world_size() > 1:
+        distributed.all_reduce(seed)
+    return seed
+
+
+class _CodebookUpdates:
+    """The codebook updates that follow the searches of one ResidualVQ forward: the lerps of the packed statistics in stage
+    order (vqp:616-617), update_ema — for a shared codebook once, at the end (rvq:593-597) — and dead-code expiry (vqp:641;
+    rvq:599-601).  `record` appends them to a program, `apply` runs them eagerly.  The statistics go to one packed buffer
+    (`stats(q)`: stage q's slice), local or the peer-memory buffer `begin` takes.  A shared codebook that replaces dead codes
+    is changed BETWEEN stages by the reference (every layer's update_codebook ends with expire_codes_, vqp:641, on the one
+    aliased Codebook): such "inline" stages update inside their own search and have no slice."""
+
+    def __init__(self, rvq, books, do_update, D, device):
+        self.books, self.do_update = books, do_update
+        self.shared = rvq.shared_codebook
+        self.inline = [u and self.shared and b.has_dead_code_replacement for b, u in zip(books, do_update)]
+        self.sizes = [ops.stats_floats(b.codebook_size, D) if (u and not i) else 0
+                      for b, u, i in zip(books, do_update, self.inline)]
+        self.offs = [sum(self.sizes[:q]) for q in range(len(books))]
+        total = sum(self.sizes)
+        self.use_ddp = any(b.use_ddp for b in books)
+        self.peer = self.peer_ptrs = self.packed = None
+        if total and self.use_ddp:
+            self.peer = rvq._peer_reducer(total, device)
+        if self.peer is not None:   # the buffer `begin` takes: statistics summed over the ranks inside the EMA kernels
+            parity = self.peer.step & 1
+            self.packed, self.peer_ptrs = self.peer.bufs[parity][:total], self.peer.stats_ptrs[parity]
+        elif total:
+            self.packed = torch.empty((total,), dtype=torch.float32, device=device)
+        # (stage, codebook, update_ema after the lerp): a shared codebook is manual (rvq:213-217) and normalised once, at the end
+        self.steps = [(q, b, b.ema_update and not b.manual_ema_update) for q, b in enumerate(books) if self.sizes[q]]
+        self.final_ema = rvq.training and self.shared and rvq.vq_is_ema_updating and any(do_update)   # rvq:593-597
+        self.stage_inputs = []      # the stage inputs (N, D), kept by the stage-wise path when codes can expire
+        self.rows0 = 0              # rows of batch element 0: the shared codebook's expiry samples only those (see `apply`)
+
+    def stats(self, q):
+        return self.packed[self.offs[q]:self.offs[q] + self.sizes[q]] if self.sizes[q] else None
+
+    def begin(self):
+        """Once per forward, before its statistics are written: the peer reducer moves on to the other parity buffer."""
+        if self.peer is not None:
+            self.peer.next_buffer()
+
+    def record(self, prog, lane):
+        """Append the updates to `prog` (no inline stages: the program path has no dead-code expiry).  Returns the codebooks
+        whose search operands the program refreshes."""
+        books, peer = self.books, self.peer
+        if peer is not None:
+            prog.barrier(lane, peer)      # every rank's statistics of this forward are in place (vqp:603, :607)
+
+        def ema(book, q, normalise, **kw):
+            cs, ea, emb = book._state2d()
+            if peer is not None:
+                prog.ema_peers(lane, cs, ea, emb, peer, self.peer_ptrs, self.offs[q], book.operands(), decay=book.decay,
+                               eps=book.eps, do_normalise=normalise, **kw)
+            else:
+                prog.ema(lane, cs, ea, emb, self.stats(q), book.operands(), decay=book.decay, eps=book.eps, do_lerp=True,
+                         do_normalise=normalise, **kw)
+
+        if self.shared and len(self.steps) == len(books) > 1:
+            # one codebook, Q stages: ONE op applies the Q statistics slices in stage order, then normalises once
+            ema(books[0], 0, self.final_ema, n_lerp=len(books), slice_stride=self.sizes[0])
+            return [books[0]] if self.final_ema else []
+        for q, book, normalise in self.steps:
+            ema(book, q, normalise)
+        refreshed = [book for _, book, normalise in self.steps if normalise]
+        if self.final_ema:
+            cs, ea, emb = books[0]._state2d()
+            prog.ema(lane, cs, ea, emb, None, books[0].operands(), decay=books[0].decay, eps=books[0].eps, do_lerp=False,
+                     do_normalise=True)
+            refreshed.append(books[0])
+        return refreshed
+
+    @staticmethod
+    def apply_all(pending):
+        """Run the updates of one or more forwards (the groups of a GroupedResidualVQ) eagerly: without peer memory ONE
+        all-reduce covers every codebook of all of them (reference: 2 per codebook per stage, vqp:603/:607)."""
+        local = [u for u in pending if u.packed is not None]
+        if local and any(u.use_ddp for u in pending) and all(u.peer is None for u in pending):
+            flat = allreduce_packed(local[0].packed if len(local) == 1 else torch.cat([u.packed for u in local]))
+            pos = 0
+            for u in local:   # every forward's slice of the summed statistics
+                n = u.packed.numel()
+                u.packed = flat[pos:pos + n]
+                pos += n
+        for u in pending:
+            u.apply()
+
+    def apply(self):
+        """The lerps, update_ema and expiry, after the statistics are summed over the ranks (`apply_all`)."""
+        peer = self.peer
+        if peer is not None:
+            peer.barrier()       # every rank's statistics of this forward are in place
+        for q, book, normalise in self.steps:
+            if peer is not None:
+                book.lerp_stats_peers(peer, self.peer_ptrs, self.offs[q], normalise)
+            else:
+                book.lerp_stats(self.stats(q), normalise=normalise)
+            if not self.shared and book.has_dead_code_replacement:
+                book.expire_codes_(book.transform_input(self.stage_inputs[q]).float())  # vqp:641 on the fp32 `flatten`
+        shared = self.books[0]
+        if self.final_ema:
+            shared.update_ema()
+        if self.shared and shared.has_dead_code_replacement and any(self.do_update):
+            # rvq:599-601 -> vqp:1051-1054 -> :573-574: the reference hands '(b) (n l) d' to Codebook.expire_codes_, whose
+            # 'h ... d -> h (...) d' reads the batch axis as the codebook axis, and `replace` zips it with the (1, K)
+            # mask: only batch element 0's rows (n-major, stage-minor) are sampled from.  Reproduced as is.
+            rows = torch.stack([r[:self.rows0] for r in self.stage_inputs], dim=1).reshape(-1, self.stage_inputs[0].shape[-1])
+            shared.expire_codes_(shared.transform_input(rows))
+
+
+def _run_program(owner, rvqs, flats, plan, persistent_io=False):
+    """ResidualVQ forwards — stages, running sum, codebook updates — as ONE vqb_rvq_forward call / one CUDA graph, the forwards
+    (the groups of a GroupedResidualVQ) as independent chains on parallel lanes.  The op list is cached on `owner`; only the
+    per-call pointers (input, indices, output) are patched.  plan: each forward's (codebooks, stages that update).
+    Returns each forward's (quantized rows, indices (N, Q), losses (Q,))."""
+    for rvq, flat in zip(rvqs, flats):
+        rvq._ensure_loss_buf(flat.device)
+    key = tuple(rvq._part_key(flat, books, upd) for rvq, flat, (books, upd) in zip(rvqs, flats, plan))
+
+    def build():
+        prog = ops.RvqProgram(flats[0].device)
+        parts = [_PlanPart(rvq, prog, g % 4, flat, books, upd, persistent_io)
+                 for g, (rvq, flat, (books, upd)) in enumerate(zip(rvqs, flats, plan))]
+        return prog.freeze(), parts
+    prog, parts = _PlanCache.get_or_build(owner, key, build)
+    bound = [part.bind(prog.arr, flat) for part, flat in zip(parts, flats)]
+    prog.run()
+    return [part.finish(b) for part, b in zip(parts, bound)]
+
 
 class _PlanPart:
-    """One ResidualVQ forward inside an ops.RvqProgram: stage ops (rvq:469-568), the running sum (rvq:525), the deferred EMA
-    ops (rvq:593-597 / vqp:616-617, :576-584).  Built once per configuration; `bind` patches the per-call pointers."""
+    """One ResidualVQ forward inside an ops.RvqProgram: stage ops (rvq:469-568), the running sum (rvq:525), the recorded
+    codebook updates (`_CodebookUpdates.record`).  Built once per configuration; `bind` patches the per-call pointers."""
 
     def __init__(self, rvq, prog, lane, flat, books, do_update, persistent_io=False):
         # persistent_io (GroupedResidualVQ: its cat / stack copy the results anyway): input, indices and output live in
@@ -46,19 +196,10 @@ class _PlanPart:
         N, D = flat.shape
         Q = rvq.num_quantizers
         dev, dtype = flat.device, flat.dtype
-        training = rvq.training
         self.rvq, self.N, self.D, self.Q, self.dtype, self.dev = rvq, N, D, Q, dtype, dev
         self.bufs = [torch.empty_like(flat) for _ in range(min(2, Q - 1))]          # persistent: the residual ping-pong
-        stat_sizes = [ops.stats_floats(b.codebook_size, D) if u else 0 for b, u in zip(books, do_update)]
-        offs = [sum(stat_sizes[:i]) for i in range(Q)]
-        self.peer = rvq._peer if (sum(stat_sizes) and any(b.use_ddp and u for b, u in zip(books, do_update))) else None
-        if self.peer is not None:   # this plan is bound to ONE of the two alternating symmetric buffers (the key holds the parity)
-            par = self.peer.step & 1
-            self.packed, peer_ptrs = self.peer.bufs[par][:sum(stat_sizes)], self.peer.stats_ptrs[par]
-        else:
-            self.packed = torch.empty((sum(stat_sizes),), dtype=torch.float32, device=dev) if sum(stat_sizes) else None
+        self.updates = _CodebookUpdates(rvq, books, do_update, D, dev)
         self.losses = rvq._loss_buf
-        self.books = books
         all_idx = torch.empty((N, Q), dtype=torch.int64, device=dev)               # placeholders: `bind` patches the pointers
         out0 = torch.empty((N, D), dtype=dtype, device=dev)
         if persistent_io:
@@ -71,12 +212,11 @@ class _PlanPart:
         residual = flat
         for q, book in enumerate(books):
             nxt = self.bufs[q & 1] if q + 1 < Q else None
-            want_loss = training and rvq.layers[q].has_commitment_loss
+            want_loss = rvq.training and rvq.layers[q].has_commitment_loss
             prog.stage(lane, residual, book.operands(), book._state2d(), update=1 if do_update[q] else 0, do_normalise=False,
                        decay=book.decay, eps=book.eps, idx64_out=all_idx[:, q], idx_stride=Q,
                        loss_out=self.losses[q:q + 1] if want_loss else None, loss_weight=rvq.layers[q].commitment_weight,
-                       resid_out=nxt, stats=self.packed[offs[q]:offs[q] + stat_sizes[q]] if stat_sizes[q] else None,
-                       ws_key=id(book),
+                       resid_out=nxt, stats=self.updates.stats(q), ws_key=id(book),
                        a_planes_in=self.planes[(q - 1) & 1] if (split and q > 0) else None,
                        planes_out=self.planes[q & 1] if (split and nxt is not None) else None)
             residual = nxt
@@ -85,56 +225,19 @@ class _PlanPart:
         embeds = books[0].embed[0] if rvq.shared_codebook else self.stack
         self.acc = len(prog.ops)
         prog.accumulate(lane, embeds, all_idx, out0)
-        self.refreshed = []
-        if self.peer is not None:
-            prog.barrier(lane, self.peer)      # every rank's statistics of this forward are in place (vqp:603, :607)
-        final_ema = training and rvq.shared_codebook and rvq.vq_is_ema_updating and any(do_update)   # rvq:593-597
-        if rvq.shared_codebook and all(stat_sizes) and Q > 1 and books[0].manual_ema_update:
-            # one codebook, Q stages: every stage lerps the same buffers in turn (rvq:302-306) and update_ema follows once
-            # (rvq:593-597) — ONE launch pair applies the Q statistics slices in order and normalises
-            shared = books[0]
-            cs, ea, emb = shared._state2d()
-            if self.peer is not None:
-                prog.ema_peers(lane, cs, ea, emb, self.peer, peer_ptrs, 0, shared.operands(), decay=shared.decay, eps=shared.eps,
-                               do_normalise=final_ema, n_lerp=Q, slice_stride=stat_sizes[0])
-            else:
-                prog.ema(lane, cs, ea, emb, self.packed, shared.operands(), decay=shared.decay, eps=shared.eps, do_lerp=True,
-                         do_normalise=final_ema, n_lerp=Q, slice_stride=stat_sizes[0])
-            if final_ema:
-                self.refreshed.append(shared)
-            return
-        for q, book in enumerate(books):
-            if not stat_sizes[q]:
-                continue
-            normalise = book.ema_update and not book.manual_ema_update
-            cs, ea, emb = book._state2d()
-            if self.peer is not None:
-                prog.ema_peers(lane, cs, ea, emb, self.peer, peer_ptrs, offs[q], book.operands(), decay=book.decay, eps=book.eps,
-                               do_normalise=normalise)
-            else:
-                prog.ema(lane, cs, ea, emb, self.packed[offs[q]:offs[q] + stat_sizes[q]], book.operands(), decay=book.decay,
-                         eps=book.eps, do_lerp=True, do_normalise=normalise)
-            if normalise:
-                self.refreshed.append(book)
-        if final_ema:
-            shared = books[0]
-            cs, ea, emb = shared._state2d()
-            prog.ema(lane, cs, ea, emb, None, shared.operands(), decay=shared.decay, eps=shared.eps, do_lerp=False,
-                     do_normalise=True)
-            self.refreshed.append(shared)
+        self.refreshed = self.updates.record(prog, lane)
 
     def bind(self, arr, flat):
         """Fresh outputs for this call + the pointers of the cached ops that change from call to call."""
         if self.stack is not None:
-            torch.stack([b.embed[0] for b in self.books], out=self.stack)
+            torch.stack([b.embed[0] for b in self.updates.books], out=self.stack)
         if not self.rvq.training:
             self.losses.zero_()
-        if self.peer is not None:
-            self.peer.step += 1          # the next forward uses the other symmetric buffer (and the plan cached for it)
+        self.updates.begin()          # with peer memory the next forward uses the other buffer (and the plan cached for it)
         if self.io is not None:
             if flat is not self.io[0]:
                 self.io[0].copy_(flat.reshape(self.N, self.D))
-            return self.io[1], self.io[2], None
+            return self.io[1], self.io[2]
         all_idx = torch.empty((self.N, self.Q), dtype=torch.int64, device=self.dev)
         out = torch.empty((self.N, self.D), dtype=self.dtype, device=self.dev)
         ip = all_idx.data_ptr()
@@ -143,20 +246,14 @@ class _PlanPart:
             arr[self.first + q].stage.idx64_out = ip + 8 * q
         arr[self.acc].acc.idx = ip
         arr[self.acc].acc.out = out.data_ptr()
-        return all_idx, out, flat
+        return all_idx, out
 
-    def finish(self, bound, shape, return_all_codes, project=True):
-        all_idx, out, _ = bound
-        rvq = self.rvq
+    def finish(self, bound):
+        """(quantized rows, indices (N, Q), losses (Q,)) of the call `bound` came from, after the program ran."""
         for b in self.refreshed:
             b._mark_operands_fresh()
-        out = out.reshape(shape)
-        if project:
-            out = rvq.project_out(out)  # rvq:610
-        ret = (out, all_idx.reshape(*shape[:-1], self.Q), self.losses.clone())
-        if return_all_codes:
-            ret = (*ret, rvq.get_codes_from_indices(ret[1]))
-        return ret
+        all_idx, out = bound
+        return out, all_idx, self.losses.clone()
 
 
 class ResidualVQ(nn.Module):
@@ -268,6 +365,10 @@ class ResidualVQ(nn.Module):
     def _stage_plan(self):
         return [vq._codebook for vq in self.layers]
 
+    def _do_update(self, books, freeze_codebook, n_run):
+        """Which stages change their codebook in this forward: the active ones (quantize dropout, rvq:473-476) that update."""
+        return [q < n_run and b.updates(self.training, freeze_codebook) for q, b in enumerate(books)]
+
     def _peer_reducer(self, numel, device):
         """One symmetric-memory buffer for the statistics of ALL stages (dist.PeerReducer); None -> NCCL all-reduce."""
         if not getattr(self, "_peer_tried", False) or (self._peer is not None and self._peer.numel < numel):
@@ -275,124 +376,84 @@ class ResidualVQ(nn.Module):
             self._peer = PeerReducer.create(numel, device)
         return self._peer
 
+    def _takes_layered(self, x):
+        """Gradients (to the input or to project_in, rvq:406, or to learnable codebooks) need the per-stage straight-through /
+        rotation / codebook-gradient glue of VectorQuantize: the layered path."""
+        return torch.is_grad_enabled() and (x.requires_grad or self._codebooks_need_grad())
+
     def forward(self, x, mask=None, indices=None, return_all_codes=False, sample_codebook_temp=None,
-                freeze_codebook=False, beam_size=None, rand_quantize_dropout_fixed_seed=None,
-                _stats_sink=None, _projected=False):
+                freeze_codebook=False, beam_size=None, rand_quantize_dropout_fixed_seed=None):
         if indices is not None:
             _unsupported("ResidualVQ.forward(indices=)")
         if beam_size is not None and beam_size > 1:
             _unsupported("beam search")
+        return self._forward_projected(self.project_in(x), mask, return_all_codes, freeze_codebook,  # rvq:406
+                                       rand_quantize_dropout_fixed_seed)
+
+    def _forward_projected(self, x, mask, return_all_codes, freeze_codebook, dropout_seed, pending=None):
+        """The row pipeline after project_in.  `pending` (GroupedResidualVQ): a list the stage-wise path appends its
+        `_CodebookUpdates` to instead of applying them, so that all groups share one all-reduce."""
         if not x.is_cuda:
             raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
-        if mask is not None:
-            return self._forward_masked(x, mask, return_all_codes, freeze_codebook, rand_quantize_dropout_fixed_seed)
-        if not _projected:   # _projected: the masked path hands in compacted rows that went through project_in already
-            x = self.project_in(x)
-        if torch.is_grad_enabled() and (x.requires_grad or self._codebooks_need_grad()):
-            # gradients (to the input or to project_in, rvq:406, or to learnable codebooks) need the per-stage
-            # straight-through / rotation / codebook-gradient glue of VectorQuantize: take the layered path
-            return self._forward_layered(x, freeze_codebook, return_all_codes,
-                                         self._active_layers(rand_quantize_dropout_fixed_seed, x.device))
-        shape, dtype = x.shape, x.dtype
-        if dtype not in (torch.float32, torch.bfloat16):
-            raise TypeError(f"vqb200 supports float32 and bfloat16 inputs, got {dtype}")
-        flat = x.detach().reshape(-1, shape[-1]).contiguous()
-        N, D = flat.shape
-        Q = self.num_quantizers
-        dev = flat.device
-        training = self.training
+        shape, D, Q = x.shape, x.shape[-1], self.num_quantizers
         books = self._stage_plan()
+        rows = masked = None
+        if mask is not None:
+            if any(b.learnable_codebook for b in books):
+                _unsupported("ResidualVQ.forward(mask=) with learnable codebooks")
+            if any(b.use_cosine_sim for b in books):
+                _unsupported("ResidualVQ.forward(mask=) with use_cosine_sim (the masked loss is taken against the un-normalised input, vqp:1319)")
+            if any(not vq.return_zeros_for_masked_padding for vq in self.layers):
+                _unsupported("ResidualVQ.forward(mask=) with return_zeros_for_masked_padding=False")
+            if self.training and any(b.has_dead_code_replacement for b in books):
+                _unsupported("ResidualVQ.forward(mask=) with dead-code replacement")
+            # The reference hands the mask to every layer (rvq:495): a layer searches every row, but masked rows take no part
+            # in its statistics or loss (vqp:599-600, :1317-1325) and come back as zeros / index -1 (vqp:1378-1396), so their
+            # residual is never reduced and their running sum stays zero.  That is exactly the forward over the COMPACTED
+            # unmasked rows with zeros / -1 scattered around it (stage-wise: the row count changes from call to call, a
+            # cached program per count would not pay).
+            if x.requires_grad and torch.is_grad_enabled():
+                _unsupported("ResidualVQ.forward(mask=) on inputs / projections that require grad")
+            assert x.ndim == 3 and mask.shape == x.shape[:2]
+            rows = mask.reshape(-1).nonzero(as_tuple=True)[0]  # host sync (the reference's masked path syncs as well)
+            masked = (rows, torch.zeros((mask.numel(), D), dtype=x.dtype, device=x.device),
+                      torch.full((mask.numel(), Q), -1, dtype=torch.int64, device=x.device))
 
-        losses = self._ensure_loss_buf(dev)
-        n_run = self._active_layers(rand_quantize_dropout_fixed_seed, dev)   # < Q: quantize dropout skips the layers after it
-        do_update = [q < n_run and b.updates(training, freeze_codebook) for q, b in enumerate(books)]
-        if not _projected and n_run == Q and self._program_ok(books, do_update):
-            # the whole forward — stages, running sum, deferred EMA updates — as ONE vqb_rvq_forward call / one CUDA graph,
-            # from a cached op list in which only the per-call pointers (input, indices, output) are patched
-            key = self._part_key(flat, books, do_update)
-            plans = self.__dict__.setdefault("_plans", _PlanCache())
-            plan = plans.get(key)
-            if plan is None:
-                if len(plans) >= 8:
-                    plans.clear()
-                prog = ops.RvqProgram(dev)
-                part = self._plan_part(prog, 0, flat, books, do_update)
-                plan = plans[key] = (prog.freeze(), part)
-            prog, part = plan
-            bound = part.bind(prog.arr, flat)
-            prog.run()
-            if not self.diveq:
-                return part.finish(bound, shape, return_all_codes)
-            out, *rest = part.finish(bound, shape, return_all_codes, project=False)
-            return (self.project_out(directional_reparam(x, out)), *rest)   # rvq:603-606, in every mode
-
-        if n_run < Q:   # rvq:473-476: the skipped layers report index -1 and loss 0
-            all_idx = torch.full((N, Q), -1, dtype=torch.int64, device=dev)
-            losses.zero_()
+        if rows is not None and rows.numel() == 0:   # nothing to quantize: no quantizer runs, not even the dropout draw
+            quantized = indices = None
+            losses = torch.zeros((Q,), dtype=torch.float32, device=x.device)
+        elif self._takes_layered(x):
+            quantized, indices, losses = self._quantize_layered(x, freeze_codebook, self._active_layers(dropout_seed, x.device))
         else:
-            all_idx = torch.empty((N, Q), dtype=torch.int64, device=dev)
-        if not training:
-            losses.zero_()
-        # dead-code expiry samples from the stage inputs after the (deferred) EMA update: keep them all then
-        keep_inputs = training and not freeze_codebook and any(b.has_dead_code_replacement for b in books)
-        bufs = [torch.empty_like(flat) for _ in range(Q - 1 if keep_inputs else min(2, Q - 1))]
-        residual = flat  # rvq:411 (never written: stage 0 reads the caller's tensor)
-        stage_inputs = []
-        # A shared codebook that replaces dead codes is modified BETWEEN stages by the reference (every layer's
-        # update_codebook ends with expire_codes_, vqp:641, on the one aliased Codebook): such stages cannot be deferred.
-        inline = [u and self.shared_codebook and b.has_dead_code_replacement for b, u in zip(books, do_update)]
-        stat_sizes = [ops.stats_floats(b.codebook_size, D) if (u and not i) else 0 for b, u, i in zip(books, do_update, inline)]
-        packed, peer_ptrs = None, None
-        if sum(stat_sizes):
-            peer = self._peer_reducer(sum(stat_sizes), dev) if any(b.use_ddp for b in books) else None
-            if peer is not None:   # statistics straight into symmetric memory: summed over the ranks inside the EMA kernels
-                buf, peer_ptrs = peer.next_buffer()
-                packed = buf[:sum(stat_sizes)]
+            if x.dtype not in _DTYPES:
+                raise TypeError(f"vqb200 supports float32 and bfloat16 inputs, got {x.dtype}")
+            flat = x.detach().reshape(-1, D)
+            flat = flat[rows] if rows is not None else flat.contiguous()
+            n_run = self._active_layers(dropout_seed, x.device)   # < Q: quantize dropout skips the layers after it
+            do_update = self._do_update(books, freeze_codebook, n_run)
+            if rows is None and n_run == Q and self._program_ok(books, do_update):
+                quantized, indices, losses = _run_program(self, [self], [flat], [(books, do_update)])[0]
             else:
-                packed = torch.empty((sum(stat_sizes),), dtype=torch.float32, device=dev)
-        offs = [sum(stat_sizes[:i]) for i in range(Q)]
+                rows0 = flat.shape[0] // shape[0] if (rows is None and len(shape) > 2) else flat.shape[0]
+                quantized, indices, losses = self._quantize_stagewise(flat, books, do_update, n_run, freeze_codebook, rows0,
+                                                                      pending)
 
-        inline_embeds = []   # the shared codebook as each inline stage searched it
-        for q, book in enumerate(books[:n_run]):  # rvq:469
-            nxt = (bufs[q] if keep_inputs else bufs[q & 1]) if q + 1 < n_run else None
-            if keep_inputs:
-                stage_inputs.append(residual)
-            if inline[q]:
-                if not book._initted_host:   # k-means init precedes the search (quantize_rows would run it next)
-                    book.init_embed_(book.transform_input(residual).float())
-                inline_embeds.append(book.embed[0].clone())
-            want_loss = training and self.layers[q].has_commitment_loss
-            book.quantize_rows(
-                residual, update=do_update[q], idx64_out=all_idx[:, q], idx_stride=Q,
-                loss_out=losses[q:q + 1] if want_loss else None, loss_weight=self.layers[q].commitment_weight,
-                resid_out=nxt, stats_out=packed[offs[q]:offs[q] + stat_sizes[q]] if stat_sizes[q] else None,
-                defer_ema=not inline[q])
-            residual = nxt
+        return self._tail(x, masked, quantized, indices, losses, return_all_codes)
 
-        # quantized_out (rvq:410, :525): rebuilt from the indices of the stages that ran, in one pass over the codebooks they
-        # searched, instead of a read-modify-write of (N x D) in every stage.  Only inline stages change a codebook between
-        # stages; every other update is deferred to _finish_update below.  Codebooks of different sizes are zero-padded to
-        # the largest: every index of a stage is below its own size.
-        if inline_embeds:
-            searched = torch.stack(inline_embeds)
-        elif self.shared_codebook:
-            searched = books[0].embed[0]
-        else:
-            searched = torch.nn.utils.rnn.pad_sequence([b.embed[0] for b in books[:n_run]], batch_first=True)
-        quantized_out = ops.rvq_accumulate(searched, all_idx[:, :n_run].contiguous(), dtype)
-
-        if packed is not None or any(inline):
-            if _stats_sink is not None:  # GroupedResidualVQ gathers every group's statistics into one collective
-                _stats_sink.append((self, packed, offs, stat_sizes, do_update, (stage_inputs, shape, peer_ptrs)))
-            else:
-                self._finish_update(packed, offs, stat_sizes, do_update, (stage_inputs, shape, peer_ptrs), synced=False)
-
-        quantized_out = quantized_out.reshape(shape)
-        if self.diveq:   # rvq:603-606, in every mode
-            quantized_out = directional_reparam(x, quantized_out)
-        if not _projected:
-            quantized_out = self.project_out(quantized_out)  # rvq:610
-        ret = (quantized_out, all_idx.reshape(*shape[:-1], Q), losses.clone())
+    def _tail(self, x, masked, quantized, indices, losses, return_all_codes):
+        """Rows out: the compacted rows scattered into zeros / index -1 (vqp:1378-1396), DiVeQ (rvq:603-606, in every mode),
+        project_out (rvq:610) and the codes of `return_all_codes`."""
+        shape = x.shape
+        if masked is not None:
+            rows, quantized_all, indices_all = masked
+            if rows.numel() > 0:
+                quantized_all[rows] = quantized
+                indices_all[rows] = indices
+            quantized, indices = quantized_all, indices_all
+        quantized = quantized.reshape(shape)
+        if self.diveq:
+            quantized = directional_reparam(x, quantized)
+        ret = (self.project_out(quantized), indices.reshape(*shape[:-1], self.num_quantizers), losses)
         if return_all_codes:
             ret = (*ret, self.get_codes_from_indices(ret[1]))
         return ret
@@ -400,87 +461,48 @@ class ResidualVQ(nn.Module):
     def _active_layers(self, fixed_seed, device) -> int:
         """Number of leading layers that quantize in this forward.  Training with quantize_dropout (rvq:423-439): python's
         random.Random(seed).randrange(cutoff, Q) is the last active layer, rounded up to a multiple if asked; without an explicit
-        seed one is drawn like the reference's get_maybe_sync_seed (rvq:96-103: torch.randint on the device, all-reduced, .item())."""
+        seed one is drawn like the reference's get_maybe_sync_seed."""
         Q = self.num_quantizers
         if not (self.training and self.quantize_dropout):
             return Q
         if fixed_seed is None:
-            seed = torch.randint(0, 10_000, (), device=device)
-            if distributed.is_available() and distributed.is_initialized() and distributed.get_world_size() > 1:
-                distributed.all_reduce(seed)
-            fixed_seed = seed.item()
+            fixed_seed = _sync_seed(device).item()
         index = random.Random(fixed_seed).randrange(self.quantize_dropout_cutoff_index, Q)
         mult = self.quantize_dropout_multiple_of
         if mult != 1:
             index = math.ceil((index + 1) / mult) * mult - 1  # rvq:39-40, :439
         return min(index + 1, Q)
 
-    def _forward_masked(self, x, mask, return_all_codes, freeze_codebook, dropout_seed=None):
-        """mask (B, N) bool.  The reference hands the mask to every layer (rvq:495): a layer searches every row, but masked rows
-        take no part in its statistics or loss (vqp:599-600, :1317-1325) and come back as zeros / index -1 (vqp:1378-1396), so their
-        residual is never reduced and their running sum stays zero.  That is exactly the forward over the COMPACTED unmasked rows
-        with zeros / -1 scattered around it — which is what runs here (stage-wise path: the compacted row count changes from call
-        to call, a cached program per count would not pay).  project_in / project_out see every row (rvq:406, :610)."""
-        books = self._stage_plan()
-        if any(b.learnable_codebook for b in books):
-            _unsupported("ResidualVQ.forward(mask=) with learnable codebooks")
-        if any(b.use_cosine_sim for b in books):
-            _unsupported("ResidualVQ.forward(mask=) with use_cosine_sim (the masked loss is taken against the un-normalised input, vqp:1319)")
-        if any(not vq.return_zeros_for_masked_padding for vq in self.layers):
-            _unsupported("ResidualVQ.forward(mask=) with return_zeros_for_masked_padding=False")
-        if self.training and any(b.has_dead_code_replacement for b in books):
-            _unsupported("ResidualVQ.forward(mask=) with dead-code replacement")
-        xp = self.project_in(x)  # rvq:406
-        if xp.requires_grad and torch.is_grad_enabled():
-            _unsupported("ResidualVQ.forward(mask=) on inputs / projections that require grad")
-        assert xp.ndim == 3 and mask.shape == xp.shape[:2]
-        B, N, D = xp.shape
-        Q = self.num_quantizers
-        rows = mask.reshape(-1).nonzero(as_tuple=True)[0]  # host sync (the reference's masked path syncs as well)
-        quantized = torch.zeros((B * N, D), dtype=xp.dtype, device=xp.device)
-        all_idx = torch.full((B * N, Q), -1, dtype=torch.int64, device=xp.device)
-        if rows.numel() > 0:
-            xc = xp.detach().reshape(-1, D)[rows].unsqueeze(0)
-            qc, ic, losses = self.forward(xc, freeze_codebook=freeze_codebook, _projected=True,
-                                          rand_quantize_dropout_fixed_seed=dropout_seed)
-            quantized[rows] = qc[0]
-            all_idx[rows] = ic[0]
-        else:
-            losses = torch.zeros((Q,), dtype=torch.float32, device=xp.device)
-        ret = (self.project_out(quantized.reshape(B, N, D)), all_idx.reshape(B, N, Q), losses)  # rvq:610
-        if return_all_codes:
-            ret = (*ret, self.get_codes_from_indices(ret[1]))
-        return ret
-
     def _codebooks_need_grad(self):
         return any(vq._codebook.embed.requires_grad for vq in self.layers)
 
     def _program_ok(self, books, do_update):
         """One-call path (ops.RvqProgram): every stage deferred, no collective, no dead-code expiry, nothing parked on `.grad`
-        (accum_ema_update), codebooks initialised and stackable."""
-        if os.environ.get("VQB_RVQ_PROGRAM", "1") == "0":
-            return False
-        if ops.PROFILE_EVENTS is not None or not self.uniform_codebook_size:
-            return False
+        (accum_ema_update), codebooks initialised and stackable.  Returns the program's op count (stages, running sum, one EMA
+        op per updated stage, peer barrier, update_ema of a shared codebook), 0 when the forward cannot run as a program."""
         n_ops = len(books) + 1 + sum(do_update) + 2
+        if os.environ.get("VQB_RVQ_PROGRAM", "1") == "0":
+            return 0
+        if ops.PROFILE_EVENTS is not None or not self.uniform_codebook_size:
+            return 0
         if n_ops > ops.RvqProgram.MAX_OPS:
-            return False
+            return 0
         for b, u in zip(books, do_update):
             if not b._initted_host:
-                return False
+                return 0
             if u and (b.has_dead_code_replacement or b.cluster_size.grad is not None or b.embed_avg.grad is not None):
-                return False
+                return 0
         ddp = [b.use_ddp for b, u in zip(books, do_update) if u]
         if any(ddp):
             # multi-GPU: the statistics go to symmetric memory and the EMA ops sum over the ranks (barrier + peer loads inside
             # the program); without peer memory the stage-wise path does ONE NCCL all-reduce instead
             if not all(ddp):
-                return False
+                return 0
             dev, D = books[0].embed.device, books[0].embed.shape[-1]
             numel = sum(ops.stats_floats(b.codebook_size, D) for b, u in zip(books, do_update) if u)
             if self._peer_reducer(numel, dev) is None:
-                return False
-        return True
+                return 0
+        return n_ops
 
     def _ensure_loss_buf(self, dev):
         """Per-stage losses land in a persistent buffer (stable pointers for the graph cache); callers get a clone."""
@@ -497,51 +519,69 @@ class ResidualVQ(nn.Module):
         return (tuple(flat.shape), flat.dtype, flat.device, self.training, tuple(do_update), None if peer is None else peer.step & 1,
                 tuple((id(b), id(b.operands()), b.embed.data_ptr(), b.cluster_size.data_ptr(), b.embed_avg.data_ptr()) for b in books))
 
-    def _plan_part(self, prog, lane, flat, books, do_update, persistent_io=False):
-        return _PlanPart(self, prog, lane, flat, books, do_update, persistent_io)
+    def _quantize_stagewise(self, flat, books, do_update, n_run, freeze_codebook, rows0, pending):
+        """One search call per active stage (rvq:469); the codebook updates follow the running sum."""
+        N, D = flat.shape
+        Q = self.num_quantizers
+        dev = flat.device
+        training = self.training
+        losses = self._ensure_loss_buf(dev)
+        if n_run < Q:   # rvq:473-476: the skipped layers report index -1 and loss 0
+            all_idx = torch.full((N, Q), -1, dtype=torch.int64, device=dev)
+            losses.zero_()
+        else:
+            all_idx = torch.empty((N, Q), dtype=torch.int64, device=dev)
+        if not training:
+            losses.zero_()
+        # dead-code expiry samples from the stage inputs after the (deferred) EMA update: keep them all then
+        keep_inputs = training and not freeze_codebook and any(b.has_dead_code_replacement for b in books)
+        bufs = [torch.empty_like(flat) for _ in range(Q - 1 if keep_inputs else min(2, Q - 1))]
+        updates = _CodebookUpdates(self, books, do_update, D, dev)
+        updates.begin()
+        updates.rows0 = rows0
+        residual = flat  # rvq:411 (never written: stage 0 reads the caller's tensor)
+        inline_embeds = []   # the shared codebook as each inline stage searched it
+        for q, book in enumerate(books[:n_run]):  # rvq:469
+            nxt = (bufs[q] if keep_inputs else bufs[q & 1]) if q + 1 < n_run else None
+            if keep_inputs:
+                updates.stage_inputs.append(residual)
+            if updates.inline[q]:
+                if not book._initted_host:   # k-means init precedes the search (quantize_rows would run it next)
+                    book.init_embed_(book.transform_input(residual).float())
+                inline_embeds.append(book.embed[0].clone())
+            want_loss = training and self.layers[q].has_commitment_loss
+            book.quantize_rows(
+                residual, update=do_update[q], idx64_out=all_idx[:, q], idx_stride=Q,
+                loss_out=losses[q:q + 1] if want_loss else None, loss_weight=self.layers[q].commitment_weight,
+                resid_out=nxt, stats_out=updates.stats(q), defer_ema=not updates.inline[q])
+            residual = nxt
 
-    def _finish_update(self, packed, offs, stat_sizes, do_update, stage_inputs, synced):
-        """ONE all-reduce for all stages (reference: 2 per stage, vqp:603/:607), then the per-stage lerps in
-        order (vqp:616-617) and update_ema — once at the end for a shared codebook (rvq:593-597) — and the dead-code
-        expiry: per stage from that stage's input (vqp:641), for a shared codebook once over all residuals (rvq:599-601).
-        stage_inputs: (the Q stage inputs (N, D) — kept only when some codebook replaces dead codes —, input shape)."""
-        stage_inputs, shape, peer_ptrs = stage_inputs
-        books = self._stage_plan()
-        peer = self._peer if peer_ptrs is not None else None
-        if peer is not None:
-            peer.barrier()       # every rank's statistics of this forward are in place
-        elif not synced and packed is not None and any(b.use_ddp for b in books):
-            allreduce_packed(packed)
-        for q, book in enumerate(books):
-            if not do_update[q] or not stat_sizes[q]:   # nothing to do, or already applied inline
-                continue
-            normalise = book.ema_update and not book.manual_ema_update
-            if peer is not None:
-                book.lerp_stats_peers(peer, peer_ptrs, offs[q], normalise)
+        # quantized_out (rvq:410, :525): rebuilt from the indices of the stages that ran, in one pass over the codebooks they
+        # searched, instead of a read-modify-write of (N x D) in every stage.  Only inline stages change a codebook between
+        # stages.  Codebooks of different sizes are zero-padded to the largest: every index of a stage is below its own size.
+        if inline_embeds:
+            searched = torch.stack(inline_embeds)
+        elif self.shared_codebook:
+            searched = books[0].embed[0]
+        else:
+            searched = torch.nn.utils.rnn.pad_sequence([b.embed[0] for b in books[:n_run]], batch_first=True)
+        quantized = ops.rvq_accumulate(searched, all_idx[:, :n_run].contiguous(), flat.dtype)
+
+        if any(do_update):
+            if pending is not None:
+                pending.append(updates)
             else:
-                book.lerp_stats(packed[offs[q]:offs[q] + stat_sizes[q]], normalise=normalise)
-            if not self.shared_codebook and book.has_dead_code_replacement:
-                book.expire_codes_(book.transform_input(stage_inputs[q]).float())  # vqp:641 on the fp32 `flatten`
-        if self.training and self.shared_codebook:
-            shared = books[0]
-            if self.vq_is_ema_updating and any(do_update):
-                shared.update_ema()
-            if shared.has_dead_code_replacement and any(do_update):
-                # rvq:599-601 -> vqp:1051-1054 -> :573-574: the reference hands '(b) (n l) d' to Codebook.expire_codes_, whose
-                # 'h ... d -> h (...) d' reads the batch axis as the codebook axis, and `replace` zips it with the (1, K)
-                # mask: only batch element 0's rows (n-major, stage-minor) are sampled from.  Reproduced as is.
-                n0 = stage_inputs[0].shape[0] // shape[0] if len(shape) > 2 else stage_inputs[0].shape[0]
-                rows = torch.stack([r[:n0] for r in stage_inputs], dim=1).reshape(-1, stage_inputs[0].shape[-1])
-                shared.expire_codes_(shared.transform_input(rows))
+                _CodebookUpdates.apply_all([updates])
+        return quantized, all_idx, losses.clone()
 
-    def _forward_layered(self, x, freeze_codebook, return_all_codes, n_run=None):
+    def _quantize_layered(self, x, freeze_codebook, n_run):
         """Differentiable path: the reference's Python loop (rvq:469-568) over our VectorQuantize layers.
-        `x` is already projected (rvq:406).  n_run < Q: quantize dropout (rvq:473-476)."""
+        n_run < Q: quantize dropout (rvq:473-476)."""
         quantized_out = torch.zeros_like(x)
         residual = x
         all_idx, all_losses = [], []
         for q, vq in enumerate(self.layers):
-            if n_run is not None and q >= n_run:
+            if q >= n_run:
                 all_idx.append(torch.full(x.shape[:-1], -1, dtype=torch.int64, device=x.device))
                 all_losses.append(torch.zeros((), dtype=torch.float32, device=x.device))
                 continue
@@ -552,12 +592,8 @@ class ResidualVQ(nn.Module):
             all_losses.append(loss)
         if self.training and self.shared_codebook and self.vq_is_ema_updating and not freeze_codebook:
             self.layers[0]._codebook.update_ema()
-        if self.diveq:   # rvq:603-606: every stage's codebook gets the DiVeQ gradient of quantized_out
-            quantized_out = directional_reparam(x, quantized_out)
-        ret = (self.project_out(quantized_out), torch.stack(all_idx, dim=-1), torch.stack(all_losses))
-        if return_all_codes:
-            ret = (*ret, self.get_codes_from_indices(ret[1]))
-        return ret
+        D, Q = x.shape[-1], self.num_quantizers
+        return quantized_out.reshape(-1, D), torch.stack(all_idx, dim=-1).reshape(-1, Q), torch.stack(all_losses)
 
 
 class GroupedResidualVQ(nn.Module):
@@ -585,24 +621,21 @@ class GroupedResidualVQ(nn.Module):
     def get_output_from_indices(self, indices):
         return torch.cat(tuple(rvq.get_output_from_indices(i) for rvq, i in zip(self.rvqs, indices)), dim=-1)
 
-    def _program_ok(self, chunks, freeze_codebook):
-        """All groups in one ops.RvqProgram: every group qualifies (ResidualVQ._program_ok), no gradient path, and the op list fits."""
-        if torch.is_grad_enabled() and (any(c.requires_grad for c in chunks) or any(r._codebooks_need_grad() for r in self.rvqs)):
-            return False
-        if any(rvq.diveq for rvq in self.rvqs):
-            return False
-        total = 0
-        for rvq, c in zip(self.rvqs, chunks):
-            if not c.is_cuda or c.dtype not in (torch.float32, torch.bfloat16):
-                return False
-            if torch.is_grad_enabled() and any(p.requires_grad for p in rvq.project_in.parameters()):
-                return False
+    def _program_ok(self, xs, freeze_codebook):
+        """All groups in one ops.RvqProgram: every group takes its own program path (ResidualVQ._program_ok), and the op list
+        fits.  Returns every group's (codebooks, stages that update), or None."""
+        if any(rvq.diveq or rvq._takes_layered(x) or not x.is_cuda or x.dtype not in _DTYPES for rvq, x in zip(self.rvqs, xs)):
+            return None
+        plan, n_ops = [], 0
+        for rvq in self.rvqs:
             books = rvq._stage_plan()
-            upd = [b.updates(rvq.training, freeze_codebook) for b in books]
-            if not rvq._program_ok(books, upd):
-                return False
-            total += len(books) + 1 + sum(upd) + 2
-        return total <= ops.RvqProgram.MAX_OPS
+            upd = rvq._do_update(books, freeze_codebook, rvq.num_quantizers)
+            n = rvq._program_ok(books, upd)
+            if not n:
+                return None
+            plan.append((books, upd))
+            n_ops += n
+        return plan if n_ops <= ops.RvqProgram.MAX_OPS else None
 
     def forward(self, x, indices=None, return_all_codes=False, sample_codebook_temp=None, freeze_codebook=False, mask=None):
         if indices is not None:
@@ -612,60 +645,25 @@ class GroupedResidualVQ(nn.Module):
         if self.training:
             # the reference draws one torch.randint here even without quantize-dropout (rvq:701 -> :96-103);
             # consume it too so that seeded runs stay aligned with the reference's RNG stream.
-            seed = torch.randint(0, 10_000, (), device=x.device)
-            if distributed.is_available() and distributed.is_initialized() and distributed.get_world_size() > 1:
-                distributed.all_reduce(seed)
+            seed = _sync_seed(x.device)
         dropout_seed = None
         if self.training and any(rvq.quantize_dropout for rvq in self.rvqs):
             dropout_seed = int(seed.item())   # rvq:701: the SAME dropout index in every group
-        if mask is not None:   # rvq:698: every group receives the mask (ResidualVQ._forward_masked)
+        if mask is not None:   # rvq:698: every group receives the mask
             outs = [rvq(c, mask=mask, freeze_codebook=freeze_codebook, return_all_codes=return_all_codes,
                         rand_quantize_dropout_fixed_seed=dropout_seed) for rvq, c in zip(self.rvqs, chunks)]
-            sink = []
-        elif dropout_seed is None and self._program_ok(chunks, freeze_codebook):
-            # every group's stages in ONE vqb_rvq_forward call: the groups are independent chains on parallel lanes; the op
-            # list is cached, only the per-call pointers are patched
-            flats, keys = [], []
-            for rvq, c in zip(self.rvqs, chunks):
-                xin = rvq.project_in(c).detach()
-                flat = xin.reshape(-1, xin.shape[-1])     # a strided view of the group's columns: copied into the plan's buffer
-                books = rvq._stage_plan()
-                upd = [b.updates(rvq.training, freeze_codebook) for b in books]
-                rvq._ensure_loss_buf(flat.device)
-                flats.append((flat, xin.shape, books, upd))
-                keys.append(rvq._part_key(flat, books, upd))
-            key = tuple(keys)
-            plans = self.__dict__.setdefault("_plans", _PlanCache())
-            plan = plans.get(key)
-            if plan is None:
-                if len(plans) >= 8:
-                    plans.clear()
-                prog = ops.RvqProgram(x.device)
-                parts = [rvq._plan_part(prog, g % 4, f[0], f[2], f[3], persistent_io=True)
-                         for g, (rvq, f) in enumerate(zip(self.rvqs, flats))]
-                plan = plans[key] = (prog.freeze(), parts)
-            prog, parts = plan
-            bound = [part.bind(prog.arr, f[0]) for part, f in zip(parts, flats)]
-            prog.run()
-            outs = [part.finish(b, f[1], return_all_codes) for part, b, f in zip(parts, bound, flats)]
-            sink = []
         else:
-            sink = []
-            outs = [rvq(c, freeze_codebook=freeze_codebook, return_all_codes=return_all_codes, _stats_sink=sink,
-                        rand_quantize_dropout_fixed_seed=dropout_seed) for rvq, c in zip(self.rvqs, chunks)]  # rvq:706
-        if sink:
-            need_sync = any(b.use_ddp for rvq, *_ in sink for b in rvq._stage_plan()) and all(e[5][2] is None for e in sink)
-            if need_sync:  # no peer memory: ONE NCCL collective for every codebook of every group
-                flat_all = torch.cat([p for _, p, *_ in sink])
-                allreduce_packed(flat_all)
-                pos = 0
-                for rvq, packed, offs, sizes, upd, inputs in sink:
-                    n = packed.numel()
-                    rvq._finish_update(flat_all[pos:pos + n], offs, sizes, upd, inputs, synced=True)
-                    pos += n
+            xs = [rvq.project_in(c) for rvq, c in zip(self.rvqs, chunks)]
+            plan = self._program_ok(xs, freeze_codebook) if dropout_seed is None else None
+            if plan is not None:   # every group in ONE call; the groups' cat / stack copy the plan's persistent outputs
+                flats = [xp.detach().reshape(-1, xp.shape[-1]) for xp in xs]   # strided views of the groups' columns
+                outs = [rvq._tail(xp, None, *o, return_all_codes)
+                        for rvq, xp, o in zip(self.rvqs, xs, _run_program(self, self.rvqs, flats, plan, persistent_io=True))]
             else:
-                for rvq, packed, offs, sizes, upd, inputs in sink:
-                    rvq._finish_update(packed, offs, sizes, upd, inputs, synced=True)
+                pending = []
+                outs = [rvq._forward_projected(xp, None, return_all_codes, freeze_codebook, dropout_seed, pending)
+                        for rvq, xp in zip(self.rvqs, xs)]  # rvq:706
+                _CodebookUpdates.apply_all(pending)   # without peer memory: ONE NCCL collective for every group
         quantized = torch.cat([o[0] for o in outs], dim=-1)  # rvq:719-721
         all_indices = torch.stack([o[1] for o in outs])
         commit_losses = torch.stack([o[2] for o in outs])
