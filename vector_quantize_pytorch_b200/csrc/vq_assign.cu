@@ -21,6 +21,7 @@
 // over which the reference's own fp32 formula ties distinct codes (its sqrt collapse and, Euclid, its 1e-8 clamp floor);
 // otherwise (row, two best candidates, candidate count) goes to `flagged` and vqb_fix_flagged re-scores it with
 // the reference's exact formula (count > 3: whole-row rescan).  Conservative: may over-flag, never under-flag.
+#include <type_traits>
 #include "ptx.cuh"
 #include "vqb_common.cuh"
 #include "gather_row.cuh"
@@ -37,10 +38,10 @@ namespace vqb {
 
 constexpr int BM = 128;         // rows of x per tile
 constexpr int WM = 64;          // rows per consumer warpgroup (wgmma M)
-constexpr int WN = 128;         // codes per MMA step (wgmma N)
+constexpr int BN_STAGE = 128;   // codes per ring stage; a code step (wgmma N = WN, 128 or 256) spans WN / 128 stages
 constexpr int BK = 64;          // bf16 elements per 128-byte swizzle row
 constexpr int A_SUB_BYTES = BM * BK * 2;  // 16 KiB: one (plane, k-block) sub-tile of A
-constexpr int B_SUB_BYTES = WN * BK * 2;  // 16 KiB: one (plane, k-block) sub-tile of a code step
+constexpr int B_SUB_BYTES = BN_STAGE * BK * 2;  // 16 KiB: one ring stage, 128 codes of one (plane, k-block)
 constexpr int MAX_A_SUB = 8;    // n_a * ceil(D/64) <= 8  -> A <= 128 KiB
 constexpr int MAX_STAGES = 8;
 constexpr int NUM_CONSUMER_WARPS = 8;   // two warpgroups
@@ -48,15 +49,16 @@ constexpr int NUM_STORE_WARPS = 3;      // warps 1..3 (warp 0 is the TMA produce
 constexpr int NUM_THREADS = 128 + NUM_CONSUMER_WARPS * 32;
 constexpr int SMEM_CTRL_BYTES = 14336;  // barriers + winner hand-off + merge area
 constexpr int SMEM_LIMIT = 232448;      // 227 KiB opt-in maximum per CTA
-constexpr int SEED_BYTES = WN * 32;     // one code step of bext ([128 codes][16] bf16): B of the step's bias MMA
+constexpr int SEED_BYTES = BN_STAGE * 32;   // bext of 128 codes ([128][16] bf16); a seed slot holds WN / 128 of them:
+                                            // B of the step's bias MMA
 
 struct AssignParams {
   int64_t N;
   int D, K, Kpad;
   int n_a, n_passes;   // pass 0 (a0,c_hi), 1 (a0,c_lo), 2 (a1,c_hi): bf16 operands, fp32 accumulation
   int KB;              // ceil(D / 64)
-  int n_stages;
-  int n_seed;          // seed slots: ceil(n_stages / items per code step), so that a slot is refilled only after every
+  int n_stages;        // ring stages of 16 KiB; an item of a 256-code step takes two adjacent ones
+  int n_seed;          // seed slots: ceil(ring items / items per code step), so that a slot is refilled only after every
                        // consumer released the first item of the step that last used it
   int stream_a;        // A does not fit in smem next to a useful B ring (fp32 split input with D > 256): its k-blocks travel
                        // through the ring together with the codebook k-blocks (re-read from L2 for every code step)
@@ -89,6 +91,7 @@ struct Ctrl {  // lives at the start of dynamic smem
   uint64_t g_full[2], g_empty[2];        // winners of a row tile handed to the store warps
   int gidx[2][BM];                       // certified winner per row (-1: flagged / out of range)
   MergeSlot merge[BM][3];                // slices 1..3 of each row, published for the quad's lane 0
+  float x2[BM];                          // ||x||^2 of each row of the tile (kept out of the consumers' registers)
 };
 static_assert(sizeof(Ctrl) <= SMEM_CTRL_BYTES, "control block too large");
 
@@ -120,26 +123,61 @@ __device__ __forceinline__ float sq_diff16(const uint4& xa, const uint4& ca, boo
   return s;
 }
 
+// What the 256-code step keeps in static shared memory rather than in registers (its 128 accumulators leave 40 for
+// everything else; ptxas of CUDA 12.9 needs both moves to stay at 168 registers with no spill):
+//  - the per-thread sum of the commitment loss read off the scores (touched once per row);
+//  - A of the bias MMA, a 64 x 16 bf16 tile of ones read from shared memory: the register form of that MMA needs four
+//    A registers at the point where the accumulators are allocated.  Ones in every column are exact here: the bext
+//    columns past the three bias terms are zero.
+// The 128-code step keeps both in registers and has no static shared memory (its tightest plan uses all 227 KiB).
+template <int WN>
+struct StepLocals {
+  float loss_ = 0.f;
+  __device__ __forceinline__ float& loss() { return loss_; }
+};
+template <>
+struct StepLocals<256> {
+  static __device__ __forceinline__ float& loss() {
+    __shared__ float s[NUM_CONSUMER_WARPS * 32];
+    return s[threadIdx.x - 128];
+  }
+  static __device__ __forceinline__ uint32_t* bias_ones() {   // [64 rows][16] bf16 1.0, 32-byte swizzle (any layout: all ones)
+    __shared__ __align__(256) uint32_t o[WM * 16 / 2];
+    return o;
+  }
+  __device__ __forceinline__ StepLocals() { loss() = 0.f; }
+};
+constexpr int WIDE_STATIC_SMEM = NUM_CONSUMER_WARPS * 32 * 4 + WM * 16 * 2;   // 1 KiB + 2 KiB
+
 // TAIL selects the work of the store warps at compile time (one instantiation each: the variants do not share a register
 // budget): 0 = none / generic (x re-read: running sum, cosine residual), 1 = copy mode, 2 = resid mode.
-template <int TAIL>
+// WN = codes per code step (wgmma N): 128, or 256 where the launch plan allows it (wide_step below).  A 256-code step pays
+// the drain, the quad's shuffles and the restart of the MMA pipe once per 256 codes instead of once per 128, and reads A
+// from shared memory half as often.  Its item is two adjacent ring stages (codes 0..127 and 128..255 of one k-block),
+// filled by one 256-row TMA box on one barrier pair; its 128 accumulators leave no room for a register-resident live
+// group, so its scan keeps live groups in the thread-local queue (ScanState<16>).
+template <int TAIL, int WN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmS, const AssignParams p) {
+  static_assert(WN == 128 || WN == 256, "code step width");
+  constexpr int SPAN = WN / BN_STAGE;                  // ring stages per item
+  constexpr uint32_t STEP_SEED_BYTES = SPAN * SEED_BYTES;
   extern __shared__ __align__(1024) uint8_t smem[];
   Ctrl* ctrl = reinterpret_cast<Ctrl*>(smem);
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t a_base = (smem_base + SMEM_CTRL_BYTES + 1023u) & ~1023u;    // swizzled tiles need 1024 B alignment
-  const int n_sub = p.stream_a ? 0 : p.n_a * p.KB;                            // stationary A sub-tiles
+  const bool stream_a = WN == 128 && p.stream_a;                              // the wide step keeps A resident
+  const int n_sub = stream_a ? 0 : p.n_a * p.KB;                              // stationary A sub-tiles
   const uint32_t b_base = a_base + n_sub * A_SUB_BYTES;
-  // ring stage = [A k-block (stream_a only) | codebook k-block of the code step]
-  const uint32_t a_stage_bytes = p.stream_a ? A_SUB_BYTES : 0;
-  const uint32_t stage_stride = a_stage_bytes + B_SUB_BYTES;
-  const uint32_t seed_base = b_base + p.n_stages * stage_stride;             // [n_seed][128 codes][16] bf16
+  // ring item = [A k-block (stream_a only) | codebook k-block of the code step: SPAN stages of 128 codes, back to back]
+  const uint32_t a_stage_bytes = stream_a ? A_SUB_BYTES : 0;
+  const uint32_t stage_stride = a_stage_bytes + SPAN * B_SUB_BYTES;
+  const int n_ring = p.n_stages / SPAN;                                       // ring items (the plan's stage count is even for WN = 256)
+  const uint32_t seed_base = b_base + n_ring * stage_stride;                 // [n_seed][WN codes][16] bf16
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int my_tiles = (p.num_row_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
 
   // ------------------------------------------------------------------ one-time setup
   if (threadIdx.x == 0) {
@@ -150,7 +188,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       mbar_init(smem_u32(&ctrl->a_full[s]), 1);
       mbar_init(smem_u32(&ctrl->a_empty[s]), NUM_CONSUMER_WARPS);
     }
-    for (int s = 0; s < p.n_stages; ++s) {
+    for (int s = 0; s < n_ring; ++s) {
       mbar_init(smem_u32(&ctrl->b_full[s]), 1);
       mbar_init(smem_u32(&ctrl->b_empty[s]), NUM_CONSUMER_WARPS);
     }
@@ -159,6 +197,10 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       mbar_init(smem_u32(&ctrl->g_empty[s]), NUM_STORE_WARPS);
     }
     fence_barrier_init();
+  }
+  if constexpr (WN == 256) {
+    for (int i = threadIdx.x; i < WM * 16 / 2; i += NUM_THREADS) StepLocals<256>::bias_ones()[i] = 0x3F803F80u;
+    fence_proxy_async_shared();   // generic-proxy stores, read by wgmma
   }
   __syncthreads();
 
@@ -169,9 +211,9 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const long long pstart = PROF_CLOCK();
       int stage = 0, gstep = 0;
       uint32_t ph = 0;
-      for (int t = 0; t < my_tiles; ++t) {
-        const int row0 = (static_cast<int>(blockIdx.x) + t * static_cast<int>(gridDim.x)) * BM;
-        if (!p.stream_a && t + 1 < my_tiles) {   // the next tile's x into L2: its refill below then does not wait on HBM
+      for (int t = 0, tile = static_cast<int>(blockIdx.x); tile < p.num_row_tiles; ++t, tile += static_cast<int>(gridDim.x)) {
+        const int row0 = tile * BM;
+        if (!stream_a && tile + static_cast<int>(gridDim.x) < p.num_row_tiles) {   // the next tile's x into L2: its refill below then does not wait on HBM
           for (int ap = 0; ap < p.n_a; ++ap)
             for (int kb = 0; kb < p.KB; ++kb) tma_prefetch_l2_3d(&tmA, kb * BK, row0 + static_cast<int>(gridDim.x) * BM, ap);
         }
@@ -182,23 +224,29 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int ps = 0; ps < p.n_passes; ++ps) {
               const int bplane = (ps == 1) ? 1 : 0;
               const int aplane = (ps == 2) ? 1 : 0;
-              if (!p.stream_a && ct == 0 && (ps == 0 || ps == 2)) {  // refill this A sub-tile once the previous row tile released it
+              if (!stream_a && ct == 0 && (ps == 0 || ps == 2)) {  // refill this A sub-tile once the previous row tile released it
                 const int sub = aplane * p.KB + kb;
                 { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->a_empty[sub]), (t & 1) ^ 1); w_aempty += PROF_CLOCK() - c0; }
                 mbar_arrive_expect_tx(smem_u32(&ctrl->a_full[sub]), A_SUB_BYTES);
                 tma_load_3d(a_base + sub * A_SUB_BYTES, &tmA, smem_u32(&ctrl->a_full[sub]), kb * BK, row0, aplane);
               }
               { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_empty[stage]), ph ^ 1); w_empty += PROF_CLOCK() - c0; }
-              // the step's seeds ride on the barrier of its first item (a whole box: rows past Kpad are zero-filled)
+              // the step's seeds ride on the barrier of its first item (a whole box: rows past Kpad are zero-filled).
+              // Seed-slot reuse: slot gstep % n_seed was last read by the bias MMA of step gstep - n_seed, committed with
+              // that step's first item, n_seed * n_items ring items before this one.  The b_empty wait above proves that
+              // every consumer warp released the item n_ring items back, and releases run in item order, so with
+              // n_seed * n_items >= n_ring (n_seed = ceil(n_ring / n_items)) that first item — and the bias MMA — has
+              // completed.  The rule counts ring items, not stages: a 256-code item is one item on one barrier pair.
               const bool seeds = kb == 0 && ps == 0;
-              mbar_arrive_expect_tx(smem_u32(&ctrl->b_full[stage]), stage_stride + (seeds ? SEED_BYTES : 0));
+              mbar_arrive_expect_tx(smem_u32(&ctrl->b_full[stage]), stage_stride + (seeds ? STEP_SEED_BYTES : 0));
               if (seeds)
-                tma_load_3d(seed_base + (gstep % p.n_seed) * SEED_BYTES, &tmS, smem_u32(&ctrl->b_full[stage]), 0, ct * WN, 0);
-              if (p.stream_a)
+                tma_load_3d(seed_base + (gstep % p.n_seed) * STEP_SEED_BYTES, &tmS, smem_u32(&ctrl->b_full[stage]), 0, ct * WN, 0);
+              if (stream_a)
                 tma_load_3d(b_base + stage * stage_stride, &tmA, smem_u32(&ctrl->b_full[stage]), kb * BK, row0, aplane);
+              // one box of WN codes (the tensor map's box is WN rows): for WN = 256 it fills two adjacent 16 KiB stages
               tma_load_3d(b_base + stage * stage_stride + a_stage_bytes, &tmB, smem_u32(&ctrl->b_full[stage]), kb * BK,
                           ct * WN, bplane);
-              if (++stage == p.n_stages) { stage = 0; ph ^= 1; }
+              if (++stage == n_ring) { stage = 0; ph ^= 1; }
             }
           }
         }
@@ -213,8 +261,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // ================================================================ store warps: fused gather tail
     const int sw = warp - 1;
     float lsum = 0.f;
-    for (int t = 0; p.fo.enabled && t < my_tiles; ++t) {
-      const int tile = static_cast<int>(blockIdx.x) + t * static_cast<int>(gridDim.x);
+    for (int t = 0, tile = static_cast<int>(blockIdx.x); p.fo.enabled && tile < p.num_row_tiles; ++t, tile += static_cast<int>(gridDim.x)) {
       mbar_wait(smem_u32(&ctrl->g_full[t & 1]), (t >> 1) & 1);
       const int* gi = ctrl->gidx[t & 1];
       if (TAIL >= 1) {
@@ -317,43 +364,116 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int wg = (warp >> 2) - 1;                              // 0: rows 0..63, 1: rows 64..127
     const int q = lane & 3;                                      // column slice of the thread's rows
     const int rit0 = wg * WM + (warp & 3) * 16 + (lane >> 2);    // the thread's rows: rit0 and rit0 + 8
-    const float cmax = __ldg(p.cmax + CMAX_NORM);
-    // Exact norms of what the passes leave out of the codebook operand (code_operands.cuh): ||c - hi - lo||.  fp32 inputs
-    // (x = hi + lo + res, |res| <= 2^-8 |lo| per element) add x_res . c and the omitted x_lo . c_lo:  ||x_lo|| * caux.
-    const float cres = __ldg(p.cmax + CMAX_RES);
-    const float caux = p.n_a == 2 ? 0x1.02p-8f * cmax + __ldg(p.cmax + CMAX_LO) : 0.f;
     const int n_items = p.KB * p.n_passes;
     const uint32_t a_row_off = wg * WM * 128;          // this warpgroup's 64 rows inside an A sub-tile (1024 B aligned)
     // A of the bias MMA: 1 at k = 0, 1, 2 of every row, 0 elsewhere (the thread's fragment holds columns 2q, 2q + 1)
     const uint32_t bias_a = q == 0 ? 0x3F803F80u : (q == 1 ? 0x00003F80u : 0u);
     long long w_full = 0, w_afull = 0, w_gap = 0, gap0 = -1;   // gap: last commit of a step -> first wait of the next
     const long long cstart = PROF_CLOCK();
-    float acc[64];
+    float acc[WN / 2];
     int stage = 0, gstep = 0;
     uint32_t ph = 0;
-    float epi_loss = 0.f;
+    StepLocals<WN> locals;
     auto release = [&](int st, int sub) {   // this warp's MMAs of a ring stage (and A sub-tile) have completed
       if (lane == 0) {
         mbar_arrive(smem_u32(&ctrl->b_empty[st]));
         if (sub >= 0) mbar_arrive(smem_u32(&ctrl->a_empty[sub]));
       }
     };
-    for (int t = 0; t < my_tiles; ++t) {
-      const int tile = static_cast<int>(blockIdx.x) + t * static_cast<int>(gridDim.x);
-      ScanReg sc[2];               // hot-loop state of the two rows: running maximum + the live group, in registers
-      ScanQueue<16> sq[2];         // further live groups of a near tie (thread-local memory, rarely touched)
-      float x2[2] = {0.f, 0.f}, xlo[2] = {0.f, 0.f};
+    // ||x||^2 of the thread's two rows (the quad splits each row), from the bf16 planes in global memory (L2: the TMA
+    // just read them, or the producer prefetched them).  fp32 accumulation: the norm scales the certification band AND
+    // carries the commitment loss (sum ||q - x||^2 = sum ||x||^2 - 2 score), so it must be as exact as the scores.
+    // ||x||^2 goes to shared memory for the merge, ||x_lo||^2 to xlo.  WN = 128 runs this under the first code step's
+    // last MMAs; the 256-code step's accumulators leave no registers for it there, so WN = 256 runs it before the
+    // tile's first MMA (the rows are in L2: prefetched one tile ahead).
+    auto row_norms = [&](int tile, float (&xlo)[2]) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = static_cast<int64_t>(tile) * BM + rit0 + 8 * h;
+        float a = 0.f, alo = 0.f;
+        if (row < p.N) {
+          const uint16_t* hp = p.a_global + row * p.D;
+          for (int c = q * 8; c < p.D; c += 32) {
+            const uint4 u = __ldg(reinterpret_cast<const uint4*>(hp + c));
+            uint4 l = make_uint4(0u, 0u, 0u, 0u);
+            if (p.n_a == 2) l = __ldg(reinterpret_cast<const uint4*>(hp + p.N * p.D + c));
+            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+            const uint32_t wl[4] = {l.x, l.y, l.z, l.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float h0 = __uint_as_float(w[e] << 16), h1 = __uint_as_float(w[e] & 0xFFFF0000u);
+              const float l0 = __uint_as_float(wl[e] << 16), l1 = __uint_as_float(wl[e] & 0xFFFF0000u);
+              a = fmaf(h0 + l0, h0 + l0, a);
+              a = fmaf(h1 + l1, h1 + l1, a);
+              alo = fmaf(l0, l0, alo);
+              alo = fmaf(l1, l1, alo);
+            }
+          }
+        }
+        a += __shfl_xor_sync(0xffffffffu, a, 1);
+        a += __shfl_xor_sync(0xffffffffu, a, 2);
+        alo += __shfl_xor_sync(0xffffffffu, alo, 1);
+        alo += __shfl_xor_sync(0xffffffffu, alo, 2);
+        if (q == 0) ctrl->x2[rit0 + 8 * h] = a;
+        xlo[h] = alo;   // squared: the sqrt (a subroutine call) waits until no wgmma is in flight
+      }
+    };
+    // The certification band W of the thread's two rows (after row_norms; the sqrt is a subroutine call, which must not
+    // sit where a wgmma is in flight), and a fresh scan state.
+    auto init_band = [&](auto (&sc)[2], float (&xlo)[2]) {
+      const bool euclid = p.metric != VQB_METRIC_COSINE;
+      const float cmax = __ldg(p.cmax + CMAX_NORM);
+      // Exact norms of what the passes leave out of the codebook operand (code_operands.cuh): ||c - hi - lo||.  fp32 inputs
+      // (x = hi + lo + res, |res| <= 2^-8 |lo| per element) add x_res . c and the omitted x_lo . c_lo:  ||x_lo|| * caux.
+      const float cres = __ldg(p.cmax + CMAX_RES);
+      const float caux = p.n_a == 2 ? 0x1.02p-8f * cmax + __ldg(p.cmax + CMAX_LO) : 0.f;
+      __syncwarp();   // the quad's lane 0 wrote the norms
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float x2 = ctrl->x2[rit0 + 8 * h];
+        // band = 2 * (MMA error bound) + 2 * (tag perturbation: 16 ulp <= 2^-19 |score|, |score| <= |x||c| + |c|^2/2)
+        // + (Euclid) the width over which the reference's own evaluation collapses distinct d^2 into one distance:
+        // d = sqrt(fl(fl(x2 + y2) - 2xy)) has ~d^2 * 2^-23 of resolution in d^2 (vqp:58-62); with a small-norm codebook
+        // (the default init) that exceeds the MMA band.  Rows inside it go to the exact re-score, which evaluates the
+        // reference formula including the sqrt.  In score units (d^2 / 2), with a 2x safety factor.
+        // 2 * |score error|: what the passes leave out of the codebook (||x|| * cres) and of the row (xaux * caux), both by
+        // Cauchy-Schwarz on exact norms; the fp32 accumulation in the tensor core (margin_rel relative to ||x|| max||c||,
+        // 2^-20 relative to the bias the bias MMA sums); then the tag slack and the sqrt-collapse width.
+        // Last (Euclid), the clamp floor: the reference clamps d^2 at 1e-8 before the sqrt (vqp:58-62), so every code with
+        // fp32 d^2 <= 1e-8 scores -1e-4 and the lowest such index wins, although their exact scores differ by up to
+        // (1e-8 + the d^2 rounding) / 2.  The norm-scaled terms above are narrower than that once ||x|| and max||c|| fall
+        // to ~1e-2 (late ResidualVQ stages, zero residuals); 1e-8 keeps those codes inside the band, and the band of a
+        // normal-norm codebook (~1e-5 and up) does not notice it.
+        const float xn = sqrtf(x2);
+        const float xc = xn * cmax;
+        xlo[h] = p.n_a == 2 ? sqrtf(xlo[h]) * 1.0001f : 0.f;
+        sc[h].init(2.f * (xn * cres + xlo[h] * caux + p.margin_rel * xc + (euclid ? 0x1p-21f * cmax * cmax : 0.f)) +
+                   0x1p-18f * (xc + (euclid ? 0.5f * cmax * cmax : 0.f)) +
+                   (euclid ? 0x1p-22f * (x2 + cmax * cmax) + 1e-8f : 1e-30f));
+      }
+    };
+    for (int t = 0, tile = static_cast<int>(blockIdx.x); tile < p.num_row_tiles; ++t, tile += static_cast<int>(gridDim.x)) {
+      // hot-loop state of the two rows: running maximum (+ for WN = 128 the live group, in registers)
+      typename std::conditional<WN == 128, ScanReg, ScanState<16>>::type sc[2];
+      ScanQueue<16> sq[2];         // (further) live groups (thread-local memory, rarely touched)
 
+      float xlo[2] = {0.f, 0.f};
       for (int ct = 0; ct < p.num_code_steps; ++ct) {
         const bool last_ct = ct == p.num_code_steps - 1;
         // The bias MMA (scale-d = 0) sets the accumulators to -0.5||c||^2 (Euclid; 0 for cosine, -3e38 for padding codes):
         // A = [1 1 1 0 ...] times the step's bext rows, which the producer loaded into a seed slot on the barrier of the
         // step's first item; b1 + b2 + b3 is exact in fp32.  It is committed with item 0, so the release of item 0's
         // stage also proves that the slot has been read.
+        if (WN == 256 && ct == 0) {   // no accumulator is live and no wgmma in flight
+          row_norms(tile, xlo);
+          init_band(sc, xlo);
+        }
         if (gap0 >= 0) w_gap += PROF_CLOCK() - gap0;
         { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_full[stage]), ph); w_full += PROF_CLOCK() - c0; }
         wgmma_fence();
-        wgmma_m64n128k16_bf16_rs_set(acc, bias_a, wgmma_desc_sw32(seed_base + (gstep % p.n_seed) * SEED_BYTES));
+        const uint64_t sd = wgmma_desc_sw32(seed_base + (gstep % p.n_seed) * STEP_SEED_BYTES);
+        if constexpr (WN == 128) wgmma_m64n128k16_bf16_rs_set(acc, bias_a, sd);
+        else wgmma_m64n256k16_bf16_ss_set(acc, wgmma_desc_sw32(smem_u32(StepLocals<256>::bias_ones())), sd);
         // Items of a code step in k-block-major order (kb, ps) — the order the producer stages them in.  One wgmma group
         // stays in flight: the stage of item i - 1 is released once item i has been issued.
         int kb = 0, ps = 0;
@@ -361,104 +481,49 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = 0; i < n_items; ++i) {
           const int aplane = (ps == 2) ? 1 : 0;
           const int sub = aplane * p.KB + kb;
-          if (ct == 0 && !p.stream_a) { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->a_full[sub]), t & 1); w_afull += PROF_CLOCK() - c0; }
+          if (ct == 0 && !stream_a) { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->a_full[sub]), t & 1); w_afull += PROF_CLOCK() - c0; }
           if (i > 0) { const long long c0 = PROF_CLOCK(); mbar_wait(smem_u32(&ctrl->b_full[stage]), ph); w_full += PROF_CLOCK() - c0; }
           const uint32_t st_addr = b_base + stage * stage_stride;
-          const uint32_t a_addr = (p.stream_a ? st_addr : a_base + sub * A_SUB_BYTES) + a_row_off;
+          const uint32_t a_addr = (stream_a ? st_addr : a_base + sub * A_SUB_BYTES) + a_row_off;
           const uint64_t ad = wgmma_desc_sw128(a_addr);
-          const uint64_t bd = wgmma_desc_sw128(st_addr + a_stage_bytes);
+          const uint64_t bd = wgmma_desc_sw128(st_addr + a_stage_bytes);   // WN rows of 128 B, 8-row groups 1024 B apart
           fence_regs(acc);
           wgmma_fence();
           // four K=16 steps, descriptors advance by 32 B.  A ragged last k-block (D % 64 != 0) runs them all too: the TMA
           // zero-fills both operands past D, so the extra steps add exact zeros (a data-dependent step count would make
           // ptxas serialise the wgmmas)
-          wgmma_m64n128k16_bf16(acc, ad, bd);
-          wgmma_m64n128k16_bf16(acc, ad + 2, bd + 2);
-          wgmma_m64n128k16_bf16(acc, ad + 4, bd + 4);
-          wgmma_m64n128k16_bf16(acc, ad + 6, bd + 6);
+#pragma unroll
+          for (int k = 0; k < 8; k += 2) {
+            if constexpr (WN == 128) wgmma_m64n128k16_bf16(acc, ad + k, bd + k);
+            else wgmma_m64n256k16_bf16(acc, ad + k, bd + k);
+          }
           wgmma_commit();
           if (i == n_items - 1) gap0 = PROF_CLOCK();
           wgmma_wait<1>();
           fence_regs(acc);
           if (pend_stage >= 0) release(pend_stage, pend_sub);
-          const bool last_use = last_ct && !p.stream_a && (aplane == 1 ? ps == 2 : ps == 1);  // pass 1: the last one of a k-block on A plane 0
+          const bool last_use = last_ct && !stream_a && (aplane == 1 ? ps == 2 : ps == 1);  // pass 1: the last one of a k-block on A plane 0
           pend_stage = stage;
           pend_sub = last_use ? sub : -1;
-          if (++stage == p.n_stages) { stage = 0; ph ^= 1; }
+          if (++stage == n_ring) { stage = 0; ph ^= 1; }
           if (++ps == p.n_passes) { ps = 0; ++kb; }
         }
-        if (ct == 0) {
-          // ||x||^2 of the thread's two rows (the quad splits each row), from the bf16 planes in global memory (L2: the TMA
-          // just read them), while the last MMAs of the step run.  fp32 accumulation: the norm scales the certification band
-          // AND carries the commitment loss (sum ||q - x||^2 = sum ||x||^2 - 2 score), so it must be as exact as the scores.
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int64_t row = static_cast<int64_t>(tile) * BM + rit0 + 8 * h;
-            float a = 0.f, alo = 0.f;
-            if (row < p.N) {
-              const uint16_t* hp = p.a_global + row * p.D;
-              for (int c = q * 8; c < p.D; c += 32) {
-                const uint4 u = __ldg(reinterpret_cast<const uint4*>(hp + c));
-                uint4 l = make_uint4(0u, 0u, 0u, 0u);
-                if (p.n_a == 2) l = __ldg(reinterpret_cast<const uint4*>(hp + p.N * p.D + c));
-                const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-                const uint32_t wl[4] = {l.x, l.y, l.z, l.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float h0 = __uint_as_float(w[e] << 16), h1 = __uint_as_float(w[e] & 0xFFFF0000u);
-                  const float l0 = __uint_as_float(wl[e] << 16), l1 = __uint_as_float(wl[e] & 0xFFFF0000u);
-                  a = fmaf(h0 + l0, h0 + l0, a);
-                  a = fmaf(h1 + l1, h1 + l1, a);
-                  alo = fmaf(l0, l0, alo);
-                  alo = fmaf(l1, l1, alo);
-                }
-              }
-            }
-            a += __shfl_xor_sync(0xffffffffu, a, 1);
-            a += __shfl_xor_sync(0xffffffffu, a, 2);
-            alo += __shfl_xor_sync(0xffffffffu, alo, 1);
-            alo += __shfl_xor_sync(0xffffffffu, alo, 2);
-            x2[h] = a;
-            xlo[h] = alo;   // squared: the sqrt (a subroutine call) waits until no wgmma is in flight
-          }
-        }
+        if (WN == 128 && ct == 0) row_norms(tile, xlo);   // while the last MMAs of the step run
         wgmma_wait<0>();
         fence_regs(acc);
         release(pend_stage, pend_sub);
         ++gstep;
         if ((ct + 1) * WN > p.Kpad) {   // tiny codebooks: codes past Kpad (zero-filled seeds and operands) score -3e38
 #pragma unroll
-          for (int j = 0; j < 16; ++j)
+          for (int j = 0; j < WN / 8; ++j)
 #pragma unroll
             for (int b = 0; b < 2; ++b)
               if (ct * WN + 8 * j + 2 * q + b >= p.Kpad) { acc[4 * j + b] = -3.0e38f; acc[4 * j + 2 + b] = -3.0e38f; }
         }
 
-        if (ct == 0) {
-          const bool euclid = p.metric != VQB_METRIC_COSINE;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            // band = 2 * (MMA error bound) + 2 * (tag perturbation: 16 ulp <= 2^-19 |score|, |score| <= |x||c| + |c|^2/2)
-            // + (Euclid) the width over which the reference's own evaluation collapses distinct d^2 into one distance:
-            // d = sqrt(fl(fl(x2 + y2) - 2xy)) has ~d^2 * 2^-23 of resolution in d^2 (vqp:58-62); with a small-norm codebook
-            // (the default init) that exceeds the MMA band.  Rows inside it go to the exact re-score, which evaluates the
-            // reference formula including the sqrt.  In score units (d^2 / 2), with a 2x safety factor.
-            // 2 * |score error|: what the passes leave out of the codebook (||x|| * cres) and of the row (xaux * caux), both by
-            // Cauchy-Schwarz on exact norms; the fp32 accumulation in the tensor core (margin_rel relative to ||x|| max||c||,
-            // 2^-20 relative to the bias the bias MMA sums); then the tag slack and the sqrt-collapse width.
-            // Last (Euclid), the clamp floor: the reference clamps d^2 at 1e-8 before the sqrt (vqp:58-62), so every code with
-            // fp32 d^2 <= 1e-8 scores -1e-4 and the lowest such index wins, although their exact scores differ by up to
-            // (1e-8 + the d^2 rounding) / 2.  The norm-scaled terms above are narrower than that once ||x|| and max||c|| fall
-            // to ~1e-2 (late ResidualVQ stages, zero residuals); 1e-8 keeps those codes inside the band, and the band of a
-            // normal-norm codebook (~1e-5 and up) does not notice it.
-            const float xn = sqrtf(x2[h]);
-            const float xc = xn * cmax;
-            xlo[h] = p.n_a == 2 ? sqrtf(xlo[h]) * 1.0001f : 0.f;
-            sc[h].init(2.f * (xn * cres + xlo[h] * caux + p.margin_rel * xc + (euclid ? 0x1p-21f * cmax * cmax : 0.f)) +
-                       0x1p-18f * (xc + (euclid ? 0.5f * cmax * cmax : 0.f)) +
-                       (euclid ? 0x1p-22f * (x2[h] + cmax * cmax) + 1e-8f : 1e-30f));
-          }
-        } else {
+        if (WN == 128 && ct == 0) {
+          init_band(sc, xlo);
+        } else if (ct > 0) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {  // the row's running maximum over the quad raises every slice's skip threshold
             float m = sc[h].t1;
@@ -467,15 +532,17 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             sc[h].raise(m);
           }
         }
-        // Per row, the thread holds two groups of 16 scores: group g = 8-column blocks 8g..8g+7, columns 2q, 2q + 1 of each
+        // Per row, the thread holds WN / 64 groups of 16 scores: group g = 8-column blocks 8g..8g+7, columns 2q, 2q + 1 of each.
+        // Group-major: the two rows' groups of a column block are scanned together and their accumulators die together.
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
+        for (int g = 0; g < WN / 64; ++g) {
 #pragma unroll
-          for (int g = 0; g < 2; ++g) {
+          for (int h = 0; h < 2; ++h) {
             uint32_t r[16];
 #pragma unroll
             for (int e = 0; e < 16; ++e) r[e] = __float_as_uint(acc[4 * (8 * g + (e >> 1)) + 2 * h + (e & 1)]);
-            sc[h].scan16<true, false>(sq[h], r, ct * WN + 64 * g + 2 * q, p.mul1);
+            if constexpr (WN == 128) sc[h].template scan16<true, false>(sq[h], r, ct * WN + 64 * g + 2 * q, p.mul1);
+            else sc[h].template scan16<true>(sq[h], r, ct * WN + 64 * g + 2 * q);
           }
         }
       }
@@ -506,10 +573,10 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             // codebook) cancels in this difference, so unless d2 leads W by 2^14 the store warps evaluate sum((q - x)^2)
             // from the rows themselves; randn-like rows (d2 ~ 6e4 W at config 2) never take that path.  Flagged rows get the exact
             // evaluation in vqb_fix_flagged.
-            float d2 = x2[h] - 2.f * best;
+            float d2 = ctrl->x2[rit] - 2.f * best;
             if (p.metric == VQB_METRIC_COSINE) d2 += __ldg(p.cnorm2 + i0);
             exact_loss = !(d2 >= 0x1p14f * st.W);
-            if (!exact_loss) epi_loss += d2;
+            if (!exact_loss) locals.loss() += d2;
           }
           // hand the certified winners to the store warps: k, or -2 - k when the row's loss is left to them
           if (p.fo.enabled) ctrl->gidx[t & 1][rit] = (live && n < 2) ? (exact_loss ? -2 - i0 : i0) : -1;
@@ -542,7 +609,7 @@ vq_assign_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if (p.fo.enabled && lane == 0) mbar_arrive(smem_u32(&ctrl->g_full[t & 1]));
     }
     if (TAIL >= 1 && p.fo.loss_sum) {
-      const double w = warp_sum(static_cast<double>(epi_loss));
+      const double w = warp_sum(static_cast<double>(locals.loss()));
       if (lane == 0) atomicAdd(p.fo.loss_sum, w);
     }
     if (p.prof && threadIdx.x == 128) {
@@ -626,6 +693,23 @@ static int assign_plan(int n_a, int D, int n_passes, AssignPlan* pl) {
   return VQB_OK;
 }
 
+// The 256-code step on the same ring: an item takes two adjacent stages, so the stage count must be even, and the ring
+// has n_stages / 2 items, each step's seeds take 8 KiB, and a slot is reused after ceil(ring items / items per step)
+// steps.  It needs A resident (a streamed A k-block would sit between the two halves of B) and the larger seed slots
+// and its 3 KiB of static shared memory (StepLocals) inside 227 KiB; and a codebook of more than 128 padded codes (Kpad <= 128 is one 128-code step, which the wide step
+// could only double).  Config 2 (bf16, D = 256) and fp32 at D = 128 qualify: 8 stages, one 8 KiB seed slot.
+// Fills the seed slots and dynamic shared memory of the wide step; the launch plan and its stage count are unchanged.
+static bool wide_step(const AssignPlan& pl, int Kpad, int* n_seed, int* smem_bytes) {
+  if (pl.stream_a || pl.n_stages % 2 != 0 || Kpad <= BN_STAGE) return false;
+  const int ring = pl.n_stages / 2;
+  const int seeds = (ring + pl.n_items - 1) / pl.n_items;
+  const int bytes = pl.smem_bytes - pl.n_seed * SEED_BYTES + seeds * 2 * SEED_BYTES;
+  if (bytes + WIDE_STATIC_SMEM > SMEM_LIMIT) return false;
+  *n_seed = seeds;
+  *smem_bytes = bytes;
+  return true;
+}
+
 }  // namespace vqb
 
 using namespace vqb;
@@ -697,6 +781,10 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   p.Kpad = vqb_padded_codes(K);
   p.n_a = n_a; p.n_passes = n_passes; p.KB = plan.KB;
   p.num_row_tiles = static_cast<int>((N + BM - 1) / BM);
+  int smem_bytes = plan.smem_bytes;
+  p.n_seed = plan.n_seed;
+  const bool wide = wide_step(plan, p.Kpad, &p.n_seed, &smem_bytes);
+  const int WN = wide ? 256 : 128;   // codes per code step
   p.num_code_steps = (p.Kpad + WN - 1) / WN;
   p.margin_rel = margin_rel;
   p.cmax = cmax; p.idx = idx; p.idx_prov = idx_prov; p.hist = hist; p.hist_shift = hist_shift; p.flagged = flagged; p.flag_count = flag_count; p.dbg_best = dbg_best;
@@ -715,8 +803,6 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
   p.stream_a = plan.stream_a;
   p.a_global = static_cast<const uint16_t*>(a_planes);
   p.n_stages = plan.n_stages;
-  p.n_seed = plan.n_seed;
-  const int smem_bytes = plan.smem_bytes;
 
   CUtensorMap tmA, tmB, tmS;
   rc = make_map(&tmA, a_planes, D, N, n_a, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);  // plane stride = N*D either way
@@ -728,16 +814,26 @@ int vqb::assign_launch(const void* a_planes, int n_a, int64_t N, int D, const vo
 
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(vq_assign_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(vq_assign_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(vq_assign_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
-    if (e != cudaSuccess) return static_cast<int>(e);
+    void (*const kernels[6])(CUtensorMap, CUtensorMap, CUtensorMap, AssignParams) = {
+        vq_assign_kernel<0, 128>, vq_assign_kernel<1, 128>, vq_assign_kernel<2, 128>,
+        vq_assign_kernel<0, 256>, vq_assign_kernel<1, 256>, vq_assign_kernel<2, 256>};
+    for (int i = 0; i < 6; ++i) {   // dynamic + static shared memory <= 227 KiB
+      const int dyn = i < 3 ? SMEM_LIMIT : SMEM_LIMIT - WIDE_STATIC_SMEM;
+      const cudaError_t e = cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, dyn);
+      if (e != cudaSuccess) return static_cast<int>(e);
+    }
     attr_set = true;
   }
   const int grid = p.num_row_tiles < num_sms() ? p.num_row_tiles : num_sms();
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (p.copy_mode) vq_assign_kernel<1><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
-  else if (p.resid_mode) vq_assign_kernel<2><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
-  else vq_assign_kernel<0><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
+  if (wide) {
+    if (p.copy_mode) vq_assign_kernel<1, 256><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
+    else if (p.resid_mode) vq_assign_kernel<2, 256><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
+    else vq_assign_kernel<0, 256><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
+  } else {
+    if (p.copy_mode) vq_assign_kernel<1, 128><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
+    else if (p.resid_mode) vq_assign_kernel<2, 128><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
+    else vq_assign_kernel<0, 128><<<grid, NUM_THREADS, smem_bytes, s>>>(tmA, tmB, tmS, p);
+  }
   return static_cast<int>(cudaGetLastError());
 }
