@@ -359,6 +359,33 @@ int vqb_rotate(const void* src, const void* tgt, const void* grad_out, int64_t N
 int vqb_diveq(const void* x, const void* q, const void* noise, const void* grad_out, int64_t N, int D, int dtype,
               float noise_scale, void* out, float* grad_q, void* stream);
 
+/* Finite scalar quantization (finite_scalar_quantization.py "fsq", residual_fsq.py "rfsq"), one thread per (row, group) item.
+ * z [N][G][D] (D = len(levels) <= 16, 16-byte aligned base) in in_dtype; work_dtype is the dtype of the reference's outer
+ * chain and of `out` (the soft clamp, the stage scaling, the residual, the running sum): f32, or bf16 for bf16 inputs only.
+ * consts f32 [7][D], computed by the caller with the reference's torch expressions:
+ *   row 0  L - 1 (sym) | half_l = (L - 1) (1 + eps) / 2 (fsq:152)      row 1  2 / (L - 1) (sym) | offset (fsq:153)
+ *   row 2  shift (fsq:154; unused when sym)                            row 3  L // 2 (fsq:156)     row 4  basis (fsq:92)
+ *   row 5  1 / (2 / (L - 1))                                           row 6  1 / (L // 2)
+ * (the reciprocals, rounded to nearest, turn every division by a constant into a correctly rounded product-and-fma).
+ * sym: symmetry_preserving_bound (fsq:161-169), else bound (fsq:147-157); hard: the clamp replaces tanh (and atanh).
+ * scales f32 [2][Q][D]: the W values of rfsq's `scales`, then their reciprocals (NULL for a plain FSQ: no scaling, Q = 1);
+ * clampv f32 [2][D]: the soft-clamp value (rfsq:193-195) and its reciprocal (NULL: none).  Stages >= n_active (quantize
+ * dropout) write index -1 and add nothing.  N * G < 2^31. */
+int vqb_fsq_forward(const void* z, int in_dtype, int work_dtype, int64_t N, int G, int D, int Q, int n_active, int sym, int hard,
+                    const float* consts, const float* scales, const float* clampv, void* out, void* idx, int idx64,
+                    int64_t idx_s_row, int64_t idx_s_g, int64_t idx_s_q, void* stream);
+/* d z of vqb_fsq_forward's `out` given grad_out [N][G][D] (work_dtype), the straight-through chain in autograd's order,
+ * every stage recomputed from z (nothing kept from the forward).  grad_z [N][G][D] in in_dtype.  n_active * D <= 768. */
+int vqb_fsq_backward(const void* z, int in_dtype, int work_dtype, int64_t N, int G, int D, int Q, int n_active, int sym, int hard,
+                     const float* consts, const float* scales, const float* clampv, const void* grad_out, void* grad_z,
+                     void* stream);
+/* indices (element (row, g, q) at idx + row * idx_s_row + g * idx_s_g + q * idx_s_q, int32 or int64; -1 = dropped stage) ->
+ * out [N][G][D] = sum_q code_q * scale_q (work_dtype) and/or codes [Q][N][G][D] (the scaled stage codes), each code from the
+ * index digits (index // basis) % L.  levels_basis i32 [2][D]: levels, basis.  scales NULL: unscaled (fsq indices_to_codes). */
+int vqb_fsq_decode(const void* idx, int idx64, int64_t idx_s_row, int64_t idx_s_g, int64_t idx_s_q, int64_t N, int G, int D,
+                   int Q, int work_dtype, int sym, const float* consts, const int32_t* levels_basis, const float* scales, void* out,
+                   void* codes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

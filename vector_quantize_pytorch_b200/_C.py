@@ -106,6 +106,10 @@ SIGNATURES = {
     "vqb_rvq_forward": (_i32, [_vp, _i32, _vp]),
     "vqb_rsimvq_tail": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _i32, _vp, _i64, _vp, _vp, _f32, _f32, _vp]),
     "vqb_rsimvq_backward": (_i32, [_vp, _vp, _i32, _i32, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "vqb_fsq_forward": (_i32, [_vp, _i32, _i32, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64,
+                               _i64, _vp]),
+    "vqb_fsq_backward": (_i32, [_vp, _i32, _i32, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "vqb_fsq_decode": (_i32, [_vp, _i32, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 

@@ -1,8 +1,8 @@
 """H100-native (sm_90a) nearest-code search / gather / EMA kernels behind the vector-quantize-pytorch API.
 
 Drop-in for ONE path of lucidrains/vector-quantize-pytorch: `VectorQuantize`, `ResidualVQ`,
-`GroupedResidualVQ` forward (`(quantized, indices, commit_loss)`), the `Codebook` surface, `SimVQ`'s search and
-`ResidualSimVQ`.
+`GroupedResidualVQ` forward (`(quantized, indices, commit_loss)`), the `Codebook` surface, `SimVQ`'s search,
+`ResidualSimVQ`, and finite scalar quantization (`FSQ`, `ResidualFSQ`, `GroupedResidualFSQ`).
 The hot path is hand-written CUDA (wgmma / TMA / mbarrier) in `csrc/`, bound through the C ABI in
 `include/vqb200.h`.  No Triton, no CPU fallback.
 """
@@ -11,6 +11,8 @@ from .vector_quantize import VectorQuantize  # noqa: E402
 from .residual_vq import ResidualVQ, GroupedResidualVQ  # noqa: E402
 from .sim_vq import SimVQ  # noqa: E402
 from .residual_sim_vq import ResidualSimVQ  # noqa: E402
+from .fsq import FSQ  # noqa: E402
+from .residual_fsq import ResidualFSQ, GroupedResidualFSQ  # noqa: E402
 
 __all__ = ["Codebook", "EuclideanCodebook", "CosineSimCodebook", "VectorQuantize", "ResidualVQ", "GroupedResidualVQ", "SimVQ",
-           "ResidualSimVQ"]
+           "ResidualSimVQ", "FSQ", "ResidualFSQ", "GroupedResidualFSQ"]

@@ -527,3 +527,58 @@ def diveq(x: torch.Tensor, q: torch.Tensor, noise: torch.Tensor, noise_scale: fl
     if g2 is None:
         return out.reshape(shape)
     return out.reshape(shape), dq.reshape(shape)
+
+
+def _fsq_strides(idx: torch.Tensor) -> tuple:
+    """(row, group, stage) element strides of an (N, G, Q) view of an index tensor (a size-1 axis has stride 0)."""
+    return tuple(0 if n == 1 else s for n, s in zip(idx.shape, idx.stride()))
+
+
+def fsq_forward(z: torch.Tensor, work_dtype: torch.dtype, Q: int, n_active: int, sym: bool, hard: bool, consts: torch.Tensor,
+                scales: torch.Tensor | None, clampv: torch.Tensor | None, indices: torch.Tensor) -> torch.Tensor:
+    """vqb_fsq_forward: z (N, G, D) contiguous in fp32 / bf16 -> out (N, G, D) in `work_dtype`; writes the indices into
+    `indices`, an (N, G, Q) view (int32 / int64, any strides) of the caller's index tensor.  consts (7, D), scales (2, Q, D), clampv (2, D): fp32 tables
+    of the module (include/vqb200.h)."""
+    _require_cuda(z, consts, scales, clampv, indices)
+    N, G, D = z.shape
+    out = torch.empty(z.shape, dtype=work_dtype, device=z.device)
+    s_row, s_g, s_q = _fsq_strides(indices)
+    with torch.cuda.device(z.device):
+        check(lib.vqb_fsq_forward(_p(z), _dtype_code(z), _DT[work_dtype], N, G, D, Q, n_active, int(sym), int(hard), _p(consts),
+                                  _p(scales), _p(clampv), _p(out), _p(indices), int(indices.dtype == torch.int64), s_row, s_g, s_q,
+                                  _stream()), "vqb_fsq_forward")
+    _count(1)
+    return out
+
+
+def fsq_backward(z: torch.Tensor, grad_out: torch.Tensor, Q: int, n_active: int, sym: bool, hard: bool, consts: torch.Tensor,
+                 scales: torch.Tensor | None, clampv: torch.Tensor | None) -> torch.Tensor:
+    """vqb_fsq_backward: d z (z's dtype) of fsq_forward's output given its gradient (N, G, D) in the work dtype."""
+    _require_cuda(z, grad_out, consts, scales, clampv)
+    N, G, D = z.shape
+    gz = torch.empty_like(z)
+    g = grad_out.contiguous()
+    with torch.cuda.device(z.device):
+        check(lib.vqb_fsq_backward(_p(z), _dtype_code(z), _dtype_code(g), N, G, D, Q, n_active, int(sym), int(hard), _p(consts),
+                                   _p(scales), _p(clampv), _p(g), _p(gz), _stream()), "vqb_fsq_backward")
+    _count(1)
+    return gz
+
+
+def fsq_decode(indices: torch.Tensor, D: int, work_dtype: torch.dtype, sym: bool, consts: torch.Tensor, levels_basis: torch.Tensor,
+               scales: torch.Tensor | None, want_sum: bool, want_codes: bool):
+    """vqb_fsq_decode: indices, an (N, G, Q) view (any strides) -> (sum over the stages (N, G, D) or None, stage codes
+    (Q, N, G, D) or None) in `work_dtype`."""
+    _require_cuda(indices, consts, levels_basis, scales)
+    if indices.dtype not in (torch.int32, torch.int64):
+        raise TypeError(f"FSQ indices must be int32 or int64, got {indices.dtype}")
+    N, G, Q = indices.shape
+    dev = indices.device
+    out = torch.empty((N, G, D), dtype=work_dtype, device=dev) if want_sum else None
+    codes = torch.empty((Q, N, G, D), dtype=work_dtype, device=dev) if want_codes else None
+    s_row, s_g, s_q = _fsq_strides(indices)
+    with torch.cuda.device(dev):
+        check(lib.vqb_fsq_decode(_p(indices), int(indices.dtype == torch.int64), s_row, s_g, s_q, N, G, D, Q, _DT[work_dtype], int(sym),
+                                 _p(consts), _p(levels_basis), _p(scales), _p(out), _p(codes), _stream()), "vqb_fsq_decode")
+    _count(1)
+    return out, codes
