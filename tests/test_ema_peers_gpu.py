@@ -138,7 +138,7 @@ def test_rvq_ema_peers_matches_ema(D, K, cosine):
     assert_same(got, ref, f"D={D} K={K} n_lerp={n_lerp}")
 
 
-def test_vq_forward_update3_single_rank():
+def test_vq_forward_peer_update_on_one_rank():
     from vector_quantize_pytorch_b200 import ops
     D, K, N, decay, eps = 256, 512, 65536, 0.8, 1e-5
     gen = torch.Generator().manual_seed(N + K + 1)
@@ -153,7 +153,7 @@ def test_vq_forward_update3_single_rank():
     ptrs = (ctypes.c_void_p * 1)(buf.data_ptr())
     idx32, _ = ops.vq_forward(x, cb, state, update=3, do_normalise=True, decay=decay, eps=eps,
                               stats=buf[SLICE_OFFSET:SLICE_OFFSET + ops.stats_floats(K, D)], peer=peer, peer_ptrs=ptrs,
-                              peer_slice_offset=SLICE_OFFSET, ws_key=("ema_peers", 1))
+                              peer_slice_offset=SLICE_OFFSET)
     torch.cuda.synchronize()
     assert peer.epoch.item() == 2   # one barrier per EMA launch group
     idx = idx32.long()

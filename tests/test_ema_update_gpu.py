@@ -145,7 +145,7 @@ def stats_case(dt, D, K, N, cosine, skew, gen):
 
 
 @pytest.mark.parametrize("name,dt,D,K,N,cosine,skew,path", STATS_CASES, ids=[c[0] for c in STATS_CASES])
-def test_counting_sort_statistics(name, dt, D, K, N, cosine, skew, path):
+def test_counting_sort_statistics_within_bound(name, dt, D, K, N, cosine, skew, path):
     from vector_quantize_pytorch_b200 import ops
     s = sms()
     if N == "cap":
@@ -189,7 +189,7 @@ def test_counting_sort_statistics(name, dt, D, K, N, cosine, skew, path):
     zero = torch.zeros_like(cnt)
     state = (torch.ones(K, device=DEV), c.clone(), c)
     worst = {}
-    idx32, st = ops.vq_forward(x, cb, state, update=1, do_normalise=False, decay=0.8, eps=1e-5, ws_key=("ema_stats", name))
+    idx32, st = ops.vq_forward(x, cb, state, update=1, do_normalise=False, decay=0.8, eps=1e-5)
     torch.cuda.synchronize()
     assert torch.equal(idx32.long(), idx), "vq_forward: indices differ from the search"
     # segment chains + one atomicAdd per work item and per re-scored row

@@ -55,6 +55,9 @@ PROGRAM_CASES = {
     "freeze_codebook": dict(grouped=False, dt=torch.float32, width=64, kw={}, call=dict(freeze_codebook=True)),
     "grvq_shared_bf16": dict(grouped=True, dt=torch.bfloat16, width=128, kw=dict(shared_codebook=True)),
     "grvq_shared_bf16_eval": dict(grouped=True, dt=torch.bfloat16, width=128, kw=dict(shared_codebook=True), eval=True),
+    # (training, rows per batch element) of each step: an eval plan is cached before training needs more scratch, and replayed
+    "eval_train_rows_eval": dict(grouped=False, dt=torch.float32, width=64, kw={},
+                                 schedule=[(False, 700), (True, 700), (True, 1400), (False, 700)]),
 }
 
 
@@ -72,15 +75,14 @@ def test_program_equals_stagewise(case, monkeypatch):
     c = PROGRAM_CASES[case]
     mod = _build(c["grouped"], c["width"], **c["kw"])
     ref = copy.deepcopy(mod)
-    if c.get("eval"):
-        mod.eval(), ref.eval()
     noise = {}
     monkeypatch.setattr(vqm, "diveq_noise", lambda like: noise["z"].to(like.dtype))
     with torch.no_grad():
-        for step in range(4):
+        for step, (training, rows) in enumerate(c.get("schedule", [(not c.get("eval"), 700)] * 4)):
+            mod.train(training), ref.train(training)
             gen = torch.Generator(device=DEV).manual_seed(100 + step)
-            x = torch.randn(3, 700, c["width"], device=DEV, generator=gen).to(c["dt"])
-            noise["z"] = torch.randn(3, 700, 64, device=DEV, generator=gen)
+            x = torch.randn(3, rows, c["width"], device=DEV, generator=gen).to(c["dt"])
+            noise["z"] = torch.randn(3, rows, 64, device=DEV, generator=gen)
             monkeypatch.setenv("VQB_RVQ_PROGRAM", "1")
             o1 = mod(x, **c.get("call", {}))
             monkeypatch.setenv("VQB_RVQ_PROGRAM", "0")

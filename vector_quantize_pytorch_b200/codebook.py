@@ -147,6 +147,7 @@ class Codebook(nn.Module):
         self._head_views = None
         self._operands: ops.CodebookOperands | None = None
         self._operands_key = None
+        self._scratch = ops.Scratch()   # the search scratch of `quantize_rows` (a plain attribute: not in the state_dict)
         self._peer = None          # dist.PeerReducer of this codebook's packed statistics (use_ddp, created on first use)
         self._peer_tried = False
 
@@ -158,7 +159,8 @@ class Codebook(nn.Module):
 
     def head(self, i: int) -> "Codebook":
         """The view of this module that works on codebook `i` of the (num_codebooks, K, D) buffers.  A shallow copy: it shares
-        the buffer dict with its parent (so `.to()`, `load_state_dict` reach it) and keeps its own slot and operand cache."""
+        the buffer dict with its parent (so `.to()`, `load_state_dict` reach it) and keeps its own slot, operand cache and
+        search scratch."""
         if self.num_codebooks == 1:
             return self
         if self._head_views is None:
@@ -167,6 +169,7 @@ class Codebook(nn.Module):
             for j in range(self.num_codebooks):
                 v = copy.copy(self)
                 v._slot, v._head_views, v._operands, v._operands_key, v._peer, v._peer_tried = j, None, None, None, None, False
+                v._scratch = ops.Scratch()
                 views.append(v)
             self._head_views = views
         v = self._head_views[i]
@@ -438,7 +441,7 @@ class Codebook(nn.Module):
         idx32, stats = ops.vq_forward(
             x, cb, self._state2d(), update=mode, do_normalise=normalise, decay=self.decay, eps=self.eps, q_out=q_out,
             idx64_out=idx64_out, idx_stride=idx_stride, loss_out=loss_out, loss_weight=loss_weight, resid_out=resid_out,
-            stats=stats_out, margin=margin, ws_key=id(self),
+            stats=stats_out, margin=margin, scratch=self._scratch,
             peer=peer, peer_ptrs=peer_ptrs, row_mask=row_mask, n_live=n_live)
         if mode >= 2 and normalise:
             self._mark_operands_fresh()

@@ -172,31 +172,44 @@ def search(x: torch.Tensor, ops: CodebookOperands, embed: torch.Tensor, *, margi
     return SearchResult(idx, x_eff, count[:1], flagged, best, count[1:])
 
 
-_WS_CACHE: dict = {}
+class Scratch:
+    """The two device scratch buffers of `vq_forward_args` (the int32 index row and the workspace) for ONE owner: a `Codebook`
+    for its eager calls, an `RvqProgram` lane for the stage ops it freezes.  Reused from call to call (calls of one owner are
+    ordered on its stream), so the pointers stay stable and the CUDA-graph cache of vqb_vq_forward keeps replaying; grown when a
+    call needs more bytes or another device, so a batch whose row count changes does not pin a buffer per count.  A grown
+    buffer is dropped, so whoever froze a pointer into the old one must hold it itself.  Never copied or pickled with its
+    owner: a copy starts empty."""
 
+    def __init__(self):
+        self.idx = None
+        self.ws = None
 
-def _workspace(key, nbytes: int, device) -> torch.Tensor:
-    """Scratch buffers are reused across calls (same stream => ordered).  Keyed by owner / device only and grown on
-    demand: a masked batch that compacts to a different N every call must not pin a new buffer per N."""
-    buf = _WS_CACHE.get(key)
-    if buf is None or buf.numel() < nbytes or buf.device != device:
-        buf = torch.empty((max(nbytes, 256),), dtype=torch.uint8, device=device)
-        _WS_CACHE[key] = buf
-    return buf
+    def __deepcopy__(self, memo):
+        return Scratch()
 
+    def __reduce__(self):
+        return (Scratch, ())
 
-def take_workspaces(ws_key, device) -> list:
-    """Remove the scratch buffers `vq_forward_args` made for `ws_key` on `device` from the shared cache and return them: the
-    caller (a cached program that points into them) owns them from now on, and they are freed together with it."""
-    return [b for b in (_WS_CACHE.pop((kind, ws_key, device.index), None) for kind in ("idx32", "fwd")) if b is not None]
+    @staticmethod
+    def _fit(buf, nbytes, device):
+        if buf is None or buf.numel() < nbytes or buf.device != device:
+            buf = torch.empty((max(nbytes, 256),), dtype=torch.uint8, device=device)
+        return buf
+
+    def take(self, idx_bytes: int, ws_bytes: int, device) -> tuple[torch.Tensor, torch.Tensor]:
+        """(index buffer, workspace) of at least these sizes (uint8) on `device`."""
+        self.idx = self._fit(self.idx, idx_bytes, device)
+        self.ws = self._fit(self.ws, ws_bytes, device)
+        return self.idx, self.ws
 
 
 def vq_forward_args(x: torch.Tensor, ops: CodebookOperands, state: tuple, *, update: int, do_normalise: bool, decay: float,
                     eps: float, q_out=None, idx64_out=None, idx_stride: int = 1, loss_out=None, loss_weight: float = 1.0,
                     resid_out=None, stats=None, margin: float | None = None, already_normalised: bool = False,
-                    ws_key=None, peer=None, peer_ptrs=None, peer_slice_offset: int = 0,
+                    scratch: Scratch | None = None, peer=None, peer_ptrs=None, peer_slice_offset: int = 0,
                     a_planes_in=None, planes_out=None, row_mask=None, n_live=None):
     """The argument block of one vqb_vq_forward call (also one VQB_RVQ_STAGE op of vqb_rvq_forward).
+    scratch: the caller's `Scratch` (None: a fresh one, freed after the call — for one-off calls).
     row_mask (N,) uint8 / n_live (1,) int64 on the device: a masked batch (vqp:1116-1119) — padding rows (0) keep the values
     q_out / idx64_out were pre-filled with and stay out of the loss and the statistics (include/vqb200.h).
     Returns (args, idx32, stats, n_launches)."""
@@ -210,12 +223,11 @@ def vq_forward_args(x: torch.Tensor, ops: CodebookOperands, state: tuple, *, upd
     dt = _dtype_code(x)
     dev = x.device
     cs, ea, emb = state
-    # internal scratch lives in reusable buffers: stable pointers keep the CUDA-graph cache of vqb_vq_forward hot
-    idx32 = _workspace(("idx32", ws_key, dev.index), 4 * N, dev)[:4 * N].view(torch.int32)
+    nbytes = lib.vqb_vq_forward_workspace(N, D, K, dt, int(ops.cosine), int(update))
+    idx_buf, ws = (scratch or Scratch()).take(4 * N, nbytes, dev)
+    idx32 = idx_buf[:4 * N].view(torch.int32)
     if update and stats is None:
         stats = torch.empty((stats_floats(K, D),), dtype=torch.float32, device=dev)
-    nbytes = lib.vqb_vq_forward_workspace(N, D, K, dt, int(ops.cosine), int(update))
-    ws = _workspace(("fwd", ws_key, dev.index), nbytes, dev)
     a = _C.VQForwardArgs(
         x=_p(x), dtype=dt, metric=int(ops.cosine), N=N, D=D, K=K, already_normalised=int(already_normalised),
         cluster_size=_p(cs), embed_avg=_p(ea), embed=_p(emb), planes=_p(ops.planes), bext=_p(ops.bext), bias=_p(ops.bias),
@@ -263,14 +275,20 @@ class RvqProgram:
         self.device = device
         self.ops = []
         self.keep = []       # tensors the ops point into
+        # the stage ops' scratch: one per lane (the ops of a lane run in order, every stage joins its side stream before the
+        # next op; lanes run in parallel), and every buffer an op was handed, even one a later stage of its lane outgrew
+        self.scratch = {}
+        self.scratch_bufs = []
         self.launches = 0
 
     def stage(self, lane, x, cb_ops, state, **kw):
-        a, idx32, stats, n = vq_forward_args(x, cb_ops, state, **kw)
+        scratch = self.scratch.setdefault(lane, Scratch())
+        a, idx32, stats, n = vq_forward_args(x, cb_ops, state, scratch=scratch, **kw)
         op = _C.RvqOp(kind=_C.RVQ_STAGE, lane=lane)
         op.stage = a
         self.ops.append(op)
         self.keep.append((x, cb_ops, state, kw, idx32, stats))
+        self.scratch_bufs += [scratch.idx, scratch.ws]
         self.launches += n
         return idx32, stats
 
@@ -343,7 +361,9 @@ class RvqProgram:
         self.arr = (_C.RvqOp * n)(*self.ops)
         self.n = n
         self.ops = None
-        self.keep = None     # the owner of a cached program keeps its persistent tensors alive itself (and re-binds the rest)
+        # whoever freezes a pointer owns the memory behind it: the program keeps the scratch its stage ops point into (freed
+        # with the program), the owner of a cached program keeps its other persistent tensors alive itself (and re-binds the rest)
+        self.keep = None
         return self
 
     def run(self):

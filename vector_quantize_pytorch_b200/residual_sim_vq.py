@@ -20,8 +20,9 @@ from .sim_vq import SimVQ
 
 class _Plan:
     """The cached program of one forward configuration on one device.  It owns every buffer its ops keep pointing into — codebook
-    operands, the residual ping-pong, loss scratch and the search's scratch (index and workspace) — so they are freed together
-    with the plan; the per-call pointers (input, codebooks, outputs, statistics) are patched by `run` before every launch."""
+    operands, the residual ping-pong, loss scratch and, through its program, the search's scratch (index and workspace) — so
+    they are freed together with the plan; the per-call pointers (input, codebooks, outputs, statistics) are patched by `run`
+    before every launch."""
 
     def __init__(self, mod, N, D, K, n_active, want_stats, device):
         Q = mod.num_quantizers
@@ -38,20 +39,18 @@ class _Plan:
         losses0 = torch.empty((Q,), dtype=torch.float32, device=device)
         stats0 = torch.empty((max(1, n_active * self.stat_floats),), dtype=torch.float32, device=device)
         prog = ops.RvqProgram(device)
-        ws_key = ("rsimvq", id(self))
         r = x0
         for q in range(n_active):
             layer = mod.layers[q]
             nxt = self.bufs[q & 1] if q + 1 < n_active else None
             F_ = self.stat_floats
             idx32, _ = prog.stage(0, r, self.operands[q], (None, None, codes0[q]), update=1 if want_stats else 0,
-                                  do_normalise=False, decay=0.0, eps=0.0, ws_key=ws_key,
+                                  do_normalise=False, decay=0.0, eps=0.0,
                                   stats=stats0[q * F_:(q + 1) * F_] if want_stats else None)
             prog.simvq_tail(0, r, codes0[q], idx32, rotation=layer.rotation_trick, r_next=nxt, qsum=out0, first=q == 0,
                             idx64_out=idx0[:, q], idx_stride=Q, loss_sum=self.loss_sum[q:q + 1], loss_out=losses0[q:q + 1],
                             input_weight=layer.input_to_quantize_commit_loss_weight, weight=layer.commitment_weight)
             r = nxt
-        self.workspaces = ops.take_workspaces(ws_key, torch.device(device))
         self.prog = prog.freeze()
 
     def run(self, flat, codes, indices, out, losses, stats):

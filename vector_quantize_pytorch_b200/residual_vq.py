@@ -208,15 +208,17 @@ class _PlanPart:
         # so that only stage 0 runs the split kernel over its input (536 MB of HBM traffic per stage at config 3)
         split = dtype == torch.float32 and not books[0].use_cosine_sim and Q > 1
         self.planes = [torch.empty((2, N, D), dtype=torch.bfloat16, device=dev) for _ in range(min(2, Q - 1))] if split else None
+        # the operands the ops point into, held so that the id() of each in `ResidualVQ._part_key` names them for this plan's life
+        self.operands = [book.operands() for book in books]
         self.first = len(prog.ops)
         residual = flat
         for q, book in enumerate(books):
             nxt = self.bufs[q & 1] if q + 1 < Q else None
             want_loss = rvq.training and rvq.layers[q].has_commitment_loss
-            prog.stage(lane, residual, book.operands(), book._state2d(), update=1 if do_update[q] else 0, do_normalise=False,
+            prog.stage(lane, residual, self.operands[q], book._state2d(), update=1 if do_update[q] else 0, do_normalise=False,
                        decay=book.decay, eps=book.eps, idx64_out=all_idx[:, q], idx_stride=Q,
                        loss_out=self.losses[q:q + 1] if want_loss else None, loss_weight=rvq.layers[q].commitment_weight,
-                       resid_out=nxt, stats=self.updates.stats(q), ws_key=id(book),
+                       resid_out=nxt, stats=self.updates.stats(q),
                        a_planes_in=self.planes[(q - 1) & 1] if (split and q > 0) else None,
                        planes_out=self.planes[q & 1] if (split and nxt is not None) else None)
             residual = nxt
