@@ -1,5 +1,6 @@
 """Shared loading of the FSQ fixtures (tests/golden/fsq/*.npz, oracle/gen_golden_fsq.py) for the CPU oracle replay and the GPU
-replay.  The quantizer proper sees rows (N, G, d): G = the FSQ's codebooks or the GroupedResidualFSQ's groups."""
+replay, and the rounding-boundary finder of the kernel tests.  The quantizer proper sees rows (N, G, d): G = the FSQ's codebooks
+or the GroupedResidualFSQ's groups."""
 from __future__ import annotations
 
 import glob
@@ -7,6 +8,8 @@ import json
 import os
 
 import numpy as np
+
+from oracle import fsq_oracle as O
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 FIXTURES = sorted(glob.glob(os.path.join(HERE, "golden", "fsq", "*.npz")))
@@ -75,6 +78,54 @@ def part_rows(t, d):
     if P == 1:
         return np.ascontiguousarray(t[0].reshape(t.shape[1], -1, d))
     return np.ascontiguousarray(t.transpose(1, 0, 2))
+
+
+def _key(f):
+    """float32 -> int64 keys ordered like the values (adjacent floats differ by 1; -0 and +0 share 0)."""
+    b = np.asarray(f, np.float32).view(np.int32).astype(np.int64)
+    return np.where(b < 0, -(b & 0x7FFFFFFF), b)
+
+
+def _unkey(k):
+    k = np.asarray(k, np.int64)
+    return np.where(k < 0, (-k) | 0x80000000, k).astype(np.uint32).view(np.float32)
+
+
+def stage_values(z, j, levels, Q, q, sym, hard, scales=None, clampv=None, w_bf16=False):
+    """The oracle's stage-q (code, pre-floor / pre-round value, stage input u) of element j for 1-D float32 inputs z of that
+    element (each element's chain is independent of the others, which are left 0)."""
+    zz = np.zeros((len(z), 1, len(levels)), np.float32)
+    zz[:, 0, j] = z
+    f = O.forward(zz, levels, Q, q + 1, sym, hard, scales, clampv, w_bf16)
+    u = f["u"][q][:, 0, :]
+    code, _, _, br = O.stage(u, O.tables(levels, sym, hard), sym, hard)
+    return code[:, j], br[:, j], u[:, j]
+
+
+def boundary_pairs(levels, Q, q, j, sym, hard, scales=None, clampv=None, w_bf16=False, lo=-2.5, hi=2.5, n=2001):
+    """Adjacent float32 inputs (a, b = the next float after a) of element j across which the oracle's stage-q code changes:
+    every sign change of the code on an n-point grid of [lo, hi], bisected on the float32 bit pattern down to one ulp.  The
+    bisection keeps code(a) != code(b), so it needs no monotone chain."""
+    def code(z):
+        return stage_values(z, j, levels, Q, q, sym, hard, scales, clampv, w_bf16)[0]
+
+    grid = np.linspace(lo, hi, n, dtype=np.float32)
+    c = code(grid)
+    k = np.nonzero(c[:-1] != c[1:])[0]
+    a, b, ca = _key(grid[k]), _key(grid[k + 1]), c[k]
+    while (b - a > 1).any():
+        wide = b - a > 1
+        m = a + (b - a) // 2
+        same = code(_unkey(m)) == ca
+        a = np.where(wide & same, m, a)
+        b = np.where(wide & ~same, m, b)
+    return _unkey(a), _unkey(b)
+
+
+def exact_ties(br, sym):
+    """Pre-floor values that are exactly an integer (sym) or pre-round values exactly k + 1/2 (non-sym)."""
+    br = np.asarray(br, np.float64)
+    return br == np.floor(br) if sym else br - np.floor(br) == 0.5
 
 
 def flipped_rows(idx, ref_idx, near):

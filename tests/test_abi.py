@@ -55,6 +55,39 @@ def test_argument_errors_are_return_codes_not_crashes():
     assert lib.vqb_ema_apply_weighted(p, p, p, p, 10, 1032, 0.8, 1e-5, 0, 1, 1, None, p, p, p, p, p, p, None) == -2
 
 
+def test_fsq_argument_errors_are_return_codes_not_crashes():
+    """vqb_fsq_forward / _backward / _decode refuse, before any CUDA call, more than 64 stages, d > 16, null pointers, unknown
+    dtypes, an fp32 input with a bf16 chain (torch would promote it) and an unaligned z or decode output."""
+    from vector_quantize_pytorch_b200 import _C
+    lib = _C.lib
+    p = 0x10000   # non-null, 16-byte aligned; never dereferenced
+    f, b = _C.DTYPE_F32, _C.DTYPE_BF16
+
+    def fwd(z=p, in_dt=f, w_dt=f, D=4, Q=2, n_active=2, consts=p, out=p, idx=p):
+        return lib.vqb_fsq_forward(z, in_dt, w_dt, 8, 1, D, Q, n_active, 1, 1, consts, None, None, out, idx, 1, Q, 0, 1, None)
+
+    def bwd(z=p, in_dt=f, w_dt=f, D=4, Q=2, n_active=2, consts=p, gout=p, gz=p):
+        return lib.vqb_fsq_backward(z, in_dt, w_dt, 8, 1, D, Q, n_active, 1, 1, consts, None, None, gout, gz, None)
+
+    def dec(idx=p, D=4, Q=2, w_dt=f, consts=p, ints=p, out=p, codes=None):
+        return lib.vqb_fsq_decode(idx, 1, Q, 0, 1, 8, 1, D, Q, w_dt, 1, consts, ints, None, out, codes, None)
+
+    for call in (fwd, bwd):
+        assert call(Q=65, n_active=65) == -2
+        assert call(D=17) == -2
+        assert call(z=None) == -1 and call(consts=None) == -1
+        assert call(n_active=0) == -1 and call(n_active=3) == -1
+        assert call(in_dt=7) == -1 and call(w_dt=7) == -1
+        assert call(w_dt=b) == -2
+        assert call(z=p + 4) == -3
+    assert fwd(out=None) == -1 and fwd(idx=None) == -1
+    assert bwd(gout=None) == -1 and bwd(gz=None) == -1
+    assert dec(Q=65) == -2 and dec(D=17) == -2
+    assert dec(idx=None) == -1 and dec(consts=None) == -1 and dec(ints=None) == -1 and dec(out=None) == -1
+    assert dec(w_dt=7) == -1
+    assert dec(out=p + 4) == -3 and dec(out=None, codes=p + 4) == -3
+
+
 def test_struct_layout_is_pinned():
     """The ctypes mirrors have the layout of include/vqb200.h (the library static_asserts the same sizes); fields that no
     longer select anything keep their place."""

@@ -6,7 +6,7 @@ import pytest
 import torch
 
 from oracle import fsq_oracle as O
-from fsq_golden import FIXTURES, Case, fixture_id, flipped_rows
+from fsq_golden import FIXTURES, Case, _key, boundary_pairs, fixture_id, flipped_rows, stage_values
 
 import vector_quantize_pytorch_b200 as vqb
 from vector_quantize_pytorch_b200.fsq import fsq_tables
@@ -113,6 +113,45 @@ def test_seeded_construction_matches_reference(path):
     torch.manual_seed(c.meta["init_seed"])
     CLASSES[c.cls](**c.meta["kw"])
     np.testing.assert_array_equal(torch.randn(3).numpy(), after.numpy())
+
+
+@pytest.mark.parametrize("sym", [True, False], ids=["sym", "nonsym"])
+@pytest.mark.parametrize("hard", [True, False], ids=["hard", "tanh"])
+@pytest.mark.parametrize("soft", [False, True], ids=["nosoft", "soft"])
+def test_boundary_finder(sym, hard, soft):
+    """fsq_golden.boundary_pairs (the planted boundaries of tests/test_fsq_kernels_gpu.py): across every pair it returns the
+    oracle's stage code changes, and the pre-floor / pre-round value recomputed in float64 from each side's stage input lies
+    within one float32 step of a rounding boundary (plus, on the tanh paths, tanhf's two-ulp error times the slope)."""
+    levels = [2, 3, 4, 5] if sym else [3, 4, 5, 8]
+    Q = 3
+    L = np.asarray(levels, np.float32)
+    scales = np.stack([L ** -q for q in range(Q)]).astype(np.float32)
+    clampv = (1 + 1 / (L - 1)).astype(np.float32) if soft else None
+    t = O.tables(levels, sym, hard)
+    bound = (lambda v: np.clip(v, -1, 1)) if hard else np.tanh
+    total = 0
+    for q in (0, Q - 1):
+        for j in range(len(levels)):
+            a, b = boundary_pairs(levels, Q, q, j, sym, hard, scales, clampv)
+            assert len(a) >= 1
+            np.testing.assert_array_equal(_key(b) - _key(a), 1)
+            sides = [stage_values(z, j, levels, Q, q, sym, hard, scales, clampv) for z in (a, b)]
+            assert (sides[0][0] != sides[1][0]).all(), "the code does not change across a pair"
+            b64 = []
+            tol = 0.0
+            for _, br, u in sides:
+                x = bound(u.astype(np.float64) + t["shift"][j])
+                b64.append(t["a"][j] * (x + 1) / 2 + 0.5 if sym else x * t["a"][j] - t["b"][j])
+                tol = np.maximum(tol, np.spacing(np.abs(br).astype(np.float32)).astype(np.float64))
+                if not hard:
+                    h = np.abs(np.tanh((u + t["shift"][j]).astype(np.float32)))
+                    tol = tol + 2 * np.spacing(h).astype(np.float64) * t["a"][j] * (0.5 if sym else 1.0)
+            lo, hi = np.minimum(*b64), np.maximum(*b64)
+            k = np.floor(lo) + np.arange(-1, 3)[:, None] + (0.0 if sym else 0.5)   # the boundaries around the pair
+            dist = np.maximum(0.0, np.maximum(k - hi, lo - k)).min(axis=0)
+            assert (dist <= tol).all(), float((dist / tol).max())
+            total += len(a)
+    print(f"{total} pairs")
 
 
 def test_codebook_and_helpers_match_reference_expressions():

@@ -578,6 +578,8 @@ def fsq_backward(z: torch.Tensor, grad_out: torch.Tensor, Q: int, n_active: int,
     N, G, D = z.shape
     gz = torch.empty_like(z)
     g = grad_out.contiguous()
+    if g.data_ptr() % 16:   # a contiguous view at an offset (the kernel moves rows in 16-byte vectors)
+        g = g.clone()
     with torch.cuda.device(z.device):
         check(lib.vqb_fsq_backward(_p(z), _dtype_code(z), _dtype_code(g), N, G, D, Q, n_active, int(sym), int(hard), _p(consts),
                                    _p(scales), _p(clampv), _p(g), _p(gz), _stream()), "vqb_fsq_backward")
