@@ -386,6 +386,46 @@ int vqb_fsq_decode(const void* idx, int idx64, int64_t idx_s_row, int64_t idx_s_
                    int Q, int work_dtype, int sym, const float* consts, const int32_t* levels_basis, const float* scales, void* out,
                    void* codes, void* stream);
 
+/* Lookup-free quantization (lookup_free_quantization.py "lfq", residual_lfq.py "rlfq"), one thread per (row, group) item.
+ * z [N][G][D] (D = log2(codebook_size) <= 20) in dtype (f32 or bf16; the chain runs in the input dtype, rounding after every
+ * op).  params f32 [3][Q]: per stage the codebook_scale s, the code magnitude m (s, or the reference's l2norm(+-s) * s when
+ * spherical) and the soft-clamp value (0: none).  Per stage q < n_active: soft clamp, spherical l2norm, q = x > 0 ? m : -m,
+ * index bit j = 2^(D-1-j) (int64, element (row, g, q) at idx + row * idx_s_row + g * idx_s_g + q * idx_s_q; -1 for q >=
+ * n_active), value x + (q - x) (training) or q, residual -= value, out += value (residual) or out = value (a plain LFQ).
+ * ent f32 [n_active][N][G][D] or NULL: the entropy input x of every stage.  rowmask u8 [N] or NULL: rows that count in the
+ * commitment sums.  commit f64 [n_active][commit_blocks] or NULL: per-block sums of (x - q)^2, commit_blocks =
+ * vqb_lfq_forward_blocks(N, G).  N * G < 2^31, Q <= 64. */
+int vqb_lfq_forward(const void* z, int dtype, int64_t N, int G, int D, int Q, int n_active, int residual, int training, int spherical,
+                    const float* params, void* out, void* idx, int64_t idx_s_row, int64_t idx_s_g, int64_t idx_s_q, float* ent,
+                    const uint8_t* rowmask, double* commit, int commit_blocks, void* stream);
+int vqb_lfq_forward_blocks(int64_t N, int G);
+/* Entropy statistics of lfq:365-398 over K = 2^D codes without the (rows, K) matrix, every stage and group in one launch.
+ * x f32 [S][N][G][D] (vqb_lfq_forward's ent); sg = s * G + g.  rows i32 [S * G][rows_stride] or NULL (rows 0..R-1): the R
+ * rows of each sg (rows_stride 0: one list shared by all sg).  m f32 [S]; logits 2 tau m (x . sgn_k).  Writes
+ * pse f64 [S * G][chunks][vqb_lfq_entropy_tiles(D)]: partial sums of h(p) = -p ln(max(p, 1e-5)) over the rows and codes, and
+ * colsum f32 [chunks][S * G][K] (NULL: not needed) partial column sums of p; each chunk covers ceil(R / chunks) rows.  Sums run
+ * in a fixed order: equal inputs give equal bits. */
+int vqb_lfq_entropy(const float* x, int64_t N, int G, int D, int S, const int32_t* rows, int64_t R, int64_t rows_stride,
+                    const float* m, float tau, int chunks, double* pse, float* colsum, void* stream);
+int vqb_lfq_entropy_tiles(int D);
+/* d/dx of the entropy outputs given dL/dp[sg][row][k] = cp[sg] h'(p) + V[sg][k] (cp f32 [S * G]; V f32 [S * G][K] or NULL),
+ * h'(p) = -(ln p + 1) for p >= 1e-5, -ln 1e-5 below.  Writes grad (the layout of x) at the listed rows only.  ksplit: a power
+ * of two dividing K into ranges of >= 16 codes; work f32 [ksplit][S * G][R][D + 1]. */
+int vqb_lfq_entropy_backward(const float* x, int64_t N, int G, int D, int S, const int32_t* rows, int64_t R, int64_t rows_stride,
+                             const float* m, float tau, const float* cp, const float* V, int ksplit, float* work, float* grad,
+                             void* stream);
+/* d z of vqb_lfq_forward's chain: grad_out [N][G][D] (dtype) through the straight-through value, plus grad_ent (f32, the
+ * layout of ent, or NULL) and cc[q] * (x - q) for the rows of rowmask (cc f32 [Q] or NULL: the commitment gradient), through
+ * the l2norm, the soft clamp and the residual chain; every stage recomputed from z.  grad_z [N][G][D] in dtype.  In eval
+ * (training 0) the value is q, which does not depend on z: grad_out contributes nothing. */
+int vqb_lfq_backward(const void* z, int dtype, int64_t N, int G, int D, int Q, int n_active, int residual, int training, int spherical,
+                     const float* params, const void* grad_out, const float* grad_ent, const float* cc, const uint8_t* rowmask,
+                     void* grad_z, void* stream);
+/* indices (int32 / int64, strided as in vqb_lfq_forward; -1 = dropped stage: zeros) -> codes f32 [Q][N][G][D] (bit set: vals[q],
+ * else -vals[q]) and / or out f32 [N][G][D], their fp32 sum over the stages in stage order. */
+int vqb_lfq_decode(const void* idx, int idx64, int64_t idx_s_row, int64_t idx_s_g, int64_t idx_s_q, int64_t N, int G, int D, int Q,
+                   const float* vals, float* out, float* codes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -110,6 +110,14 @@ SIGNATURES = {
                                _i64, _vp]),
     "vqb_fsq_backward": (_i32, [_vp, _i32, _i32, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vqb_fsq_decode": (_i32, [_vp, _i32, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "vqb_lfq_forward": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp,
+                               _vp, _i32, _vp]),
+    "vqb_lfq_forward_blocks": (_i32, [_i64, _i32]),
+    "vqb_lfq_entropy": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _vp, _f32, _i32, _vp, _vp, _vp]),
+    "vqb_lfq_entropy_tiles": (_i32, [_i32]),
+    "vqb_lfq_entropy_backward": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _vp, _f32, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "vqb_lfq_backward": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "vqb_lfq_decode": (_i32, [_vp, _i32, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
 }
 
 

@@ -2,7 +2,8 @@
 
 Drop-in for ONE path of lucidrains/vector-quantize-pytorch: `VectorQuantize`, `ResidualVQ`,
 `GroupedResidualVQ` forward (`(quantized, indices, commit_loss)`), the `Codebook` surface, `SimVQ`'s search,
-`ResidualSimVQ`, and finite scalar quantization (`FSQ`, `ResidualFSQ`, `GroupedResidualFSQ`).
+`ResidualSimVQ`, and finite scalar quantization (`FSQ`, `ResidualFSQ`, `GroupedResidualFSQ`)
+and lookup-free quantization (`LFQ`, `ResidualLFQ`, `GroupedResidualLFQ`).
 The hot path is hand-written CUDA (wgmma / TMA / mbarrier) in `csrc/`, bound through the C ABI in
 `include/vqb200.h`.  No Triton, no CPU fallback.
 """
@@ -13,6 +14,9 @@ from .sim_vq import SimVQ  # noqa: E402
 from .residual_sim_vq import ResidualSimVQ  # noqa: E402
 from .fsq import FSQ  # noqa: E402
 from .residual_fsq import ResidualFSQ, GroupedResidualFSQ  # noqa: E402
+from .lfq import LFQ  # noqa: E402
+from .residual_lfq import ResidualLFQ, GroupedResidualLFQ  # noqa: E402
 
 __all__ = ["Codebook", "EuclideanCodebook", "CosineSimCodebook", "VectorQuantize", "ResidualVQ", "GroupedResidualVQ", "SimVQ",
-           "ResidualSimVQ", "FSQ", "ResidualFSQ", "GroupedResidualFSQ"]
+           "ResidualSimVQ", "FSQ", "ResidualFSQ", "GroupedResidualFSQ",
+           "LFQ", "ResidualLFQ", "GroupedResidualLFQ"]

@@ -604,3 +604,111 @@ def fsq_decode(indices: torch.Tensor, D: int, work_dtype: torch.dtype, sym: bool
                                  _p(consts), _p(levels_basis), _p(scales), _p(out), _p(codes), _stream()), "vqb_fsq_decode")
     _count(1)
     return out, codes
+
+
+# ---- lookup-free quantization (csrc/vq_lfq.cu) ----
+
+def _sms(dev) -> int:
+    return torch.cuda.get_device_properties(dev).multi_processor_count
+
+
+def lfq_forward(z: torch.Tensor, Q: int, n_active: int, residual: bool, training: bool, spherical: bool, params: torch.Tensor,
+                indices: torch.Tensor, want_entropy: bool, rowmask: torch.Tensor | None, want_commit: bool):
+    """vqb_lfq_forward: z (N, G, D) contiguous fp32 / bf16 -> (out (N, G, D) in z's dtype, entropy input (n_active, N, G, D) fp32
+    or None, commitment sums (n_active,) fp64 or None); writes the int64 indices into `indices`, an (N, G, Q) view (any strides).
+    params (3, Q) fp32: per-stage scale, code magnitude, soft-clamp value (0: none)."""
+    _require_cuda(z, params, indices, rowmask)
+    if indices.dtype != torch.int64:
+        raise TypeError("LFQ indices are int64")
+    N, G, D = z.shape
+    dev = z.device
+    out = torch.empty(z.shape, dtype=z.dtype, device=dev)
+    ent = torch.empty((n_active, N, G, D), dtype=torch.float32, device=dev) if want_entropy else None
+    s_row, s_g, s_q = _fsq_strides(indices)
+    with torch.cuda.device(dev):
+        blocks = lib.vqb_lfq_forward_blocks(N, G)
+        check(min(blocks, 0), "vqb_lfq_forward_blocks")
+        commit = torch.empty((n_active, blocks), dtype=torch.float64, device=dev) if want_commit else None
+        check(lib.vqb_lfq_forward(_p(z), _dtype_code(z), N, G, D, Q, n_active, int(residual), int(training), int(spherical), _p(params),
+                                  _p(out), _p(indices), s_row, s_g, s_q, _p(ent), _p(rowmask), _p(commit), blocks, _stream()),
+              "vqb_lfq_forward")
+    _count(1)
+    return out, ent, (commit.sum(1) if commit is not None else None)
+
+
+def lfq_backward(z: torch.Tensor, grad_out: torch.Tensor, Q: int, n_active: int, residual: bool, training: bool, spherical: bool,
+                 params: torch.Tensor, grad_ent: torch.Tensor | None, cc: torch.Tensor | None, rowmask: torch.Tensor | None):
+    """vqb_lfq_backward: d z (z's dtype) of lfq_forward's outputs: grad_out (N, G, D) for `out`, grad_ent for the entropy input,
+    cc (n_active,) fp32 (the gradient of each stage's commitment sum, times 2) for the commitment sums."""
+    _require_cuda(z, grad_out, params, grad_ent, cc, rowmask)
+    N, G, D = z.shape
+    gz = torch.empty_like(z)
+    g = grad_out.to(z.dtype).contiguous()
+    ge = grad_ent.contiguous() if grad_ent is not None else None
+    with torch.cuda.device(z.device):
+        check(lib.vqb_lfq_backward(_p(z), _dtype_code(z), N, G, D, Q, n_active, int(residual), int(training), int(spherical),
+                                   _p(params), _p(g), _p(ge), _p(cc), _p(rowmask), _p(gz), _stream()), "vqb_lfq_backward")
+    _count(1)
+    return gz
+
+
+def lfq_entropy(x: torch.Tensor, rows: torch.Tensor | None, R: int, m: torch.Tensor, tau: float, want_colsum: bool):
+    """vqb_lfq_entropy over x (S, N, G, D) fp32: -> (sum of h(p) per (s, g) (S * G,) fp64, column sums of p (S * G, K) fp32 or
+    None).  rows: int32 (S * G, R) or (R,) row lists, or None for rows 0..R-1."""
+    _require_cuda(x, rows, m)
+    S, N, G, D = x.shape
+    SG, K, dev = S * G, 1 << D, x.device
+    tiles = lib.vqb_lfq_entropy_tiles(D)
+    check(min(tiles, 0), "vqb_lfq_entropy_tiles")
+    chunks = -(-4 * _sms(dev) // (tiles * SG))
+    chunks = max(1, min(chunks, -(-R // 32), 65535))
+    if want_colsum:
+        chunks = max(1, min(chunks, (8 << 20) // (SG * K)))   # partial column sums <= 32 MiB
+    rs = 0 if rows is None or rows.dim() == 1 else rows.shape[1]
+    pse = torch.empty((SG, chunks, tiles), dtype=torch.float64, device=dev)
+    col = torch.empty((chunks, SG, K), dtype=torch.float32, device=dev) if want_colsum else None
+    with torch.cuda.device(dev):
+        check(lib.vqb_lfq_entropy(_p(x), N, G, D, S, _p(rows), R, rs, _p(m), float(tau), chunks, _p(pse), _p(col), _stream()),
+              "vqb_lfq_entropy")
+    _count(1)
+    return pse.sum((1, 2)), (col.sum(0) if col is not None else None)
+
+
+def lfq_entropy_backward(x: torch.Tensor, rows: torch.Tensor | None, R: int, m: torch.Tensor, tau: float, cp: torch.Tensor,
+                         V: torch.Tensor | None) -> torch.Tensor:
+    """vqb_lfq_entropy_backward: d/dx (x's layout, zero outside the listed rows) given dL/dp = cp[sg] h'(p) + V[sg, k]."""
+    _require_cuda(x, rows, m, cp, V)
+    S, N, G, D = x.shape
+    SG, K, dev = S * G, 1 << D, x.device
+    blocks = -(-R // 128) * SG
+    ksplit = 1
+    while blocks * ksplit < 4 * _sms(dev) and K // (2 * ksplit) >= 2048:
+        ksplit *= 2
+    rs = 0 if rows is None or rows.dim() == 1 else rows.shape[1]
+    work = torch.empty((ksplit, SG, R, D + 1), dtype=torch.float32, device=dev)
+    grad = torch.zeros_like(x)
+    cp = cp.float().contiguous()
+    V = V.float().contiguous() if V is not None else None
+    with torch.cuda.device(dev):
+        check(lib.vqb_lfq_entropy_backward(_p(x), N, G, D, S, _p(rows), R, rs, _p(m), float(tau), _p(cp), _p(V), ksplit, _p(work),
+                                           _p(grad), _stream()), "vqb_lfq_entropy_backward")
+    _count(2)
+    return grad
+
+
+def lfq_decode(indices: torch.Tensor, D: int, vals: torch.Tensor, want_sum: bool, want_codes: bool):
+    """vqb_lfq_decode: indices, an (N, G, Q) view (any strides, int32 / int64, -1 = dropped) -> (sum over the stages (N, G, D) or
+    None, codes (Q, N, G, D) or None), fp32."""
+    _require_cuda(indices, vals)
+    if indices.dtype not in (torch.int32, torch.int64):
+        raise TypeError(f"LFQ indices must be int32 or int64, got {indices.dtype}")
+    N, G, Q = indices.shape
+    dev = indices.device
+    out = torch.empty((N, G, D), dtype=torch.float32, device=dev) if want_sum else None
+    codes = torch.empty((Q, N, G, D), dtype=torch.float32, device=dev) if want_codes else None
+    s_row, s_g, s_q = _fsq_strides(indices)
+    with torch.cuda.device(dev):
+        check(lib.vqb_lfq_decode(_p(indices), int(indices.dtype == torch.int64), s_row, s_g, s_q, N, G, D, Q, _p(vals), _p(out),
+                                 _p(codes), _stream()), "vqb_lfq_decode")
+    _count(1)
+    return out, codes
