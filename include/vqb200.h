@@ -426,6 +426,36 @@ int vqb_lfq_backward(const void* z, int dtype, int64_t N, int G, int D, int Q, i
 int vqb_lfq_decode(const void* idx, int idx64, int64_t idx_s_row, int64_t idx_s_g, int64_t idx_s_q, int64_t N, int G, int D, int Q,
                    const float* vals, float* out, float* codes, void* stream);
 
+/* Finite scalar perturbation (finite_scalar_perturbation.py "fsp"), one thread per row.  z [N][D] (D = len(levels) <= 16,
+ * N < 2^31) in dtype (f32 or bf16), every pointer to an [N][D] plane 16-byte aligned; levels i32 [D] on the device
+ * (prod(levels) < 2^31); act 0..4 = tanh, sigmoid, normal, laplace, cauchy; inv = need_inv_act.
+ * vqb_fsp_blocks(N): the CTA count of every fsp launch over N rows (sizes accept and the stats work), or a VQB_E_* code. */
+int vqb_fsp_blocks(int64_t N);
+/* The row chain of fsp:323-351.  clamp_hi: 1 - eps cast to dtype (clamp_max before floor).  u1, u2: the two uniform draws
+ * [N][D] in dtype (fsp:334, :340), or both NULL (eval, quantize_rate == 1: no perturbation); qrate: quantize_rate cast to dtype.
+ * inv_lo, inv_hi: eps and 1 - eps cast to the output dtype (need_inv_act's clamp).  out [N][D]: f32 when perturbing, else dtype.
+ * idx i32 [N]: the exact mixed-radix index; level_idx [N][D] in dtype or NULL; accept i32 [accept_blocks] (required when
+ * perturbing): per-CTA counts of accepted proposals, accept_blocks = vqb_fsp_blocks(N). */
+int vqb_fsp_forward(const void* z, int dtype, int64_t N, int D, int act, int inv, const int32_t* levels, float clamp_hi,
+                    const void* u1, const void* u2, float qrate, float inv_lo, float inv_hi, void* out, int32_t* idx,
+                    void* level_idx, int32_t* accept, int accept_blocks, void* stream);
+/* Batch moments of z over the rows (fsp:93-99) and VectorNorm's loss (fsp:126-133), in fp64 with partials added in a fixed
+ * order.  norm: host f64 [8] = l1_target, l1_weight, ..., l4_target, l4_weight.  work f64 [4 * blocks + 1][D], blocks =
+ * vqb_fsp_blocks(N).  stats [4][D] (mean, unbiased variance, skewness, kurtosis - 3) and loss [1] in dtype; aux f64 [D][8]
+ * (mean, clamped std, skewness, kurtosis, mean(t^2), clamp mask, variance, 0) for vqb_fsp_backward. */
+int vqb_fsp_stats(const void* z, int dtype, int64_t N, int D, const double* norm, double* work, int blocks, void* stats,
+                  void* loss, double* aux, void* stream);
+/* d z of the FSP step: grad_q [N][D] (grad_dtype; NULL: zero) through the output map and the CDF (the identity with inv), plus
+ * the statistics path from grad_stats f32 [4][D] and grad_loss f32 [1] (each NULL: zero), aux from vqb_fsp_stats.
+ * grad_z [N][D] in dtype. */
+int vqb_fsp_backward(const void* z, int dtype, int64_t N, int D, int act, int inv, const void* grad_q, int grad_dtype,
+                     const double* aux, const float* grad_stats, const float* grad_loss, const double* norm, void* grad_z,
+                     void* stream);
+/* indices (contiguous [N], int32 or int64) -> act values (l + 1/2) / L (act_out f32 [N][D] or NULL) and codes f32 [N][D] (or
+ * NULL): (act - 0.5) / 0.28867513459481287, or with inv the inverse CDF of act clamped to [lo, hi] (fsp:286-307). */
+int vqb_fsp_decode(const void* idx, int idx64, int64_t N, int D, int act, int inv, const int32_t* levels, float lo, float hi,
+                   float* act_out, float* codes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -118,6 +118,12 @@ SIGNATURES = {
     "vqb_lfq_entropy_backward": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _vp, _f32, _vp, _vp, _i32, _vp, _vp, _vp]),
     "vqb_lfq_backward": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vqb_lfq_decode": (_i32, [_vp, _i32, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "vqb_fsp_blocks": (_i32, [_i64]),
+    "vqb_fsp_forward": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _vp, _f32, _vp, _vp, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _i32,
+                               _vp]),
+    "vqb_fsp_stats": (_i32, [_vp, _i32, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "vqb_fsp_backward": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "vqb_fsp_decode": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _vp, _f32, _f32, _vp, _vp, _vp]),
 }
 
 

@@ -712,3 +712,96 @@ def lfq_decode(indices: torch.Tensor, D: int, vals: torch.Tensor, want_sum: bool
                                  _p(codes), _stream()), "vqb_lfq_decode")
     _count(1)
     return out, codes
+
+
+# ---- finite scalar perturbation (csrc/vq_fsp.cu) ----
+
+def _fsp_blocks(N: int) -> int:
+    blocks = lib.vqb_fsp_blocks(N)
+    check(min(blocks, 0), "vqb_fsp_blocks")
+    return blocks
+
+
+def _aligned(t: torch.Tensor) -> torch.Tensor:
+    t = t.contiguous()
+    return t.clone() if t.data_ptr() % 16 else t   # a contiguous view at an offset (the kernels move rows in 16-byte vectors)
+
+
+def fsp_forward(z: torch.Tensor, act: int, inv: bool, levels: torch.Tensor, clamp_hi: float, u1: torch.Tensor | None,
+                u2: torch.Tensor | None, qrate: float, inv_lo: float, inv_hi: float):
+    """vqb_fsp_forward: z (N, D) contiguous, 16-byte aligned, fp32 / bf16 -> (out (N, D), fp32 when perturbing else z's dtype;
+    indices (N,) int32; level indices (N, D) in z's dtype; the accepted-proposal count (int64 scalar) or None).  u1, u2: the
+    two (N, D) draws in z's dtype, or None for no perturbation."""
+    _require_cuda(z, levels, u1, u2)
+    N, D = z.shape
+    dev = z.device
+    out = torch.empty((N, D), dtype=torch.float32 if u1 is not None else z.dtype, device=dev)
+    idx = torch.empty((N,), dtype=torch.int32, device=dev)
+    lev = torch.empty((N, D), dtype=z.dtype, device=dev)
+    with torch.cuda.device(dev):
+        blocks = _fsp_blocks(N)
+        acc = torch.empty((blocks,), dtype=torch.int32, device=dev) if u1 is not None else None
+        check(lib.vqb_fsp_forward(_p(z), _dtype_code(z), N, D, act, int(inv), _p(levels), clamp_hi, _p(u1), _p(u2), qrate, inv_lo,
+                                  inv_hi, _p(out), _p(idx), _p(lev), _p(acc), blocks, _stream()), "vqb_fsp_forward")
+    _count(1)
+    return out, idx, lev, (acc.sum(dtype=torch.int64) if acc is not None else None)
+
+
+def _norm_arg(norm) -> ctypes.Array:
+    return (ctypes.c_double * 8)(*[float(v) for v in norm])
+
+
+def fsp_stats(z: torch.Tensor, norm):
+    """vqb_fsp_stats: z (N, D) -> (stats (4, D) = mean, variance, skewness, kurtosis in z's dtype, norm loss () in z's dtype,
+    aux (D, 8) fp64 for fsp_backward).  norm: (l1_target, l1_weight, ..., l4_target, l4_weight)."""
+    _require_cuda(z)
+    N, D = z.shape
+    dev = z.device
+    stats = torch.empty((4, D), dtype=z.dtype, device=dev)
+    loss = torch.empty((), dtype=z.dtype, device=dev)
+    aux = torch.empty((D, 8), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        blocks = _fsp_blocks(N)
+        work = torch.empty((4 * blocks + 1, D), dtype=torch.float64, device=dev)
+        check(lib.vqb_fsp_stats(_p(z), _dtype_code(z), N, D, _norm_arg(norm), _p(work), blocks, _p(stats), _p(loss), _p(aux),
+                                _stream()), "vqb_fsp_stats")
+    _count(4)
+    return stats, loss, aux
+
+
+def fsp_backward(z: torch.Tensor, act: int, inv: bool, grad_q: torch.Tensor | None, aux: torch.Tensor,
+                 grad_stats: torch.Tensor | None, grad_loss: torch.Tensor | None, norm) -> torch.Tensor:
+    """vqb_fsp_backward: d z (z's dtype) given the gradients of fsp_forward's out (N, D) and of fsp_stats' stats (4, D) and
+    loss (), each None for zero."""
+    _require_cuda(z, grad_q, aux, grad_stats, grad_loss)
+    N, D = z.shape
+    gz = torch.empty_like(z)
+    g = _aligned(grad_q) if grad_q is not None else None
+    gs = grad_stats.float().contiguous() if grad_stats is not None else None
+    gl = grad_loss.float().reshape(1) if grad_loss is not None else None
+    with torch.cuda.device(z.device):
+        check(lib.vqb_fsp_backward(_p(z), _dtype_code(z), N, D, act, int(inv), _p(g), _dtype_code(g) if g is not None else 0,
+                                   _p(aux), _p(gs), _p(gl), _norm_arg(norm), _p(gz), _stream()), "vqb_fsp_backward")
+    _count(1)
+    return gz
+
+
+def fsp_decode(indices: torch.Tensor, D: int, act: int, inv: bool, levels: torch.Tensor, lo: float, hi: float, want_act: bool,
+               want_codes: bool):
+    """vqb_fsp_decode: indices (any shape, int32 / int64) -> (act values, codes), each (*indices.shape, D) fp32 or None."""
+    _require_cuda(indices, levels)
+    if indices.dtype not in (torch.int32, torch.int64):
+        raise TypeError(f"FSP indices must be int32 or int64, got {indices.dtype}")
+    idx = indices.contiguous()
+    N = idx.numel()
+    dev = idx.device
+    shape = (*indices.shape, D)
+    act_out = torch.empty(shape, dtype=torch.float32, device=dev) if want_act else None
+    codes = torch.empty(shape, dtype=torch.float32, device=dev) if want_codes else None
+    if N == 0:
+        return act_out, codes
+    with torch.cuda.device(dev):
+        check(lib.vqb_fsp_decode(_p(idx), int(idx.dtype == torch.int64), N, D, act, int(inv), _p(levels), lo, hi, _p(act_out),
+                                 _p(codes), _stream()), "vqb_fsp_decode")
+    _count(1)
+    return act_out, codes
