@@ -456,6 +456,23 @@ int vqb_fsp_backward(const void* z, int dtype, int64_t N, int D, int act, int in
 int vqb_fsp_decode(const void* idx, int idx64, int64_t N, int D, int act, int inv, const int32_t* levels, float lo, float hi,
                    float* act_out, float* codes, void* stream);
 
+
+/* BinaryMapper (binary_mapper.py "bm"): the (rows, 2^bits) one-hot and its straight-through gradient, 1 <= bits <= 20.
+ * vqb_binmap_hot: out f32 [rows][2^bits], zero-filled by the caller and 16-byte aligned; idx i64 [rows] (the sampled code).
+ * Writes out[r][idx[r]]: 1 when logits is NULL (no straight-through), else fl(fl(1 + s) - s) with s the soft code of idx[r]
+ * from logits f32 [rows][bits] (bit 0 least significant).  A row with a non-finite logit is written whole: NaN where the
+ * reference's per-code log-probability is 0 * -inf or NaN, 0 elsewhere. */
+int vqb_binmap_hot(const float* logits, const int64_t* idx, int64_t rows, int bits, float* out, void* stream);
+/* The K split and segment width vqb_binmap_backward is run with for (rows, bits) on `sms` SMs: plan[0] = ksplit (a power of
+ * two), plan[1] = codes per segment (min(32, 2^bits)).  Host-only. */
+int vqb_binmap_backward_plan(int64_t rows, int bits, int sms, int* plan);
+/* d logits [rows][bits] f32 of sum(out * g) through the straight-through soft codes: S1_j - sigmoid(l_j) S with
+ * S = sum_k g_k s_k, S1_j = sum_{bit_j(k) = 1} g_k s_k, evaluated as sigmoid(-l_j) S1_j - sigmoid(l_j) S0_j.  g[r][k] at
+ * g + r * g_row_stride + k * g_col_stride (floats, any 4-byte alignment, strides >= 0).  ksplit: a power of two dividing
+ * the segment count; ksplit > 1 needs work f64 [rows][ksplit][2 bits].  Rows with a non-finite logit get NaN. */
+int vqb_binmap_backward(const float* logits, int64_t rows, int bits, const float* g, int64_t g_row_stride,
+                        int64_t g_col_stride, int ksplit, double* work, float* dlogits, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -124,6 +124,9 @@ SIGNATURES = {
     "vqb_fsp_stats": (_i32, [_vp, _i32, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp]),
     "vqb_fsp_backward": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vqb_fsp_decode": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _vp, _f32, _f32, _vp, _vp, _vp]),
+    "vqb_binmap_hot": (_i32, [_vp, _vp, _i64, _i32, _vp, _vp]),
+    "vqb_binmap_backward_plan": (_i32, [_i64, _i32, _i32, _vp]),
+    "vqb_binmap_backward": (_i32, [_vp, _i64, _i32, _vp, _i64, _i64, _i32, _vp, _vp, _vp]),
 }
 
 

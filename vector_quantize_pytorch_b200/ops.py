@@ -805,3 +805,46 @@ def fsp_decode(indices: torch.Tensor, D: int, act: int, inv: bool, levels: torch
                                  _p(codes), _stream()), "vqb_fsp_decode")
     _count(1)
     return act_out, codes
+
+
+# ---- BinaryMapper (csrc/vq_binmap.cu) ----
+
+def binmap_hot(out: torch.Tensor, logits: torch.Tensor | None, indices: torch.Tensor) -> torch.Tensor:
+    """vqb_binmap_hot: writes the hot element of every row of the zero-filled out (rows, 2^bits) fp32 in place: 1, or with
+    logits (rows, bits) fp32 contiguous the straight-through value fl(fl(1 + s) - s).  indices: (rows,) int64."""
+    _require_cuda(out, logits, indices)
+    rows, K = out.shape
+    if rows == 0:
+        return out
+    idx = indices.to(torch.int64).contiguous()
+    with torch.cuda.device(out.device):
+        check(lib.vqb_binmap_hot(_p(logits), _p(idx), rows, K.bit_length() - 1, _p(out), _stream()), "vqb_binmap_hot")
+    _count(1)
+    return out
+
+
+def binmap_backward_plan(rows: int, bits: int, sms: int) -> tuple[int, int]:
+    """(ksplit, codes per segment) of vqb_binmap_backward for (rows, bits) on `sms` SMs."""
+    plan = (ctypes.c_int * 2)()
+    check(lib.vqb_binmap_backward_plan(rows, bits, sms, plan), "vqb_binmap_backward_plan")
+    return plan[0], plan[1]
+
+
+def binmap_backward(logits: torch.Tensor, g: torch.Tensor, ksplit: int | None = None) -> torch.Tensor:
+    """vqb_binmap_backward: d logits (rows, bits) fp32 of sum(out * g) through the soft codes.  logits (rows, bits) fp32
+    contiguous; g (rows, 2^bits) fp32 with any non-negative strides and offset (read in place).  ksplit: the plan's by default."""
+    _require_cuda(logits, g)
+    rows, bits = logits.shape
+    dl = torch.empty((rows, bits), dtype=torch.float32, device=logits.device)
+    if rows == 0:
+        return dl
+    if g.dtype != torch.float32:
+        g = g.float()
+    with torch.cuda.device(logits.device):
+        if ksplit is None:
+            ksplit = binmap_backward_plan(rows, bits, torch.cuda.get_device_properties(logits.device).multi_processor_count)[0]
+        work = torch.empty((rows, ksplit, 2 * bits), dtype=torch.float64, device=logits.device) if ksplit > 1 else None
+        check(lib.vqb_binmap_backward(_p(logits), rows, bits, _p(g), g.stride(0), g.stride(1), ksplit, _p(work), _p(dl),
+                                      _stream()), "vqb_binmap_backward")
+    _count(1 if ksplit == 1 else 2)
+    return dl
