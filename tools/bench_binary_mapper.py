@@ -14,55 +14,14 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from gpu_measure import gpu_info, time_ms, peak_mib  # noqa: E402
+
 HBM_BYTES_PER_S = 3.35e12
-
-
-def gpu_info():
-    import torch
-    name = torch.cuda.get_device_name(0)
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-        power, clock = [s.strip() for s in q.split(",")]
-    except (OSError, subprocess.SubprocessError, ValueError):
-        power, clock = "unknown", "unknown"
-    return name, power, clock
-
-
-def time_ms(fn, seconds, warmup):
-    import torch
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    fn()
-    e1.record()
-    torch.cuda.synchronize()
-    one = max(e0.elapsed_time(e1), 1e-3)
-    n = max(1, int(seconds * 1e3 / one))
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / n
-
-
-def peak_mib(fn):
-    import torch
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    base = torch.cuda.memory_allocated()
-    fn()
-    torch.cuda.synchronize()
-    return (torch.cuda.max_memory_allocated() - base) / 2 ** 20
 
 
 def eager_reference(x, bits, power_two, codes, temperature=1.0, threshold=math.log(2)):

@@ -18,7 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_lfq import gpu_info, time_ms  # noqa: E402
+from gpu_measure import gpu_info, time_ms  # noqa: E402
 
 HBM = 3.35e12
 

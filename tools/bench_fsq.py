@@ -12,45 +12,14 @@ the GPU's name and power limit belong with the numbers.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from gpu_measure import gpu_info, time_ms  # noqa: E402
+
 HBM = 3.35e12
-
-
-def gpu_info():
-    import torch
-    name = torch.cuda.get_device_name(0)
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        power = "unknown"
-    return name, power
-
-
-def time_ms(fn, seconds, warmup):
-    """Mean ms per call over enough calls to fill `seconds` (CUDA events around the whole batch)."""
-    import torch
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    torch.cuda.synchronize()
-    one = max(s.elapsed_time(e), 1e-3)
-    iters = max(10, int(seconds * 1e3 / one))
-    s.record()
-    for _ in range(iters):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / iters
 
 
 def eager_forward(m, x):
@@ -92,8 +61,12 @@ def main():
     levels = [int(v) for v in args.levels.split(",")]
     b, n = (int(v) for v in args.shape.split(","))
     d, Q = len(levels), args.stages
-    name, power = gpu_info()
-    res = dict(gpu=name, power_limit=power, dim=args.dim, levels=levels, stages=Q, shape=[b, n, args.dim])
+    name, power, clock = gpu_info()
+    res = dict(gpu=name, power_limit=power, max_sm_clock=clock, dim=args.dim, levels=levels, stages=Q, shape=[b, n, args.dim])
+
+    def ms(fn):
+        return time_ms(fn, args.seconds, args.warmup, min_iters=10)
+
     for dt_name, dt in (("fp32", torch.float32), ("bf16", torch.bfloat16)):
         torch.manual_seed(0)
         m = vqb.ResidualFSQ(dim=args.dim, levels=levels, num_quantizers=Q).to("cuda", dt).train()
@@ -136,11 +109,11 @@ def main():
         ew = torch.empty((), dtype=work).element_size()
         fwd_bytes = N * d * ez + N * d * ew + N * Q * 4
         bwd_bytes = N * d * ez + N * d * ew + N * d * ez
-        kf, kb = time_ms(kern_fwd, args.seconds, args.warmup), time_ms(kern_bwd, args.seconds, args.warmup)
+        kf, kb = ms(kern_fwd), ms(kern_bwd)
         res[dt_name] = dict(
-            forward_ms=time_ms(fwd, args.seconds, args.warmup), forward_backward_ms=time_ms(fwd_bwd, args.seconds, args.warmup),
-            eager_forward_ms=time_ms(eager_fwd, args.seconds, args.warmup),
-            eager_forward_backward_ms=time_ms(eager_fwd_bwd, args.seconds, args.warmup),
+            forward_ms=ms(fwd), forward_backward_ms=ms(fwd_bwd),
+            eager_forward_ms=ms(eager_fwd),
+            eager_forward_backward_ms=ms(eager_fwd_bwd),
             kernel_forward_ms=kf, kernel_forward_bytes=fwd_bytes, kernel_forward_hbm_share=fwd_bytes / (kf * 1e-3) / HBM,
             kernel_backward_ms=kb, kernel_backward_bytes=bwd_bytes, kernel_backward_hbm_share=bwd_bytes / (kb * 1e-3) / HBM)
     print(json.dumps(res))

@@ -1,6 +1,6 @@
 """Time one training step — forward, backward, optimizer.step — of a codebook learnt by gradient, against an eager-torch
 restatement of the reference's step (vector_quantize_pytorch.py:674-791, :1212-1237, :1327; residual_vq.py:469-606), with CUDA
-events after warm-up.  Prints the card's name, power limit and SM clock with the numbers (one JSON line per step kind).
+events after warm-up.  Prints the card's name, power limit and maximum SM clock with the numbers (one JSON line per step kind).
 
     python tools/bench_learnable.py [--steps 10] [--warmup 3]
 
@@ -12,7 +12,6 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
@@ -20,6 +19,7 @@ import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import vector_quantize_pytorch_b200 as vqb  # noqa: E402
+from gpu_measure import gpu_info, time_ms  # noqa: E402
 
 DEV = "cuda"
 
@@ -91,19 +91,6 @@ class EagerRVQ(torch.nn.Module):
 
 
 # ---------------------------------------------------------------- timing
-def time_steps(step, steps, warmup):
-    for _ in range(warmup):
-        step()
-    torch.cuda.synchronize()
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-    ev[0].record()
-    for _ in range(steps):
-        step()
-    ev[1].record()
-    torch.cuda.synchronize()
-    return ev[0].elapsed_time(ev[1]) / steps
-
-
 def make_step(mod, x, G, fwd):
     opt = torch.optim.SGD(mod.parameters(), lr=1e-3)
 
@@ -124,12 +111,6 @@ def eager_fwd(mod, x):
     return mod(x)
 
 
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
@@ -138,7 +119,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_learnable: needs a CUDA device")
     torch.manual_seed(0)
-    gpu = card()
+    gpu = ", ".join(gpu_info())
     cases = []
     D, K = 256, 1024
     xa = torch.randn(64, 4096, D, device=DEV).bfloat16().requires_grad_(True)
@@ -153,8 +134,8 @@ def main():
     cases.append(("C_diveq_bf16", c, EagerVQ(c._codebook.embed.detach()[0], diveq=True), xa, Ga))
     for name, ours, eager, x, G in cases:
         eager = eager.to(DEV).train()
-        t_ours = time_steps(make_step(ours, x, G, ours_fwd), args.steps, args.warmup)
-        t_eager = time_steps(make_step(eager, x, G, eager_fwd), args.steps, args.warmup)
+        t_ours = time_ms(make_step(ours, x, G, ours_fwd), None, args.warmup, iters=args.steps)
+        t_eager = time_ms(make_step(eager, x, G, eager_fwd), None, args.warmup, iters=args.steps)
         print(json.dumps({"case": name, "rows": x.numel() // D, "ms_per_step": round(t_ours, 3), "eager_ms_per_step": round(t_eager, 3),
                           "speedup": round(t_eager / t_ours, 2), "gpu": gpu}), flush=True)
         del eager

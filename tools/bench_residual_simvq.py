@@ -10,11 +10,12 @@ backward.  Prints one JSON line with the GPU's name and power limit, which belon
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+
+from gpu_measure import gpu_info, time_ms  # noqa: E402
 
 
 def rotate_to(src, tgt):   # vector_quantize_pytorch.py:287-318
@@ -42,31 +43,6 @@ def eager_forward(layers, x, rotation):
         qout = qout + out
         idx.append(ind)
     return qout, torch.stack(idx, -1), torch.stack(losses)
-
-
-def gpu_info():
-    import torch
-    name = torch.cuda.get_device_name(0)
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        power = "unknown"
-    return name, power
-
-
-def time_ms(fn, iters, warmup):
-    import torch
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
 
 
 def main():
@@ -121,9 +97,9 @@ def main():
     res = {}
     for name, fn in (("ours_fwd_ms", ours_fwd), ("eager_fwd_ms", eager_fwd), ("ours_fwd_bwd_ms", ours_fwd_bwd),
                      ("eager_fwd_bwd_ms", eager_fwd_bwd)):
-        res[name] = round(time_ms(fn, args.iters, args.warmup), 3)
-    gpu, power = gpu_info()
-    res.update(gpu=gpu, power_limit=power, dim=args.dim, stages=args.stages, codes=args.codes, rows=args.rows,
+        res[name] = round(time_ms(fn, None, args.warmup, iters=args.iters), 3)
+    gpu, power, clock = gpu_info()
+    res.update(gpu=gpu, power_limit=power, max_sm_clock=clock, dim=args.dim, stages=args.stages, codes=args.codes, rows=args.rows,
                rotation_trick=rotation, index_agreement=round(agree, 6),
                fwd_speedup=round(res["eager_fwd_ms"] / res["ours_fwd_ms"], 2),
                fwd_bwd_speedup=round(res["eager_fwd_bwd_ms"] / res["ours_fwd_bwd_ms"], 2))

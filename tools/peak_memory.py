@@ -16,22 +16,12 @@ import argparse
 import gc
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-
-def gpu_info():
-    import torch
-    name = torch.cuda.get_device_name(0)
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        power = "unknown"
-    return name, power
+from gpu_measure import gpu_info  # noqa: E402
 
 
 def measure(make, x, schedule):
@@ -75,8 +65,8 @@ def main():
     x = torch.randn(32, 8192, 256, device=dev)
     res["rvq_shared_train_eval_peak_bytes"], res["rvq_shared_train_eval_held_bytes"] = measure(
         lambda: vqb.ResidualVQ(dim=256, num_quantizers=8, codebook_size=1024, shared_codebook=True).to(dev), x, [True, False])
-    gpu, power = gpu_info()
-    res.update(gpu=gpu, power_limit=power, steps=args.steps)
+    gpu, power, clock = gpu_info()
+    res.update(gpu=gpu, power_limit=power, max_sm_clock=clock, steps=args.steps)
     print(json.dumps(res))
 
 

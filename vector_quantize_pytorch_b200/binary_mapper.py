@@ -19,7 +19,6 @@ from torch.autograd.function import once_differentiable
 from . import ops
 from .codebook import _unsupported
 
-_FLOAT = (torch.float32, torch.bfloat16)
 _MAX_BITS = 20
 NAT = math.log(2)
 
@@ -104,10 +103,7 @@ class BinaryMapper(nn.Module):
             straight_through = self.training
         if calc_aux_loss is None:
             calc_aux_loss = self.training
-        if logits.dtype not in _FLOAT:
-            raise TypeError(f"vqb200 BinaryMapper supports float32 and bfloat16 logits, got {logits.dtype}")
-        if not logits.is_cuda:
-            raise RuntimeError("vqb200 has no CPU path: logits must live on a CUDA (H100, sm_90) device")
+        logits = ops.float_input(logits, "BinaryMapper", what="logits")
         if straight_through and logits.dtype != torch.float32:
             raise TypeError(f"BinaryMapper's straight-through needs float32 logits, got {logits.dtype}: the reference's einsum "
                             f"of {logits.dtype} log-sigmoids against the float code table cannot run either")
@@ -121,7 +117,7 @@ class BinaryMapper(nn.Module):
         if calc_aux_loss:
             aux = self.calc_aux_loss(logits, reduce_aux_kl_loss=reduce_aux_kl_loss)
         if straight_through:
-            one_hot = _BinaryMapperST.apply(flat.contiguous(), indices, self.num_codes)
+            one_hot = _BinaryMapperST.apply(flat, indices, self.num_codes)
         else:
             one_hot = ops.binmap_hot(torch.zeros((flat.shape[0], self.num_codes), dtype=torch.float32, device=flat.device),
                                      None, indices)

@@ -1,9 +1,46 @@
-// Row moves of the one-thread-per-row kernels (vq_fsq.cu, vq_fsp.cu): the D values of one item in registers.
+// Helpers of the one-thread-per-row kernels (vq_fsq.cu, vq_lfq.cu, vq_fsp.cu, vq_binmap.cu): row moves with the D values of
+// one item in registers, the rounding and division primitives, index access and the host's alignment test and D dispatch.
 #pragma once
 #include "vqb_common.cuh"
 
 namespace vqb {
 namespace {
+
+// Rounds to the chain's work dtype: bf16 when BF, else fp32 (no-op).
+template <bool BF> __device__ __forceinline__ float rw(float v) { return BF ? bf16_round(v) : v; }
+
+// a / b, correctly rounded, for a divisor b with rb = RN(1 / b) (Markstein: q0 = RN(a rb) is within an ulp of a / b, the
+// remainder a - b q0 is exact in one fma, and RN(q0 + rem rb) = RN(a / b) while nothing over- or underflows; an infinite or
+// NaN q0 is returned as it is).  Every division by a constant goes through it, with the reciprocal computed by the caller, so no
+// kernel carries a call to the division's slow path (whose calling convention spills).
+__device__ __forceinline__ float divc(float a, float b, float rb) {
+  const float q0 = __fmul_rn(a, rb);
+  if (!isfinite(q0)) return q0;
+  return __fmaf_rn(__fmaf_rn(-b, q0, a), rb, q0);
+}
+
+// Element `off` of an int32 (idx64 = 0) or int64 index array.
+__device__ __forceinline__ int64_t load_index(const void* idx, int idx64, int64_t off) {
+  return idx64 ? reinterpret_cast<const int64_t*>(idx)[off] : static_cast<int64_t>(reinterpret_cast<const int32_t*>(idx)[off]);
+}
+
+__device__ __forceinline__ void store_index(void* idx, int idx64, int64_t off, int64_t v) {
+  if (idx64) reinterpret_cast<int64_t*>(idx)[off] = v;
+  else reinterpret_cast<int32_t*>(idx)[off] = static_cast<int32_t>(v);
+}
+
+// Whether p is a multiple of n bytes (the host's check of what a kernel's widest access needs).
+inline bool aligned(const void* p, int n) { return reinterpret_cast<uintptr_t>(p) % n == 0; }
+
+// CALL(D) for the row width D = 1..16 the kernels are instantiated for; any other D returns VQB_E_UNSUPPORTED.
+#define VQB_SWITCH_D(CALL)                                                                                                  \
+  switch (D) {                                                                                                              \
+    case 1: CALL(1); break; case 2: CALL(2); break; case 3: CALL(3); break; case 4: CALL(4); break;                         \
+    case 5: CALL(5); break; case 6: CALL(6); break; case 7: CALL(7); break; case 8: CALL(8); break;                         \
+    case 9: CALL(9); break; case 10: CALL(10); break; case 11: CALL(11); break; case 12: CALL(12); break;                   \
+    case 13: CALL(13); break; case 14: CALL(14); break; case 15: CALL(15); break; case 16: CALL(16); break;                 \
+    default: return VQB_E_UNSUPPORTED;                                                                                      \
+  }
 
 // The D values of one item as 32-bit words, moved with the widest accesses the row size allows (the host checks the 16-byte
 // alignment of every base pointer); bf16 rows of odd D move element by element.

@@ -525,14 +525,6 @@ __global__ void rotate_kernel(const void* __restrict__ src, const void* __restri
   }
 }
 
-static inline int row_grid(int64_t rows, int wpb) {
-  int64_t g = (rows + wpb - 1) / wpb;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return static_cast<int>(g);
-}
-
 }  // namespace vqb
 
 using namespace vqb;
@@ -580,7 +572,7 @@ extern "C" int vqb_input_prepare(const void* x, int dtype, int64_t N, int D, int
   if (D % 4 != 0) return VQB_E_UNSUPPORTED;   // 4 elements per lane and step
   if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(x_eff) | reinterpret_cast<uintptr_t>(a_planes)) & 15) return VQB_E_ALIGN;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int g = row_grid(N, ROW_THREADS / 32);
+  const int g = capped_grid(N, ROW_THREADS / 32, 16);
   if (dtype == VQB_DTYPE_F32)
     input_prepare_kernel<VQB_DTYPE_F32><<<g, ROW_THREADS, 0, s>>>(x, N, D, metric, x_eff, static_cast<uint16_t*>(a_planes), n_planes);
   else
@@ -626,7 +618,7 @@ extern "C" int vqb_gather(const void* x_eff, int dtype, int64_t N, int D, const 
   const int rc = make_fused(&fo, &f, D);
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int g = row_grid(N, ROW_THREADS / 32);
+  const int g = capped_grid(N, ROW_THREADS / 32, 16);
   if (dtype == VQB_DTYPE_F32) gather_kernel<VQB_DTYPE_F32><<<g, ROW_THREADS, 0, s>>>(N, D, idx, fo);
   else gather_kernel<VQB_DTYPE_BF16><<<g, ROW_THREADS, 0, s>>>(N, D, idx, fo);
   return static_cast<int>(cudaGetLastError());
@@ -689,7 +681,7 @@ extern "C" int vqb_decode(const float* embeds, int64_t embed_stride, int Q, int 
   if (D % 8 != 0) return VQB_E_UNSUPPORTED;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (gather_sum_smem<false>(embeds, embed_stride, Q, K, D, idx, N, out, dtype, s)) return static_cast<int>(cudaGetLastError());
-  const int g = row_grid(N, ROW_THREADS / 32);
+  const int g = capped_grid(N, ROW_THREADS / 32, 16);
   if (dtype == VQB_DTYPE_F32)
     rvq_accumulate_kernel<VQB_DTYPE_F32, false><<<g, ROW_THREADS, 0, s>>>(embeds, embed_stride, Q, D, idx, N, out);
   else
@@ -704,7 +696,7 @@ extern "C" int vqb_rvq_accumulate(const float* embeds, int64_t embed_stride, int
   if (D % 8 != 0) return VQB_E_UNSUPPORTED;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (gather_sum_smem<true>(embeds, embed_stride, Q, K, D, idx, N, out, dtype, s)) return static_cast<int>(cudaGetLastError());
-  const int g = row_grid(N, ROW_THREADS / 32);
+  const int g = capped_grid(N, ROW_THREADS / 32, 16);
   if (dtype == VQB_DTYPE_F32)
     rvq_accumulate_kernel<VQB_DTYPE_F32, true><<<g, ROW_THREADS, 0, s>>>(embeds, embed_stride, Q, D, idx, N, out);
   else
@@ -723,7 +715,7 @@ extern "C" int vqb_rotate(const void* src, const void* tgt, const void* grad_out
   if (!src || !tgt || !out || N <= 0 || D <= 0) return VQB_E_INVALID;
   if (dtype != VQB_DTYPE_F32 && dtype != VQB_DTYPE_BF16) return VQB_E_INVALID;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int g = row_grid(N, ROW_THREADS / 32);
+  const int g = capped_grid(N, ROW_THREADS / 32, 16);
   if (dtype == VQB_DTYPE_F32) {
     if (grad_out) rotate_kernel<VQB_DTYPE_F32, true><<<g, ROW_THREADS, 0, s>>>(src, tgt, grad_out, N, D, out);
     else rotate_kernel<VQB_DTYPE_F32, false><<<g, ROW_THREADS, 0, s>>>(src, tgt, nullptr, N, D, out);

@@ -9,6 +9,7 @@
 //                           g_k s_k and S0_j (bit 0) come from the segment column (low bits) and per-segment sums (high bits).
 //   binmap_bwd_fin_kernel   adds the K chunks' fp64 partials in chunk order: d logit_j = sigmoid(-l_j) S1_j - sigmoid(l_j) S0_j.
 #include "vqb_common.cuh"
+#include "row_io.cuh"
 
 namespace vqb {
 namespace {
@@ -225,8 +226,6 @@ void bwd_plan(int64_t rows, int bits, int sms, int* ksplit, int* seg) {
   *seg = 1 << lb;
 }
 
-bool aligned(const void* p, int n) { return (reinterpret_cast<uintptr_t>(p) % n) == 0; }
-
 }  // namespace
 }  // namespace vqb
 
@@ -236,8 +235,7 @@ extern "C" int vqb_binmap_hot(const float* logits, const int64_t* idx, int64_t r
   if (bits > BM_MAX_BITS || rows >= (int64_t{1} << 40)) return VQB_E_UNSUPPORTED;
   if (!aligned(out, 16) || !aligned(idx, 8) || (logits && !aligned(logits, 4))) return VQB_E_ALIGN;
   if (const int rc = check_device()) return rc;
-  const int64_t need = (rows + HOT_THREADS - 1) / HOT_THREADS, cap = static_cast<int64_t>(num_sms()) * 16;
-  const int grid = static_cast<int>(need < cap ? need : cap);
+  const int grid = capped_grid(rows, HOT_THREADS, 16);
   binmap_hot_kernel<<<grid, HOT_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(logits, idx, rows, bits, out);
   return static_cast<int>(cudaGetLastError());
 }

@@ -87,14 +87,6 @@ __global__ void __launch_bounds__(DV_THREADS) diveq_kernel(const void* __restric
   }
 }
 
-inline int dv_grid(int64_t rows) {
-  const int wpb = DV_THREADS / 32;
-  int64_t g = (rows + wpb - 1) / wpb;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  return static_cast<int>(g < 1 ? 1 : g);
-}
-
 }  // namespace
 }  // namespace vqb
 
@@ -111,7 +103,7 @@ extern "C" int vqb_diveq(const void* x, const void* q, const void* noise, const 
                         reinterpret_cast<uintptr_t>(grad_out) | reinterpret_cast<uintptr_t>(out);
   if ((any & (esz - 1)) || (reinterpret_cast<uintptr_t>(grad_q) & 3)) return VQB_E_ALIGN;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int g = dv_grid(N);
+  const int g = capped_grid(N, DV_THREADS / 32, 16);
   if (dtype == VQB_DTYPE_F32) {
     if (grad_out) diveq_kernel<VQB_DTYPE_F32, true><<<g, DV_THREADS, 0, s>>>(x, q, noise, grad_out, N, D, noise_scale, out, grad_q);
     else diveq_kernel<VQB_DTYPE_F32, false><<<g, DV_THREADS, 0, s>>>(x, q, noise, nullptr, N, D, noise_scale, out, nullptr);

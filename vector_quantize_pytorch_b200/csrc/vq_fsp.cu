@@ -25,6 +25,7 @@ namespace vqb {
 namespace {
 
 constexpr int FSP_THREADS = 256;
+constexpr int FSP_CTAS_PER_SM = 8;   // grid cap; vqb_fsp_blocks reports the grid, which orders the partial sums
 constexpr int FSP_MAX_D = 16;
 constexpr float SQRT2F = 1.41421356237309515f;   // fsp:47, as fp32
 constexpr float PIF = 3.14159265358979312f;      // torch.pi, as fp32
@@ -35,19 +36,7 @@ constexpr float R_UNIT_STD = 1.f / UNIT_STD;
 
 enum { ACT_TANH = 0, ACT_SIGMOID = 1, ACT_NORMAL = 2, ACT_LAPLACE = 3, ACT_CAUCHY = 4 };
 
-template <bool BF> __device__ __forceinline__ float rw(float v) { return BF ? bf16_round(v) : v; }
-
 __device__ __forceinline__ float sgn(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : v); }   // torch.sign keeps 0 and NaN
-
-// a / b, correctly rounded, for a divisor b with rb = RN(1 / b) (Markstein: q0 = RN(a rb) is within an ulp of a / b, the
-// remainder a - b q0 is exact in one fma, and RN(q0 + rem rb) = RN(a / b) while nothing over- or underflows; an infinite or
-// NaN q0 is returned as it is).  Every division by a constant goes through it, so no kernel carries a call to the division's
-// slow path (whose calling convention spills).
-__device__ __forceinline__ float divc(float a, float b, float rb) {
-  const float q0 = __fmul_rn(a, rb);
-  if (!isfinite(q0)) return q0;
-  return __fmaf_rn(__fmaf_rn(-b, q0, a), rb, q0);
-}
 
 // 1 / x in fp64 for a normal, finite x != 0: the hardware estimate refined by three Newton steps (each squares the relative
 // error, which ends at the fp64 rounding), with no call to the division's slow path (whose calling convention spills).
@@ -430,7 +419,7 @@ __global__ void __launch_bounds__(FSP_THREADS) fsp_decode_kernel(const void* __r
   load_levels<D>(t, levels);
   const auto id = [](float v) { return v; };
   for (int64_t row = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; row < N; row += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    const int64_t ix = idx64 ? reinterpret_cast<const int64_t*>(idx)[row] : static_cast<int64_t>(reinterpret_cast<const int32_t*>(idx)[row]);
+    const int64_t ix = load_index(idx, idx64, row);
     const int64_t m = floor_mod(ix, t.size);
     float p[D], c[D];
 #pragma unroll
@@ -446,14 +435,6 @@ __global__ void __launch_bounds__(FSP_THREADS) fsp_decode_kernel(const void* __r
   }
 }
 
-int fsp_grid(int64_t N) {
-  const int64_t need = (N + FSP_THREADS - 1) / FSP_THREADS;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  return static_cast<int>(need < cap ? (need > 0 ? need : 1) : cap);
-}
-
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 int fsp_shape(int64_t N, int D, int dtype) {
   if (N <= 0 || D < 1) return VQB_E_INVALID;
   if (dtype != VQB_DTYPE_F32 && dtype != VQB_DTYPE_BF16) return VQB_E_INVALID;
@@ -466,15 +447,6 @@ NormW norm_weights(const double* norm) {
   for (int k = 0; k < 4; ++k) { w.t[k] = norm[2 * k]; w.w[k] = norm[2 * k + 1]; }
   return w;
 }
-
-#define VQB_FSP_SWITCH_D(CALL)                                                                                              \
-  switch (D) {                                                                                                              \
-    case 1: CALL(1); break; case 2: CALL(2); break; case 3: CALL(3); break; case 4: CALL(4); break;                         \
-    case 5: CALL(5); break; case 6: CALL(6); break; case 7: CALL(7); break; case 8: CALL(8); break;                         \
-    case 9: CALL(9); break; case 10: CALL(10); break; case 11: CALL(11); break; case 12: CALL(12); break;                   \
-    case 13: CALL(13); break; case 14: CALL(14); break; case 15: CALL(15); break; case 16: CALL(16); break;                 \
-    default: return VQB_E_UNSUPPORTED;                                                                                      \
-  }
 
 // ACT and INV as template arguments; with need_inv_act the backward does not depend on the CDF (one instantiation).
 #define VQB_FSP_SWITCH_ACT(CALL, DD, BFV)                                                                                   \
@@ -500,7 +472,7 @@ extern "C" int vqb_fsp_blocks(int64_t N) {
   if (N <= 0) return VQB_E_INVALID;
   if (N >= (int64_t{1} << 31)) return VQB_E_UNSUPPORTED;
   if (const int rc = check_device()) return rc;
-  return fsp_grid(N);
+  return capped_grid(N, FSP_THREADS, FSP_CTAS_PER_SM);
 }
 
 extern "C" int vqb_fsp_forward(const void* z, int dtype, int64_t N, int D, int act, int inv, const int32_t* levels, float clamp_hi,
@@ -510,10 +482,11 @@ extern "C" int vqb_fsp_forward(const void* z, int dtype, int64_t N, int D, int a
   if (!z || !levels || !out || !idx || (!u1 != !u2) || (u1 && !accept)) return VQB_E_INVALID;
   if (act < ACT_TANH || act > ACT_CAUCHY) return VQB_E_INVALID;
   if (const int rc = fsp_shape(N, D, dtype)) return rc;
-  if (!aligned16(z) || !aligned16(out) || (u1 && (!aligned16(u1) || !aligned16(u2))) || (level_idx && !aligned16(level_idx)))
+  if (!aligned(z, 16) || !aligned(out, 16) || (u1 && (!aligned(u1, 16) || !aligned(u2, 16))) ||
+      (level_idx && !aligned(level_idx, 16)))
     return VQB_E_ALIGN;
   if (const int rc = check_device()) return rc;
-  const int grid = fsp_grid(N);
+  const int grid = capped_grid(N, FSP_THREADS, FSP_CTAS_PER_SM);
   if (accept && accept_blocks != grid) return VQB_E_INVALID;   // vqb_fsp_blocks() sizes the counts
   const FwdArgs a{z, u1, u2, levels, N, clamp_hi, qrate, inv_lo, inv_hi, out, idx, level_idx, u1 ? accept : nullptr};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -522,7 +495,7 @@ extern "C" int vqb_fsp_forward(const void* z, int dtype, int64_t N, int D, int a
 #define VQB_FSP_FWD(DD)                                                \
   if (bf) { VQB_FSP_SWITCH_ACT(VQB_FSP_FWD_LAUNCH, DD, true) }         \
   else { VQB_FSP_SWITCH_ACT(VQB_FSP_FWD_LAUNCH, DD, false) }
-  VQB_FSP_SWITCH_D(VQB_FSP_FWD)
+  VQB_SWITCH_D(VQB_FSP_FWD)
 #undef VQB_FSP_FWD
 #undef VQB_FSP_FWD_LAUNCH
   return static_cast<int>(cudaGetLastError());
@@ -533,9 +506,10 @@ extern "C" int vqb_fsp_stats(const void* z, int dtype, int64_t N, int D, const d
   using namespace vqb;
   if (!z || !norm || !work || !stats || !loss || !aux) return VQB_E_INVALID;
   if (const int rc = fsp_shape(N, D, dtype)) return rc;
-  if (!aligned16(z)) return VQB_E_ALIGN;
+  if (!aligned(z, 16)) return VQB_E_ALIGN;
   if (const int rc = check_device()) return rc;
-  if (blocks != fsp_grid(N)) return VQB_E_INVALID;   // work f64 [4 * blocks + 1][D], sized by vqb_fsp_blocks()
+  // work f64 [4 * blocks + 1][D], sized by vqb_fsp_blocks()
+  if (blocks != capped_grid(N, FSP_THREADS, FSP_CTAS_PER_SM)) return VQB_E_INVALID;
   double* part0 = work;
   double* part1 = work + static_cast<int64_t>(blocks) * D;
   double* colmean = work + static_cast<int64_t>(4 * blocks) * D;
@@ -551,7 +525,7 @@ extern "C" int vqb_fsp_stats(const void* z, int dtype, int64_t N, int D, const d
     fsp_mean_kernel<<<1, 32 * DD, 0, s>>>(N, DD, blocks, part0, colmean);                                \
     fsp_moments_kernel<false, DD, 1><<<blocks, FSP_THREADS, 0, s>>>(z, N, colmean, part1);               \
   }
-  VQB_FSP_SWITCH_D(VQB_FSP_MOM)
+  VQB_SWITCH_D(VQB_FSP_MOM)
 #undef VQB_FSP_MOM
   const NormW nw = norm_weights(norm);
   if (bf) fsp_stats_kernel<true><<<1, 32 * D, 0, s>>>(N, D, blocks, colmean, part1, nw, stats, loss, aux);
@@ -567,10 +541,10 @@ extern "C" int vqb_fsp_backward(const void* z, int dtype, int64_t N, int D, int 
   if (act < ACT_TANH || act > ACT_CAUCHY) return VQB_E_INVALID;
   if (grad_q && grad_dtype != VQB_DTYPE_F32 && grad_dtype != VQB_DTYPE_BF16) return VQB_E_INVALID;
   if (const int rc = fsp_shape(N, D, dtype)) return rc;
-  if (!aligned16(z) || !aligned16(grad_z) || (grad_q && !aligned16(grad_q))) return VQB_E_ALIGN;
+  if (!aligned(z, 16) || !aligned(grad_z, 16) || (grad_q && !aligned(grad_q, 16))) return VQB_E_ALIGN;
   if (const int rc = check_device()) return rc;
   const BwdArgs a{z, grad_q, grad_dtype == VQB_DTYPE_BF16, aux, grad_stats, grad_loss, norm_weights(norm), N, grad_z};
-  const int grid = fsp_grid(N);
+  const int grid = capped_grid(N, FSP_THREADS, FSP_CTAS_PER_SM);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const bool bf = dtype == VQB_DTYPE_BF16;
 #define VQB_FSP_BWD(DD)                                                                                                     \
@@ -591,7 +565,7 @@ extern "C" int vqb_fsp_backward(const void* z, int dtype, int64_t N, int D, int 
                else fsp_backward_kernel<ACT_CAUCHY, false, false, DD><<<grid, FSP_THREADS, 0, s>>>(a); break;               \
     }                                                                                                                       \
   }
-  VQB_FSP_SWITCH_D(VQB_FSP_BWD)
+  VQB_SWITCH_D(VQB_FSP_BWD)
 #undef VQB_FSP_BWD
   return static_cast<int>(cudaGetLastError());
 }
@@ -602,9 +576,9 @@ extern "C" int vqb_fsp_decode(const void* idx, int idx64, int64_t N, int D, int 
   if (!idx || !levels || (!act_out && !codes)) return VQB_E_INVALID;
   if (act < ACT_TANH || act > ACT_CAUCHY) return VQB_E_INVALID;
   if (const int rc = fsp_shape(N, D, VQB_DTYPE_F32)) return rc;
-  if ((act_out && !aligned16(act_out)) || (codes && !aligned16(codes))) return VQB_E_ALIGN;
+  if ((act_out && !aligned(act_out, 16)) || (codes && !aligned(codes, 16))) return VQB_E_ALIGN;
   if (const int rc = check_device()) return rc;
-  const int grid = fsp_grid(N);
+  const int grid = capped_grid(N, FSP_THREADS, FSP_CTAS_PER_SM);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 #define VQB_FSP_DEC_LAUNCH(A, I, DD) fsp_decode_kernel<A, I, DD><<<grid, FSP_THREADS, 0, s>>>(idx, idx64, N, levels, lo, hi, act_out, codes)
 #define VQB_FSP_DEC(DD)                                                                                                     \
@@ -614,7 +588,7 @@ extern "C" int vqb_fsp_decode(const void* idx, int idx64, int64_t N, int D, int 
     case ACT_NORMAL: VQB_FSP_DEC_LAUNCH(ACT_NORMAL, true, DD); break; case ACT_LAPLACE: VQB_FSP_DEC_LAUNCH(ACT_LAPLACE, true, DD); break; \
     default: VQB_FSP_DEC_LAUNCH(ACT_CAUCHY, true, DD); break;                                                               \
   }
-  VQB_FSP_SWITCH_D(VQB_FSP_DEC)
+  VQB_SWITCH_D(VQB_FSP_DEC)
 #undef VQB_FSP_DEC
 #undef VQB_FSP_DEC_LAUNCH
   return static_cast<int>(cudaGetLastError());

@@ -19,24 +19,13 @@ namespace vqb {
 namespace {
 
 constexpr int FSQ_THREADS = 256;
+constexpr int FSQ_CTAS_PER_SM = 16;   // grid cap
 constexpr int FSQ_MAX_D = 16;
 constexpr int FSQ_MAX_Q = 64;
 constexpr int FSQ_BWD_SMEM = 96 * 1024;   // per-thread stage gradients of the backward (see fsq_backward_kernel)
 
 // Rows of the fp32 constant table [FSQ_NCONST][D] (include/vqb200.h).
 enum { C_A = 0, C_B = 1, C_SHIFT = 2, C_HW = 3, C_BASIS = 4, C_RB = 5, C_RHW = 6, FSQ_NCONST = 7 };
-
-template <bool BF> __device__ __forceinline__ float rw(float v) { return BF ? bf16_round(v) : v; }
-
-// a / b, correctly rounded, for a divisor b with rb = RN(1 / b) (Markstein: q0 = RN(a rb) is within an ulp of a / b, the
-// remainder a - b q0 is exact in one fma, and RN(q0 + rem rb) = RN(a / b) while nothing over- or underflows; an infinite or
-// NaN q0 is returned as it is).  Every divisor here is a per-dimension constant whose reciprocal the caller computes with the
-// others, so the kernels carry no call to the division's slow path (whose calling convention would spill).
-__device__ __forceinline__ float divc(float a, float b, float rb) {
-  const float q0 = __fmul_rn(a, rb);
-  if (!isfinite(q0)) return q0;
-  return __fmaf_rn(__fmaf_rn(-b, q0, a), rb, q0);
-}
 
 __device__ __forceinline__ float clamp1(float v) { return v != v ? v : fminf(fmaxf(v, -1.f), 1.f); }   // torch.clamp keeps NaN
 
@@ -116,15 +105,6 @@ __device__ __forceinline__ float stage_elt(float r, float2 sc, bool scaled, bool
   }
   const float cw = rw<BF>(e.code);
   return scaled ? rw<BF>(__fmul_rn(cw, sc.x)) : cw;
-}
-
-__device__ __forceinline__ void store_index(void* idx, int idx64, int64_t off, int64_t v) {
-  if (idx64) reinterpret_cast<int64_t*>(idx)[off] = v;
-  else reinterpret_cast<int32_t*>(idx)[off] = static_cast<int32_t>(v);
-}
-
-__device__ __forceinline__ int64_t load_index(const void* idx, int idx64, int64_t off) {
-  return idx64 ? reinterpret_cast<const int64_t*>(idx)[off] : static_cast<int64_t>(reinterpret_cast<const int32_t*>(idx)[off]);
 }
 
 struct FsqArgs {
@@ -280,36 +260,20 @@ __global__ void __launch_bounds__(FSQ_THREADS, 1) fsq_decode_kernel(FsqArgs a, c
   }
 }
 
-int fsq_grid(int64_t items, int threads) {
-  const int64_t need = (items + threads - 1) / threads;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
-  return static_cast<int>(need < cap ? need : cap);
-}
-
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 int fsq_check(const FsqArgs& a, int D, int in_dtype, int work_dtype) {
   if (!a.z || !a.consts || a.items <= 0 || a.G <= 0 || a.Q <= 0 || a.n_active < 1 || a.n_active > a.Q) return VQB_E_INVALID;
   if (D < 1 || D > FSQ_MAX_D || a.Q > FSQ_MAX_Q || a.items >= (int64_t{1} << 31)) return VQB_E_UNSUPPORTED;
   if ((in_dtype != VQB_DTYPE_F32 && in_dtype != VQB_DTYPE_BF16) || (work_dtype != VQB_DTYPE_F32 && work_dtype != VQB_DTYPE_BF16))
     return VQB_E_INVALID;
   if (in_dtype == VQB_DTYPE_F32 && work_dtype == VQB_DTYPE_BF16) return VQB_E_UNSUPPORTED;   // torch promotes to fp32
-  if (!aligned16(a.z)) return VQB_E_ALIGN;
+  if (!aligned(a.z, 16)) return VQB_E_ALIGN;
   return check_device();
 }
 
-// The launches below cover the (input dtype, W) pairs torch can produce: (f32, f32), (bf16, f32), (bf16, bf16).
-#define VQB_FSQ_SWITCH_D(CALL)                                                                                              \
-  switch (D) {                                                                                                              \
-    case 1: CALL(1); break; case 2: CALL(2); break; case 3: CALL(3); break; case 4: CALL(4); break;                         \
-    case 5: CALL(5); break; case 6: CALL(6); break; case 7: CALL(7); break; case 8: CALL(8); break;                         \
-    case 9: CALL(9); break; case 10: CALL(10); break; case 11: CALL(11); break; case 12: CALL(12); break;                   \
-    case 13: CALL(13); break; case 14: CALL(14); break; case 15: CALL(15); break; case 16: CALL(16); break;                 \
-    default: return VQB_E_UNSUPPORTED;                                                                                      \
-  }
-
 }  // namespace
 }  // namespace vqb
+
+// The launches below cover the (input dtype, W) pairs torch can produce: (f32, f32), (bf16, f32), (bf16, bf16).
 
 extern "C" int vqb_fsq_forward(const void* z, int in_dtype, int work_dtype, int64_t N, int G, int D, int Q, int n_active, int sym,
                                int hard, const float* consts, const float* scales, const float* clampv, void* out, void* idx,
@@ -318,15 +282,15 @@ extern "C" int vqb_fsq_forward(const void* z, int in_dtype, int work_dtype, int6
   const FsqArgs a{z, N * G, G, Q, n_active, sym, hard, consts, scales, clampv};
   if (!out || !idx || N <= 0) return VQB_E_INVALID;
   if (const int rc = fsq_check(a, D, in_dtype, work_dtype)) return rc;
-  if (!aligned16(out)) return VQB_E_ALIGN;
+  if (!aligned(out, 16)) return VQB_E_ALIGN;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int grid = fsq_grid(a.items, FSQ_THREADS);
+  const int grid = capped_grid(a.items, FSQ_THREADS, FSQ_CTAS_PER_SM);
   const bool bf_in = in_dtype == VQB_DTYPE_BF16, bf_w = work_dtype == VQB_DTYPE_BF16;
 #define VQB_FSQ_FWD(DD)                                                                                                         \
   if (!bf_in) fsq_forward_kernel<VQB_DTYPE_F32, false, DD><<<grid, FSQ_THREADS, 0, s>>>(a, out, idx, idx64, idx_s_row, idx_s_g, idx_s_q);  \
   else if (!bf_w) fsq_forward_kernel<VQB_DTYPE_BF16, false, DD><<<grid, FSQ_THREADS, 0, s>>>(a, out, idx, idx64, idx_s_row, idx_s_g, idx_s_q); \
   else fsq_forward_kernel<VQB_DTYPE_BF16, true, DD><<<grid, FSQ_THREADS, 0, s>>>(a, out, idx, idx64, idx_s_row, idx_s_g, idx_s_q);
-  VQB_FSQ_SWITCH_D(VQB_FSQ_FWD)
+  VQB_SWITCH_D(VQB_FSQ_FWD)
 #undef VQB_FSQ_FWD
   return static_cast<int>(cudaGetLastError());
 }
@@ -338,7 +302,7 @@ extern "C" int vqb_fsq_backward(const void* z, int in_dtype, int work_dtype, int
   const FsqArgs a{z, N * G, G, Q, n_active, sym, hard, consts, scales, clampv};
   if (!grad_out || !grad_z || N <= 0) return VQB_E_INVALID;
   if (const int rc = fsq_check(a, D, in_dtype, work_dtype)) return rc;
-  if (!aligned16(grad_out) || !aligned16(grad_z)) return VQB_E_ALIGN;
+  if (!aligned(grad_out, 16) || !aligned(grad_z, 16)) return VQB_E_ALIGN;
   const int per_thread = n_active * D * static_cast<int>(sizeof(float));
   int threads = FSQ_THREADS;
   while (threads > 32 && threads * per_thread > FSQ_BWD_SMEM) threads -= 32;
@@ -346,7 +310,7 @@ extern "C" int vqb_fsq_backward(const void* z, int in_dtype, int work_dtype, int
   const size_t smem = static_cast<size_t>(threads) * per_thread;
   const int r0_lowp = in_dtype == VQB_DTYPE_BF16 && work_dtype == VQB_DTYPE_F32 && !clampv && scales;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int grid = fsq_grid(a.items, threads);
+  const int grid = capped_grid(a.items, threads, FSQ_CTAS_PER_SM);
   const bool bf_in = in_dtype == VQB_DTYPE_BF16, bf_w = work_dtype == VQB_DTYPE_BF16;
 #define VQB_FSQ_BWD_LAUNCH(DT, BF, DD)                                                                                   \
   {                                                                                                                      \
@@ -359,7 +323,7 @@ extern "C" int vqb_fsq_backward(const void* z, int in_dtype, int work_dtype, int
   if (!bf_in) VQB_FSQ_BWD_LAUNCH(VQB_DTYPE_F32, false, DD)               \
   else if (!bf_w) VQB_FSQ_BWD_LAUNCH(VQB_DTYPE_BF16, false, DD)          \
   else VQB_FSQ_BWD_LAUNCH(VQB_DTYPE_BF16, true, DD)
-  VQB_FSQ_SWITCH_D(VQB_FSQ_BWD)
+  VQB_SWITCH_D(VQB_FSQ_BWD)
 #undef VQB_FSQ_BWD
 #undef VQB_FSQ_BWD_LAUNCH
   return static_cast<int>(cudaGetLastError());
@@ -372,16 +336,16 @@ extern "C" int vqb_fsq_decode(const void* idx, int idx64, int64_t idx_s_row, int
   if (!idx || !consts || !levels_basis || (!out && !codes) || N <= 0 || G <= 0 || Q <= 0) return VQB_E_INVALID;
   if (D < 1 || D > FSQ_MAX_D || Q > FSQ_MAX_Q || N * G >= (int64_t{1} << 31)) return VQB_E_UNSUPPORTED;
   if (work_dtype != VQB_DTYPE_F32 && work_dtype != VQB_DTYPE_BF16) return VQB_E_INVALID;
-  if ((out && !aligned16(out)) || (codes && !aligned16(codes))) return VQB_E_ALIGN;
+  if ((out && !aligned(out, 16)) || (codes && !aligned(codes, 16))) return VQB_E_ALIGN;
   if (const int rc = check_device()) return rc;
   const FsqArgs a{nullptr, N * G, G, Q, Q, sym, 0, consts, scales, nullptr};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int grid = fsq_grid(a.items, FSQ_THREADS);
+  const int grid = capped_grid(a.items, FSQ_THREADS, FSQ_CTAS_PER_SM);
   const bool bf_w = work_dtype == VQB_DTYPE_BF16;
 #define VQB_FSQ_DEC(DD)                                                                                                          \
   if (!bf_w) fsq_decode_kernel<false, DD><<<grid, FSQ_THREADS, 0, s>>>(a, levels_basis, idx, idx64, idx_s_row, idx_s_g, idx_s_q, out, codes); \
   else fsq_decode_kernel<true, DD><<<grid, FSQ_THREADS, 0, s>>>(a, levels_basis, idx, idx64, idx_s_row, idx_s_g, idx_s_q, out, codes);
-  VQB_FSQ_SWITCH_D(VQB_FSQ_DEC)
+  VQB_SWITCH_D(VQB_FSQ_DEC)
 #undef VQB_FSQ_DEC
   return static_cast<int>(cudaGetLastError());
 }

@@ -15,11 +15,13 @@
 //                              l2norm, the soft clamp and the residual chain, every stage recomputed from z.
 //   lfq_decode_kernel          indices -> +-m codes and / or their sum over the stages (lfq:228-263, rlfq:101-136).
 #include "vqb_common.cuh"
+#include "row_io.cuh"
 
 namespace vqb {
 namespace {
 
 constexpr int LFQ_THREADS = 256;
+constexpr int LFQ_CTAS_PER_SM = 8;   // grid cap; vqb_lfq_forward_blocks reports the grid, which orders the partial sums
 constexpr int LFQ_MAX_D = 20;
 constexpr int LFQ_MAX_Q = 64;
 constexpr int ENT_THREADS = 256;   // entropy forward: codes across threads
@@ -32,8 +34,6 @@ constexpr float LN2 = 0.6931471805599453f;
 constexpr float LOG2_EPS = -16.609640474436812f;   // log2(1e-5): p >= 1e-5  <=>  log2 p >= LOG2_EPS
 constexpr float LN_EPS = -11.512925464970229f;     // ln(1e-5)
 
-template <bool BF> __device__ __forceinline__ float rw(float v) { return BF ? bf16_round(v) : v; }
-
 __device__ __forceinline__ float ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -42,10 +42,6 @@ __device__ __forceinline__ float ex2(float x) {
 
 // -softplus(y) / ln 2, the log2 of sigmoid(-y)
 __device__ __forceinline__ float neg_softplus2(float y) { return -(fmaxf(y, 0.f) + log1pf(expf(-fabsf(y)))) * LOG2E; }
-
-__device__ __forceinline__ int64_t load_index(const void* idx, int idx64, int64_t off) {
-  return idx64 ? reinterpret_cast<const int64_t*>(idx)[off] : static_cast<int64_t>(reinterpret_cast<const int32_t*>(idx)[off]);
-}
 
 struct StageParams {   // per stage, in shared memory
   float s[LFQ_MAX_Q];    // codebook_scale
@@ -452,12 +448,6 @@ __global__ void __launch_bounds__(LFQ_THREADS) lfq_decode_kernel(const void* __r
   }
 }
 
-int lfq_grid(int64_t items, int threads) {
-  const int64_t need = (items + threads - 1) / threads;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  return static_cast<int>(need < cap ? need : cap > 0 ? cap : 1);
-}
-
 int check_fwd(const FwdArgs& a, int in_dtype, int work_dtype) {
   if (!a.z || !a.params || a.N <= 0 || a.G <= 0 || a.Q <= 0 || a.n_active < 1 || a.n_active > a.Q) return VQB_E_INVALID;
   if (a.D < 1 || a.D > LFQ_MAX_D || a.Q > LFQ_MAX_Q || a.N * a.G >= (int64_t{1} << 31)) return VQB_E_UNSUPPORTED;
@@ -487,7 +477,7 @@ extern "C" int vqb_lfq_forward(const void* z, int dtype, int64_t N, int G, int D
   if (const int rc = check_fwd(a, dtype, dtype)) return rc;
   if (commit && commit_blocks <= 0) return VQB_E_INVALID;
   if (const int rc = check_device()) return rc;
-  const int grid = lfq_grid(N * G, LFQ_THREADS);
+  const int grid = capped_grid(N * G, LFQ_THREADS, LFQ_CTAS_PER_SM);
   if (commit && commit_blocks != grid) return VQB_E_INVALID;   // vqb_lfq_forward_blocks() sizes the partials
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (dtype == VQB_DTYPE_F32)
@@ -500,7 +490,7 @@ extern "C" int vqb_lfq_forward(const void* z, int dtype, int64_t N, int G, int D
 extern "C" int vqb_lfq_forward_blocks(int64_t N, int G) {
   if (N <= 0 || G <= 0) return VQB_E_INVALID;
   if (const int rc = vqb::check_device()) return rc;
-  return vqb::lfq_grid(N * G, vqb::LFQ_THREADS);
+  return vqb::capped_grid(N * G, vqb::LFQ_THREADS, vqb::LFQ_CTAS_PER_SM);
 }
 
 extern "C" int vqb_lfq_entropy(const float* x, int64_t N, int G, int D, int S, const int32_t* rows, int64_t R, int64_t rows_stride,
@@ -554,7 +544,7 @@ extern "C" int vqb_lfq_backward(const void* z, int dtype, int64_t N, int G, int 
   if (!grad_out || !grad_z) return VQB_E_INVALID;
   if (const int rc = check_fwd(a, dtype, dtype)) return rc;
   if (const int rc = check_device()) return rc;
-  const int grid = lfq_grid(N * G, LFQ_THREADS);
+  const int grid = capped_grid(N * G, LFQ_THREADS, LFQ_CTAS_PER_SM);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (dtype == VQB_DTYPE_F32)
     lfq_backward_kernel<VQB_DTYPE_F32, false><<<grid, LFQ_THREADS, 0, s>>>(a, grad_out, grad_ent, cc, rowmask, grad_z);
@@ -569,7 +559,7 @@ extern "C" int vqb_lfq_decode(const void* idx, int idx64, int64_t idx_s_row, int
   if (!idx || !vals || (!out && !codes) || N <= 0 || G <= 0 || Q <= 0) return VQB_E_INVALID;
   if (D < 1 || D > LFQ_MAX_D || Q > LFQ_MAX_Q || N * G >= (int64_t{1} << 31)) return VQB_E_UNSUPPORTED;
   if (const int rc = check_device()) return rc;
-  const int grid = lfq_grid(N * G, LFQ_THREADS);
+  const int grid = capped_grid(N * G, LFQ_THREADS, LFQ_CTAS_PER_SM);
   lfq_decode_kernel<<<grid, LFQ_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(idx, idx64, idx_s_row, idx_s_g, idx_s_q, N, G, D, Q,
                                                                                  vals, out, codes);
   return static_cast<int>(cudaGetLastError());

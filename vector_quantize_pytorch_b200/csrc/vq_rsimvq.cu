@@ -168,14 +168,6 @@ __global__ void __launch_bounds__(RS_THREADS, 1) rsimvq_backward_kernel(const fl
   }
 }
 
-int rs_grid(int64_t rows) {
-  const int wpb = RS_THREADS / 32;
-  int64_t g = (rows + wpb - 1) / wpb;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
-  if (g > cap) g = cap;
-  return static_cast<int>(g < 1 ? 1 : g);
-}
-
 // registers per lane: the smallest power of two J with 32 J >= D
 int rs_slots(int D) {
   int J = 1;
@@ -198,7 +190,7 @@ extern "C" int vqb_rsimvq_tail(const float* r, const float* codes, const int32_t
     if (e != cudaSuccess) return static_cast<int>(e);
   }
   double* ls = loss_out ? loss_sum : nullptr;
-  const int g = rs_grid(N);
+  const int g = capped_grid(N, RS_THREADS / 32, 16);
   switch (rs_slots(D)) {
 #define VQB_RS_TAIL(JJ) \
   case JJ: rsimvq_tail_kernel<JJ><<<g, RS_THREADS, 0, s>>>(r, codes, idx, N, D, rotation, r_next, qsum, first, idx64_out, idx_stride, ls); break;
@@ -217,7 +209,7 @@ extern "C" int vqb_rsimvq_backward(const float* x, const float* codes, int Q, in
   if (D > 1024) return VQB_E_UNSUPPORTED;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int64_t stride = static_cast<int64_t>(K) * D;
-  const int g = rs_grid(N);
+  const int g = capped_grid(N, RS_THREADS / 32, 16);
   switch (rs_slots(D)) {
 #define VQB_RS_BWD(JJ) \
   case JJ: rsimvq_backward_kernel<JJ><<<g, RS_THREADS, 0, s>>>(x, codes, stride, Q, n_active, idx, N, D, rotation, grad_q, grad_loss, grad_x); break;

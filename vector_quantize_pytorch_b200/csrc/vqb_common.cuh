@@ -40,6 +40,14 @@ inline int num_sms() {
   device_props(&sms, &major);
   return sms;
 }
+// CTAs of a grid-stride loop over `items` at `per_cta` items per CTA: enough to cover them, at most `ctas_per_sm` per SM, at
+// least one.
+inline int capped_grid(int64_t items, int64_t per_cta, int ctas_per_sm) {
+  const int64_t need = (items + per_cta - 1) / per_cta;
+  const int64_t cap = static_cast<int64_t>(num_sms()) * ctas_per_sm;
+  const int64_t g = need < cap ? need : cap;
+  return static_cast<int>(g > 1 ? g : 1);
+}
 
 __device__ __forceinline__ float bf16_bits_to_float(uint16_t b) { return __uint_as_float(static_cast<uint32_t>(b) << 16); }
 // round-to-nearest-even float -> bf16 bits (finite inputs)

@@ -17,7 +17,6 @@ from torch import nn
 from . import ops
 from .codebook import _unsupported
 
-_FLOAT = (torch.float32, torch.bfloat16)
 _ACTS = {"tanh": 0, "sigmoid": 1, "normal": 2, "laplace": 3, "cauchy": 4}
 _MAX_D = 16
 
@@ -35,13 +34,6 @@ _PRESETS = {   # fsp:144-193
 def _cast(v: float, dtype: torch.dtype) -> float:
     """A Python scalar as torch casts it to `dtype` for a comparison or a clamp."""
     return torch.tensor(v, dtype=torch.float64).to(dtype).item()
-
-
-def _check_input(z: torch.Tensor):
-    if z.dtype not in _FLOAT:
-        raise TypeError(f"vqb200 FSP supports float32 and bfloat16 inputs, got {z.dtype}")
-    if not z.is_cuda:
-        raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
 
 
 def _rand(z: torch.Tensor) -> torch.Tensor:
@@ -78,8 +70,7 @@ class _FSPFunction(torch.autograd.Function):
 
 def fsp_stats_apply(z: torch.Tensor, norm):
     """VectorNorm on z (N, d): (norm_loss, stats (4, d)), differentiable w.r.t. z."""
-    _check_input(z)
-    z = ops._aligned(z)
+    z = ops.float_input(z, "FSP")
     _, loss, stats, *_ = _FSPFunction.apply(z, None, None, None, 0, False, norm, 0., 0., 0., 0., False)
     return loss, stats
 
@@ -192,8 +183,7 @@ class FSP(nn.Module):
         assert z_shape[-1] == self.dim, f"expected dimension of {self.dim} but found dimension of {z_shape[-1]}"
         z = z.reshape(-1, self.dim)
         z = self.project_in(z)
-        _check_input(z)
-        z = ops._aligned(z)
+        z = ops.float_input(z, "FSP")
         quantize_rate = self.quantize_rate if self.training else 1.0
         perturb = quantize_rate < 1.0
         u1 = u2 = None

@@ -14,9 +14,6 @@ from torch import nn
 from . import ops
 from .codebook import _unsupported
 
-_FLOAT = (torch.float32, torch.bfloat16)
-
-
 def fsq_tables(levels: torch.Tensor, basis: torch.Tensor, sym: bool, hard: bool):
     """The fp32 constant table (7, d) and the int32 (levels, basis) table (2, d) of vqb_fsq_* (include/vqb200.h), from the FSQ
     buffers `_levels` / `_basis` on the CPU, with the expressions of fsq:152-156, :165-166, :197-207."""
@@ -37,22 +34,6 @@ def fsq_tables(levels: torch.Tensor, basis: torch.Tensor, sym: bool, hard: bool)
     consts = torch.stack([a, b, shift, hw, basis.float(), rb, 1 / hw]).float().contiguous()
     ints = torch.stack([levels.int(), basis.int()]).contiguous()
     return consts, ints
-
-
-class _DeviceTables:
-    """Per-device copies of a module's kernel tables, made on first use by `make()` (the tables follow from non-persistent
-    buffers fixed at construction; `key` names what may still change them, such as the buffers' dtype after `.to(dtype)`)."""
-
-    def __init__(self, make):
-        self.make = make
-        self.cache = {}
-
-    def get(self, device, key=()):
-        k = (device, key)
-        t = self.cache.get(k)
-        if t is None:
-            t = self.cache[k] = tuple(x.to(device) if x is not None else None for x in self.make())
-        return t
 
 
 class _FSQFunction(torch.autograd.Function):
@@ -77,13 +58,7 @@ class _FSQFunction(torch.autograd.Function):
 def fsq_apply(z, work_dtype, Q, n_active, sym, hard, consts, scales, clampv, indices):
     """Runs the kernel pair on z (N, G, d) (made contiguous), indices written through their (N, G, Q) view `indices`;
     differentiable w.r.t. z."""
-    if z.dtype not in _FLOAT or work_dtype not in _FLOAT:
-        raise TypeError(f"vqb200 FSQ supports float32 and bfloat16 inputs, got {z.dtype} (quantizer chain in {work_dtype})")
-    if not z.is_cuda:
-        raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
-    z = z.contiguous()
-    if z.data_ptr() % 16:
-        z = z.clone()
+    z = ops.float_input(z, "FSQ", work_dtype=work_dtype)
     return _FSQFunction.apply(z, work_dtype, Q, n_active, sym, hard, consts, scales, clampv, indices)
 
 
@@ -139,7 +114,7 @@ class FSQ(nn.Module):
         self.force_quantization_f32 = force_quantization_f32
         self.bound_hard_clamp = bound_hard_clamp
         self.orthogonal_rotation = orthogonal_rotation
-        self._tables = _DeviceTables(self._make_tables)
+        self._tables = ops.DeviceTables(self._make_tables)
 
     def _make_tables(self):
         return fsq_tables(self._levels, self._basis, self.preserve_symmetry, self.bound_hard_clamp)

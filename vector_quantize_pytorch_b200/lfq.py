@@ -26,7 +26,6 @@ from .codebook import _unsupported
 Return = namedtuple('Return', ['quantized', 'indices', 'entropy_aux_loss'])
 LossBreakdown = namedtuple('LossBreakdown', ['per_sample_entropy', 'batch_entropy', 'commitment'])
 
-_FLOAT = (torch.float32, torch.bfloat16)
 MAX_CODEBOOK_DIM = 20
 
 
@@ -117,13 +116,9 @@ class _LFQEntropy(torch.autograd.Function):
 
 
 def lfq_chain(z, Q, n_active, residual, training, spherical, params, indices, want_ent, rowmask, want_commit):
-    """Runs the row chain on z (N, G, d) (made contiguous); differentiable w.r.t. z."""
-    if z.dtype not in _FLOAT:
-        raise TypeError(f"vqb200 LFQ supports float32 and bfloat16 inputs, got {z.dtype}")
-    if not z.is_cuda:
-        raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
-    return _LFQChain.apply(z.contiguous(), Q, n_active, residual, training, spherical, params, indices, want_ent, rowmask,
-                           want_commit)
+    """Runs the row chain on z (N, G, d) (made contiguous and aligned); differentiable w.r.t. z."""
+    z = ops.float_input(z, "LFQ")
+    return _LFQChain.apply(z, Q, n_active, residual, training, spherical, params, indices, want_ent, rowmask, want_commit)
 
 
 def sample_rows(num_tokens: int, frac: float):
@@ -243,7 +238,7 @@ class LFQ(nn.Module):
         bits = ((all_codes[..., None].int() & self.mask) != 0).float()
         self.register_buffer('codebook', self.bits_to_codes(bits).float(), persistent=False)
         self._magnitude = code_magnitude(codebook_scale, codebook_dim, spherical)
-        self._params = {}
+        self._params = ops.DeviceTables(self._make_params)
 
     def bits_to_codes(self, bits):
         return bits * self.codebook_scale * 2 - self.codebook_scale
@@ -255,21 +250,17 @@ class LFQ(nn.Module):
     def maybe_l2norm(self, t):
         return F.normalize(t, dim=-1) * self.codebook_scale if self.spherical else t
 
-    def _stage_params(self, device, in_kernel_clamp):
-        """(3, 1) fp32: scale, code magnitude, soft-clamp value (0 when the clamp runs in torch or is off)."""
-        key = (device, in_kernel_clamp)
-        p = self._params.get(key)
-        if p is None:
-            c = self.soft_clamp_input_value if (in_kernel_clamp and self.soft_clamp_input_value is not None) else 0.
-            p = self._params[key] = torch.tensor([[self.codebook_scale], [self._magnitude], [c]], dtype=torch.float32,
-                                                 device=device)
-        return p
+    def _make_params(self):
+        """(3, 1) fp32: scale, code magnitude, soft-clamp value (0 when it is off, or runs in torch before the rotation)."""
+        in_kernel_clamp = self.soft_clamp_input_value is not None and not self.orthogonal_rotation
+        c = self.soft_clamp_input_value if in_kernel_clamp else 0.
+        return (torch.tensor([[self.codebook_scale], [self._magnitude], [c]], dtype=torch.float32),)
 
     def _decode(self, indices):
         """vqb_lfq_decode of (..., c) indices -> fp32 codes (..., c, d), +-magnitude."""
         idx = indices.contiguous()
         lead = idx.shape
-        vals = self._stage_params(idx.device, True)[1]
+        vals = self._params.get(idx.device)[0][1]
         _, codes = ops.lfq_decode(idx.view(-1, 1, 1), self.codebook_dim, vals, False, True)
         return codes.reshape(*lead, self.codebook_dim)
 
@@ -313,7 +304,7 @@ class LFQ(nn.Module):
         flat_mask = mask.reshape(N) if mask is not None else None
         want_commit = train and self.commitment_loss_weight > 0.
         rowmask = flat_mask.to(torch.uint8) if (want_commit and flat_mask is not None) else None
-        params = self._stage_params(z.device, not rot)
+        params, = self._params.get(z.device)
         out, ent, commit = lfq_chain(z, 1, 1, False, train, self.spherical, params, indices.view(N, c, 1), train, rowmask,
                                      want_commit)
         if train:

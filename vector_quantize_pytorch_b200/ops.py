@@ -55,6 +55,66 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+def _sms(dev) -> int:
+    return torch.cuda.get_device_properties(dev).multi_processor_count
+
+
+def _aligned(t: torch.Tensor) -> torch.Tensor:
+    t = t.contiguous()
+    return t.clone() if t.data_ptr() % 16 else t   # a contiguous view at an offset (the kernels move rows in 16-byte vectors)
+
+
+def _queried(n: int, name: str) -> int:
+    """A count returned by a query entry point, which returns a negative error code instead when it fails."""
+    check(min(n, 0), name)
+    return n
+
+
+def _index_strides(idx: torch.Tensor) -> tuple:
+    """(row, group, stage) element strides of an (N, G, Q) view of an index tensor (a size-1 axis has stride 0)."""
+    return tuple(0 if n == 1 else s for n, s in zip(idx.shape, idx.stride()))
+
+
+_fsq_strides = _index_strides   # the name FSQ's kernel tests import
+
+
+def _check_index_dtype(indices: torch.Tensor, family: str):
+    if indices.dtype not in (torch.int32, torch.int64):
+        raise TypeError(f"{family} indices must be int32 or int64, got {indices.dtype}")
+
+
+# ---- what the scalar quantizer modules (FSQ, LFQ, FSP, BinaryMapper) share ----
+
+FLOAT_DTYPES = (torch.float32, torch.bfloat16)
+
+
+def float_input(t: torch.Tensor, family: str, what: str = "inputs", work_dtype: torch.dtype | None = None) -> torch.Tensor:
+    """A module's input to the row kernels: fp32 or bf16 (TypeError; so must `work_dtype` be, the dtype of the module's chain
+    when it differs from the input's) on a CUDA device (RuntimeError), returned contiguous and 16-byte aligned."""
+    if t.dtype not in FLOAT_DTYPES or (work_dtype is not None and work_dtype not in FLOAT_DTYPES):
+        chain = f" (quantizer chain in {work_dtype})" if work_dtype is not None else ""
+        raise TypeError(f"vqb200 {family} supports float32 and bfloat16 {what}, got {t.dtype}{chain}")
+    if not t.is_cuda:
+        raise RuntimeError(f"vqb200 has no CPU path: {what} must live on a CUDA (H100, sm_90) device")
+    return _aligned(t)
+
+
+class DeviceTables:
+    """Per-device copies of a module's kernel tables, made on first use by `make()` (the tables follow from non-persistent
+    buffers fixed at construction; `key` names what may still change them, such as the buffers' dtype after `.to(dtype)`)."""
+
+    def __init__(self, make):
+        self.make = make
+        self.cache = {}
+
+    def get(self, device, key=()):
+        k = (device, key)
+        t = self.cache.get(k)
+        if t is None:
+            t = self.cache[k] = tuple(x.to(device) if x is not None else None for x in self.make())
+        return t
+
+
 def padded_codes(K: int) -> int:
     return lib.vqb_padded_codes(K)
 
@@ -549,11 +609,6 @@ def diveq(x: torch.Tensor, q: torch.Tensor, noise: torch.Tensor, noise_scale: fl
     return out.reshape(shape), dq.reshape(shape)
 
 
-def _fsq_strides(idx: torch.Tensor) -> tuple:
-    """(row, group, stage) element strides of an (N, G, Q) view of an index tensor (a size-1 axis has stride 0)."""
-    return tuple(0 if n == 1 else s for n, s in zip(idx.shape, idx.stride()))
-
-
 def fsq_forward(z: torch.Tensor, work_dtype: torch.dtype, Q: int, n_active: int, sym: bool, hard: bool, consts: torch.Tensor,
                 scales: torch.Tensor | None, clampv: torch.Tensor | None, indices: torch.Tensor) -> torch.Tensor:
     """vqb_fsq_forward: z (N, G, D) contiguous in fp32 / bf16 -> out (N, G, D) in `work_dtype`; writes the indices into
@@ -562,7 +617,7 @@ def fsq_forward(z: torch.Tensor, work_dtype: torch.dtype, Q: int, n_active: int,
     _require_cuda(z, consts, scales, clampv, indices)
     N, G, D = z.shape
     out = torch.empty(z.shape, dtype=work_dtype, device=z.device)
-    s_row, s_g, s_q = _fsq_strides(indices)
+    s_row, s_g, s_q = _index_strides(indices)
     with torch.cuda.device(z.device):
         check(lib.vqb_fsq_forward(_p(z), _dtype_code(z), _DT[work_dtype], N, G, D, Q, n_active, int(sym), int(hard), _p(consts),
                                   _p(scales), _p(clampv), _p(out), _p(indices), int(indices.dtype == torch.int64), s_row, s_g, s_q,
@@ -577,9 +632,7 @@ def fsq_backward(z: torch.Tensor, grad_out: torch.Tensor, Q: int, n_active: int,
     _require_cuda(z, grad_out, consts, scales, clampv)
     N, G, D = z.shape
     gz = torch.empty_like(z)
-    g = grad_out.contiguous()
-    if g.data_ptr() % 16:   # a contiguous view at an offset (the kernel moves rows in 16-byte vectors)
-        g = g.clone()
+    g = _aligned(grad_out)
     with torch.cuda.device(z.device):
         check(lib.vqb_fsq_backward(_p(z), _dtype_code(z), _dtype_code(g), N, G, D, Q, n_active, int(sym), int(hard), _p(consts),
                                    _p(scales), _p(clampv), _p(g), _p(gz), _stream()), "vqb_fsq_backward")
@@ -592,13 +645,12 @@ def fsq_decode(indices: torch.Tensor, D: int, work_dtype: torch.dtype, sym: bool
     """vqb_fsq_decode: indices, an (N, G, Q) view (any strides) -> (sum over the stages (N, G, D) or None, stage codes
     (Q, N, G, D) or None) in `work_dtype`."""
     _require_cuda(indices, consts, levels_basis, scales)
-    if indices.dtype not in (torch.int32, torch.int64):
-        raise TypeError(f"FSQ indices must be int32 or int64, got {indices.dtype}")
+    _check_index_dtype(indices, "FSQ")
     N, G, Q = indices.shape
     dev = indices.device
     out = torch.empty((N, G, D), dtype=work_dtype, device=dev) if want_sum else None
     codes = torch.empty((Q, N, G, D), dtype=work_dtype, device=dev) if want_codes else None
-    s_row, s_g, s_q = _fsq_strides(indices)
+    s_row, s_g, s_q = _index_strides(indices)
     with torch.cuda.device(dev):
         check(lib.vqb_fsq_decode(_p(indices), int(indices.dtype == torch.int64), s_row, s_g, s_q, N, G, D, Q, _DT[work_dtype], int(sym),
                                  _p(consts), _p(levels_basis), _p(scales), _p(out), _p(codes), _stream()), "vqb_fsq_decode")
@@ -607,10 +659,6 @@ def fsq_decode(indices: torch.Tensor, D: int, work_dtype: torch.dtype, sym: bool
 
 
 # ---- lookup-free quantization (csrc/vq_lfq.cu) ----
-
-def _sms(dev) -> int:
-    return torch.cuda.get_device_properties(dev).multi_processor_count
-
 
 def lfq_forward(z: torch.Tensor, Q: int, n_active: int, residual: bool, training: bool, spherical: bool, params: torch.Tensor,
                 indices: torch.Tensor, want_entropy: bool, rowmask: torch.Tensor | None, want_commit: bool):
@@ -624,10 +672,9 @@ def lfq_forward(z: torch.Tensor, Q: int, n_active: int, residual: bool, training
     dev = z.device
     out = torch.empty(z.shape, dtype=z.dtype, device=dev)
     ent = torch.empty((n_active, N, G, D), dtype=torch.float32, device=dev) if want_entropy else None
-    s_row, s_g, s_q = _fsq_strides(indices)
+    s_row, s_g, s_q = _index_strides(indices)
     with torch.cuda.device(dev):
-        blocks = lib.vqb_lfq_forward_blocks(N, G)
-        check(min(blocks, 0), "vqb_lfq_forward_blocks")
+        blocks = _queried(lib.vqb_lfq_forward_blocks(N, G), "vqb_lfq_forward_blocks")
         commit = torch.empty((n_active, blocks), dtype=torch.float64, device=dev) if want_commit else None
         check(lib.vqb_lfq_forward(_p(z), _dtype_code(z), N, G, D, Q, n_active, int(residual), int(training), int(spherical), _p(params),
                                   _p(out), _p(indices), s_row, s_g, s_q, _p(ent), _p(rowmask), _p(commit), blocks, _stream()),
@@ -658,8 +705,7 @@ def lfq_entropy(x: torch.Tensor, rows: torch.Tensor | None, R: int, m: torch.Ten
     _require_cuda(x, rows, m)
     S, N, G, D = x.shape
     SG, K, dev = S * G, 1 << D, x.device
-    tiles = lib.vqb_lfq_entropy_tiles(D)
-    check(min(tiles, 0), "vqb_lfq_entropy_tiles")
+    tiles = _queried(lib.vqb_lfq_entropy_tiles(D), "vqb_lfq_entropy_tiles")
     chunks = -(-4 * _sms(dev) // (tiles * SG))
     chunks = max(1, min(chunks, -(-R // 32), 65535))
     if want_colsum:
@@ -700,13 +746,12 @@ def lfq_decode(indices: torch.Tensor, D: int, vals: torch.Tensor, want_sum: bool
     """vqb_lfq_decode: indices, an (N, G, Q) view (any strides, int32 / int64, -1 = dropped) -> (sum over the stages (N, G, D) or
     None, codes (Q, N, G, D) or None), fp32."""
     _require_cuda(indices, vals)
-    if indices.dtype not in (torch.int32, torch.int64):
-        raise TypeError(f"LFQ indices must be int32 or int64, got {indices.dtype}")
+    _check_index_dtype(indices, "LFQ")
     N, G, Q = indices.shape
     dev = indices.device
     out = torch.empty((N, G, D), dtype=torch.float32, device=dev) if want_sum else None
     codes = torch.empty((Q, N, G, D), dtype=torch.float32, device=dev) if want_codes else None
-    s_row, s_g, s_q = _fsq_strides(indices)
+    s_row, s_g, s_q = _index_strides(indices)
     with torch.cuda.device(dev):
         check(lib.vqb_lfq_decode(_p(indices), int(indices.dtype == torch.int64), s_row, s_g, s_q, N, G, D, Q, _p(vals), _p(out),
                                  _p(codes), _stream()), "vqb_lfq_decode")
@@ -715,17 +760,6 @@ def lfq_decode(indices: torch.Tensor, D: int, vals: torch.Tensor, want_sum: bool
 
 
 # ---- finite scalar perturbation (csrc/vq_fsp.cu) ----
-
-def _fsp_blocks(N: int) -> int:
-    blocks = lib.vqb_fsp_blocks(N)
-    check(min(blocks, 0), "vqb_fsp_blocks")
-    return blocks
-
-
-def _aligned(t: torch.Tensor) -> torch.Tensor:
-    t = t.contiguous()
-    return t.clone() if t.data_ptr() % 16 else t   # a contiguous view at an offset (the kernels move rows in 16-byte vectors)
-
 
 def fsp_forward(z: torch.Tensor, act: int, inv: bool, levels: torch.Tensor, clamp_hi: float, u1: torch.Tensor | None,
                 u2: torch.Tensor | None, qrate: float, inv_lo: float, inv_hi: float):
@@ -739,7 +773,7 @@ def fsp_forward(z: torch.Tensor, act: int, inv: bool, levels: torch.Tensor, clam
     idx = torch.empty((N,), dtype=torch.int32, device=dev)
     lev = torch.empty((N, D), dtype=z.dtype, device=dev)
     with torch.cuda.device(dev):
-        blocks = _fsp_blocks(N)
+        blocks = _queried(lib.vqb_fsp_blocks(N), "vqb_fsp_blocks")
         acc = torch.empty((blocks,), dtype=torch.int32, device=dev) if u1 is not None else None
         check(lib.vqb_fsp_forward(_p(z), _dtype_code(z), N, D, act, int(inv), _p(levels), clamp_hi, _p(u1), _p(u2), qrate, inv_lo,
                                   inv_hi, _p(out), _p(idx), _p(lev), _p(acc), blocks, _stream()), "vqb_fsp_forward")
@@ -761,7 +795,7 @@ def fsp_stats(z: torch.Tensor, norm):
     loss = torch.empty((), dtype=z.dtype, device=dev)
     aux = torch.empty((D, 8), dtype=torch.float64, device=dev)
     with torch.cuda.device(dev):
-        blocks = _fsp_blocks(N)
+        blocks = _queried(lib.vqb_fsp_blocks(N), "vqb_fsp_blocks")
         work = torch.empty((4 * blocks + 1, D), dtype=torch.float64, device=dev)
         check(lib.vqb_fsp_stats(_p(z), _dtype_code(z), N, D, _norm_arg(norm), _p(work), blocks, _p(stats), _p(loss), _p(aux),
                                 _stream()), "vqb_fsp_stats")
@@ -790,8 +824,7 @@ def fsp_decode(indices: torch.Tensor, D: int, act: int, inv: bool, levels: torch
                want_codes: bool):
     """vqb_fsp_decode: indices (any shape, int32 / int64) -> (act values, codes), each (*indices.shape, D) fp32 or None."""
     _require_cuda(indices, levels)
-    if indices.dtype not in (torch.int32, torch.int64):
-        raise TypeError(f"FSP indices must be int32 or int64, got {indices.dtype}")
+    _check_index_dtype(indices, "FSP")
     idx = indices.contiguous()
     N = idx.numel()
     dev = idx.device
@@ -842,7 +875,7 @@ def binmap_backward(logits: torch.Tensor, g: torch.Tensor, ksplit: int | None = 
         g = g.float()
     with torch.cuda.device(logits.device):
         if ksplit is None:
-            ksplit = binmap_backward_plan(rows, bits, torch.cuda.get_device_properties(logits.device).multi_processor_count)[0]
+            ksplit = binmap_backward_plan(rows, bits, _sms(logits.device))[0]
         work = torch.empty((rows, ksplit, 2 * bits), dtype=torch.float64, device=logits.device) if ksplit > 1 else None
         check(lib.vqb_binmap_backward(_p(logits), rows, bits, _p(g), g.stride(0), g.stride(1), ksplit, _p(work), _p(dl),
                                       _stream()), "vqb_binmap_backward")

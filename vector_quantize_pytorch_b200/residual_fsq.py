@@ -11,23 +11,12 @@ fp32); a module moved to bf16 runs the outer chain in bf16, rounding after every
 """
 from __future__ import annotations
 
-import random
-from math import ceil
-
 import torch
-import torch.distributed as distributed
 from torch import nn
 
 from . import ops
-from .fsq import FSQ, _DeviceTables, fsq_apply
-
-
-def get_maybe_sync_seed(device, max_size=10_000):
-    """rfsq:39-45: one torch.randint on the device, all-reduced when distributed, then .item()."""
-    rand_int = torch.randint(0, max_size, (), device=device)
-    if distributed.is_available() and distributed.is_initialized() and distributed.get_world_size() > 1:
-        distributed.all_reduce(rand_int)
-    return rand_int.item()
+from .fsq import FSQ, fsq_apply
+from .residual_common import GroupedResidual, dropout_cut, get_maybe_sync_seed, pad_dropped
 
 
 def _work_dtype(z_dtype, clampv, scales):
@@ -76,7 +65,7 @@ class ResidualFSQ(nn.Module):
         if isinstance(soft_clamp_input_value, (list, float)):
             soft_clamp_input_value = torch.tensor(soft_clamp_input_value)
         self.register_buffer('soft_clamp_input_value', soft_clamp_input_value, persistent=False)
-        self._scale_tables = _DeviceTables(self._make_scale_tables)
+        self._scale_tables = ops.DeviceTables(self._make_scale_tables)
 
     def _make_scale_tables(self):
         """(2, Q, d) stage scales and their reciprocals, (2, d) soft-clamp value and reciprocal (None without a soft clamp): the
@@ -103,16 +92,9 @@ class ResidualFSQ(nn.Module):
 
     def _n_active(self, seed, device):
         """Leading stages that quantize (rfsq:204-223): all, or with quantize dropout in training the sampled cut."""
-        Q = self.num_quantizers
         if not (self.training and self.quantize_dropout and torch.is_grad_enabled()):
-            return Q, False
-        if seed is None:
-            seed = get_maybe_sync_seed(device)
-        index = random.Random(seed).randrange(self.quantize_dropout_cutoff_index, Q)
-        mult = self.quantize_dropout_multiple_of
-        if mult != 1:
-            index = ceil((index + 1) / mult) * mult - 1
-        return min(index + 1, Q), True
+            return self.num_quantizers, False
+        return dropout_cut(self, seed, device), True
 
     def _pre(self, x):
         """Channel-first packing and project_in (rfsq:183-189): -> rows (N, d), and what _post needs to restore the layout."""
@@ -169,24 +151,23 @@ class ResidualFSQ(nn.Module):
         return (*ret, self.get_codes_from_indices(all_indices))
 
     def _decode(self, indices, want_sum, want_codes):
-        """vqb_fsq_decode of 'b ... q' indices (rfsq:131-171): -> (sum (b, ..., d) or None, codes (Q, b, ..., d) or None)."""
-        quantize_dim = indices.shape[-1]
+        """'b ... q' indices (rfsq:131-171, rlfq:101-136) through `_decode_rows`: -> (sum (b, ..., d) or None, codes
+        (Q, b, ..., d) or None)."""
         Q = self.num_quantizers
-        if quantize_dim < Q:
-            assert self.quantize_dropout > 0., \
-                'quantize dropout must be greater than 0 if you wish to reconstruct from a signal with less fine quantizations'
+        indices = pad_dropped(indices, Q, self.quantize_dropout,
+                              'quantize dropout must be greater than 0 if you wish to reconstruct from a signal with less fine '
+                              'quantizations')
         lead = indices.shape[:-1]
-        flat = indices.reshape(-1, quantize_dim)
-        if quantize_dim < Q:
-            flat = torch.nn.functional.pad(flat, (0, Q - quantize_dim), value=-1)
-        flat = flat.contiguous()
-        N = flat.shape[0]
-        d = len(self.levels)
-        consts, ints, scales, _ = self._tables(flat.device)
-        s, codes = ops.fsq_decode(flat.view(N, 1, Q), d, self._codes_dtype(), True, consts, ints, scales, want_sum, want_codes)
-        s = s.reshape(*lead, d) if s is not None else None
-        codes = codes.reshape(Q, *lead, d) if codes is not None else None
+        flat = indices.reshape(-1, indices.shape[-1]).contiguous()
+        s, codes = self._decode_rows(flat.view(flat.shape[0], 1, Q), want_sum, want_codes)
+        s = s.reshape(*lead, s.shape[-1]) if s is not None else None
+        codes = codes.reshape(Q, *lead, codes.shape[-1]) if codes is not None else None
         return s, codes
+
+    def _decode_rows(self, idx, want_sum, want_codes):
+        """vqb_fsq_decode of (N, 1, Q) indices."""
+        consts, ints, scales, _ = self._tables(idx.device)
+        return ops.fsq_decode(idx, len(self.levels), self._codes_dtype(), True, consts, ints, scales, want_sum, want_codes)
 
     def get_codes_from_indices(self, indices):
         return self._decode(indices, False, True)[1]
@@ -195,38 +176,14 @@ class ResidualFSQ(nn.Module):
         return self.project_out(self._decode(indices, True, False)[0])
 
 
-class GroupedResidualFSQ(nn.Module):
+class GroupedResidualFSQ(GroupedResidual):
     """Drop-in for the reference's GroupedResidualFSQ (rfsq:277-350): `groups` ResidualFSQs over column blocks of the features.
     The forward is ONE vqb_fsq_forward launch for all groups (and one backward launch); the indices come out as
     torch.stack of the groups' (G, b, ..., Q)."""
 
     def __init__(self, *, dim, groups=1, accept_image_fmap=False, **kwargs):
-        super().__init__()
-        self.dim = dim
-        self.groups = groups
-        assert (dim % groups) == 0
-        dim_per_group = dim // groups
-        self.accept_image_fmap = accept_image_fmap
-        self.rvqs = nn.ModuleList([])
-        for _ in range(groups):
-            self.rvqs.append(ResidualFSQ(dim=dim_per_group, **kwargs))
+        super().__init__(ResidualFSQ, dim=dim, groups=groups, accept_image_fmap=accept_image_fmap, **kwargs)
         self.codebook_size = self.rvqs[0].codebook_size
-
-    @property
-    def codebooks(self):
-        return torch.stack(tuple(rvq.codebooks for rvq in self.rvqs))
-
-    @property
-    def split_dim(self):
-        return 1 if self.accept_image_fmap else -1
-
-    def get_codes_from_indices(self, indices):
-        codes = tuple(rvq.get_codes_from_indices(chunk_indices) for rvq, chunk_indices in zip(self.rvqs, indices))
-        return torch.stack(codes)
-
-    def get_output_from_indices(self, indices):
-        outputs = tuple(rvq.get_output_from_indices(chunk_indices) for rvq, chunk_indices in zip(self.rvqs, indices))
-        return torch.cat(outputs, dim=self.split_dim)
 
     def forward(self, x, return_all_codes=False):
         shape, split_dim, device = x.shape, self.split_dim, x.device

@@ -14,7 +14,8 @@ from torch import nn
 from . import ops
 from .lfq import LFQ, entropy_losses, lfq_chain
 from .codebook import _unsupported
-from .residual_fsq import get_maybe_sync_seed, ResidualFSQ
+from .residual_common import GroupedResidual, get_maybe_sync_seed
+from .residual_fsq import ResidualFSQ
 import torch.nn.functional as F
 
 MAX_QUANTIZERS = 64   # the stages the row kernels hold (vqb_lfq_forward)
@@ -49,23 +50,23 @@ class ResidualLFQ(nn.Module):
         self.quantize_dropout_cutoff_index = quantize_dropout_cutoff_index
         self.quantize_dropout_multiple_of = quantize_dropout_multiple_of
         self.codebook_dim = codebook_dim
-        self._params = {}
+        self._params = ops.DeviceTables(self._make_params)
 
     _n_active = ResidualFSQ._n_active
+    _decode = ResidualFSQ._decode
+    get_codes_from_indices = ResidualFSQ.get_codes_from_indices
+    get_output_from_indices = ResidualFSQ.get_output_from_indices
 
     @property
     def codebooks(self):
         return torch.stack([layer.codebook for layer in self.layers], dim=0)
 
-    def _stage_params(self, device):
+    def _make_params(self):
         """(3, Q) fp32: per layer scale, code magnitude, soft-clamp value (0: none); and (Q,) the non-spherical code values."""
-        p = self._params.get(device)
-        if p is None:
-            rows = [[float(l.codebook_scale) for l in self.layers], [l._magnitude for l in self.layers],
-                    [float(l.soft_clamp_input_value or 0.) for l in self.layers]]
-            t = torch.tensor(rows, dtype=torch.float32, device=device)
-            p = self._params[device] = (t, t[0].contiguous())
-        return p
+        rows = [[float(l.codebook_scale) for l in self.layers], [l._magnitude for l in self.layers],
+                [float(l.soft_clamp_input_value or 0.) for l in self.layers]]
+        t = torch.tensor(rows, dtype=torch.float32)
+        return t, t[0].contiguous()
 
     def _launch(self, z, mask, n_active, grouped):
         """z (N, G, d) -> (out (N, G, d), indices (N, Q) or (G, N, Q) when `grouped`, losses (G, Q) fp32)."""
@@ -73,7 +74,7 @@ class ResidualLFQ(nn.Module):
         Q = self.num_quantizers
         lay = self.layers[0]
         train = self.training
-        params, _ = self._stage_params(z.device)
+        params, _ = self._params.get(z.device)
         if grouped:
             indices = torch.empty((G, N, Q), dtype=torch.int64, device=z.device)
             view = indices.permute(1, 0, 2)
@@ -112,62 +113,21 @@ class ResidualLFQ(nn.Module):
             return ret
         return (*ret, self.get_codes_from_indices(all_indices))
 
-    def _decode(self, indices, want_sum, want_codes):
-        quantize_dim = indices.shape[-1]
-        Q = self.num_quantizers
-        if quantize_dim < Q:
-            assert self.quantize_dropout > 0., \
-                'quantize dropout must be greater than 0 if you wish to reconstruct from a signal with less fine quantizations'
-        lead = indices.shape[:-1]
-        flat = indices.reshape(-1, quantize_dim)
-        if quantize_dim < Q:
-            flat = F.pad(flat, (0, Q - quantize_dim), value=-1)
-        flat = flat.contiguous()
-        N, d = flat.shape[0], self.codebook_dim
-        _, vals = self._stage_params(flat.device)
-        s, codes = ops.lfq_decode(flat.view(N, 1, Q), d, vals, want_sum, want_codes)
-        s = s.reshape(*lead, d) if s is not None else None
-        codes = codes.reshape(Q, *lead, d) if codes is not None else None
-        return s, codes
-
-    def get_codes_from_indices(self, indices):
-        """rlfq:101-131: the layers' (non-spherical) `codebook` rows, zeros for dropped stages."""
-        return self._decode(indices, False, True)[1]
-
-    def get_output_from_indices(self, indices):
-        return self.project_out(self._decode(indices, True, False)[0])
+    def _decode_rows(self, idx, want_sum, want_codes):
+        """vqb_lfq_decode of (N, 1, Q) indices (rlfq:101-136): the layers' (non-spherical) `codebook` rows, zeros for dropped
+        stages."""
+        _, vals = self._params.get(idx.device)
+        return ops.lfq_decode(idx, self.codebook_dim, vals, want_sum, want_codes)
 
 
-class GroupedResidualLFQ(nn.Module):
+class GroupedResidualLFQ(GroupedResidual):
     """Drop-in for the reference's GroupedResidualLFQ (rlfq:218-292): `groups` ResidualLFQs over column blocks of the features,
     all groups in one forward launch, one entropy launch and one backward chain."""
 
     def __init__(self, *, dim, groups=1, accept_image_fmap=False, **kwargs):
-        super().__init__()
         if accept_image_fmap:
             _unsupported("GroupedResidualLFQ accept_image_fmap=True")
-        self.dim = dim
-        self.groups = groups
-        assert (dim % groups) == 0
-        dim_per_group = dim // groups
-        self.accept_image_fmap = accept_image_fmap
-        self.rvqs = nn.ModuleList([])
-        for _ in range(groups):
-            self.rvqs.append(ResidualLFQ(dim=dim_per_group, **kwargs))
-
-    @property
-    def codebooks(self):
-        return torch.stack(tuple(rvq.codebooks for rvq in self.rvqs))
-
-    @property
-    def split_dim(self):
-        return 1 if self.accept_image_fmap else -1
-
-    def get_codes_from_indices(self, indices):
-        return torch.stack(tuple(rvq.get_codes_from_indices(i) for rvq, i in zip(self.rvqs, indices)))
-
-    def get_output_from_indices(self, indices):
-        return torch.cat(tuple(rvq.get_output_from_indices(i) for rvq, i in zip(self.rvqs, indices)), dim=self.split_dim)
+        super().__init__(ResidualLFQ, dim=dim, groups=groups, accept_image_fmap=accept_image_fmap, **kwargs)
 
     def forward(self, x, mask=None, return_all_codes=False):
         shape, split_dim, device = x.shape, self.split_dim, x.device

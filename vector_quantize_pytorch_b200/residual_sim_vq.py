@@ -10,10 +10,10 @@ carries them into each layer's `code_transform`.
 from __future__ import annotations
 
 import torch
-import torch.nn.functional as F
 from torch import nn
 
 from . import ops
+from .residual_common import pad_dropped
 from .residual_vq import ResidualVQ, _PlanCache
 from .sim_vq import SimVQ
 
@@ -161,10 +161,9 @@ class ResidualSimVQ(nn.Module):
 
     def get_codes_from_indices(self, indices):  # rsv:99-135
         Q = self.num_quantizers
-        if indices.shape[-1] < Q:
-            assert self.quantize_dropout > 0., \
-                "quantize dropout must be greater than 0 if you wish to reconstruct from a signal with less fine quantizations"
-            indices = F.pad(indices, (0, Q - indices.shape[-1]), value=-1)
+        indices = pad_dropped(indices, Q, self.quantize_dropout,
+                              "quantize dropout must be greater than 0 if you wish to reconstruct from a signal with less fine "
+                              "quantizations")
         lead = indices.shape[:-1]
         flat = indices.reshape(-1, Q)
         mask = flat == -1

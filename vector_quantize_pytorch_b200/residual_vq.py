@@ -11,17 +11,15 @@ all-reduce per forward instead of the reference's 2 per codebook per stage.
 """
 from __future__ import annotations
 
-import math
 import os
-import random
 
 import torch
-import torch.distributed as distributed
 from torch import nn
 
 from . import ops
 from .codebook import _unsupported
 from .dist import allreduce_packed, PeerReducer
+from .residual_common import GroupedResidual, dropout_cut, pad_dropped, sync_seed
 from .vector_quantize import VectorQuantize, directional_reparam
 
 _DTYPES = (torch.float32, torch.bfloat16)
@@ -46,14 +44,6 @@ class _PlanCache(dict):
                 plans.clear()
             plan = plans[key] = build()
         return plan
-
-
-def _sync_seed(device):
-    """get_maybe_sync_seed (rvq:96-103): torch.randint on the device, all-reduced over the ranks."""
-    seed = torch.randint(0, 10_000, (), device=device)
-    if distributed.is_available() and distributed.is_initialized() and distributed.get_world_size() > 1:
-        distributed.all_reduce(seed)
-    return seed
 
 
 class _CodebookUpdates:
@@ -343,11 +333,8 @@ class ResidualVQ(nn.Module):
 
     def _pad_dropped(self, indices):
         """rvq:333-339: coarse indices (fewer than num_quantizers columns) are padded with -1 = "layer dropped"."""
-        missing = self.num_quantizers - indices.shape[-1]
-        if missing > 0:
-            assert self.quantize_dropout, "quantize dropout must be on to reconstruct from fewer than num_quantizers indices"  # rvq:338
-            indices = torch.nn.functional.pad(indices, (0, missing), value=-1)
-        return indices
+        return pad_dropped(indices, self.num_quantizers, self.quantize_dropout,
+                           "quantize dropout must be on to reconstruct from fewer than num_quantizers indices")  # rvq:338
 
     def get_codes_from_indices(self, indices):  # rvq:324-376
         indices = self._pad_dropped(indices)
@@ -461,19 +448,11 @@ class ResidualVQ(nn.Module):
         return ret
 
     def _active_layers(self, fixed_seed, device) -> int:
-        """Number of leading layers that quantize in this forward.  Training with quantize_dropout (rvq:423-439): python's
-        random.Random(seed).randrange(cutoff, Q) is the last active layer, rounded up to a multiple if asked; without an explicit
-        seed one is drawn like the reference's get_maybe_sync_seed."""
-        Q = self.num_quantizers
+        """Number of leading layers that quantize in this forward: all, or in training with quantize_dropout (rvq:423-439) the
+        cut `dropout_cut` draws."""
         if not (self.training and self.quantize_dropout):
-            return Q
-        if fixed_seed is None:
-            fixed_seed = _sync_seed(device).item()
-        index = random.Random(fixed_seed).randrange(self.quantize_dropout_cutoff_index, Q)
-        mult = self.quantize_dropout_multiple_of
-        if mult != 1:
-            index = math.ceil((index + 1) / mult) * mult - 1  # rvq:39-40, :439
-        return min(index + 1, Q)
+            return self.num_quantizers
+        return dropout_cut(self, fixed_seed, device)
 
     def _codebooks_need_grad(self):
         return any(vq._codebook.embed.requires_grad for vq in self.layers)
@@ -598,30 +577,11 @@ class ResidualVQ(nn.Module):
         return quantized_out.reshape(-1, D), torch.stack(all_idx, dim=-1).reshape(-1, Q), torch.stack(all_losses)
 
 
-class GroupedResidualVQ(nn.Module):
+class GroupedResidualVQ(GroupedResidual):
     def __init__(self, *, dim, groups=1, accept_image_fmap=False, **kwargs):
-        super().__init__()
-        self.dim = dim
-        self.groups = groups
-        assert (dim % groups) == 0  # rvq:646
         if accept_image_fmap:
             _unsupported("GroupedResidualVQ(accept_image_fmap=True)")
-        self.accept_image_fmap = accept_image_fmap
-        self.rvqs = nn.ModuleList([ResidualVQ(dim=dim // groups, **kwargs) for _ in range(groups)])  # rvq:651-658
-
-    @property
-    def codebooks(self):
-        return torch.stack(tuple(rvq.codebooks for rvq in self.rvqs))
-
-    @property
-    def split_dim(self):
-        return -1
-
-    def get_codes_from_indices(self, indices):
-        return torch.stack(tuple(rvq.get_codes_from_indices(i) for rvq, i in zip(self.rvqs, indices)))
-
-    def get_output_from_indices(self, indices):
-        return torch.cat(tuple(rvq.get_output_from_indices(i) for rvq, i in zip(self.rvqs, indices)), dim=-1)
+        super().__init__(ResidualVQ, dim=dim, groups=groups, accept_image_fmap=accept_image_fmap, **kwargs)  # rvq:646-658
 
     def _program_ok(self, xs, freeze_codebook):
         """All groups in one ops.RvqProgram: every group takes its own program path (ResidualVQ._program_ok), and the op list
@@ -647,7 +607,7 @@ class GroupedResidualVQ(nn.Module):
         if self.training:
             # the reference draws one torch.randint here even without quantize-dropout (rvq:701 -> :96-103);
             # consume it too so that seeded runs stay aligned with the reference's RNG stream.
-            seed = _sync_seed(x.device)
+            seed = sync_seed(x.device)
         dropout_seed = None
         if self.training and any(rvq.quantize_dropout for rvq in self.rvqs):
             dropout_seed = int(seed.item())   # rvq:701: the SAME dropout index in every group
