@@ -110,3 +110,115 @@ def test_abi_argument_errors():
                                         None) == E_INVALID   # ksplit not a power of two
     assert lib.vqb_lfq_decode(None, 1, 0, 0, 0, 4, 1, 4, 1, None, None, None, None) == E_INVALID
     assert lib.vqb_lfq_entropy_tiles(0) == E_UNSUPPORTED and lib.vqb_lfq_entropy_tiles(18) == 64
+
+
+# ---- the entropy kernels' error bounds (oracle/lfq_oracle.py::entropy_reference): they hold for fp32 arithmetic and have teeth
+
+def _rows(d, R, seed):
+    """Generic rows, zero rows and rows whose every |a_j| puts codes on both sides of the 1e-5 clamp, fp32 values."""
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(R, d, generator=g, dtype=torch.float64) * torch.logspace(-1, 0.5, R, dtype=torch.float64)[:, None]
+    x[R // 3] = 0.
+    return x.float().double()
+
+
+def _emulate(x, m, tau, cp, V, chunks, ksplit):
+    """The kernels' arithmetic restated in fp32 on the CPU (torch's expf / log1pf / exp2 / tanh stand in for CUDA's), in one
+    of the summation orders the bounds allow.  -> (pse, colsum (K,), grad (R, d)), float64 views of the fp32 results."""
+    f = torch.float32
+    R, d = x.shape
+    K = 1 << d
+    x = x.float()
+    tm = torch.tensor(2 * tau, dtype=f) * torch.tensor(m, dtype=f)
+    av = tm * x
+    log2e, ln2 = torch.tensor(1.4426950408889634, dtype=f), torch.tensor(0.6931471805599453, dtype=f)
+    lo2, lne = torch.tensor(O.LOG2_EPS, dtype=f), torch.tensor(O.LN_EPS, dtype=f)
+
+    def nsp2(y):
+        return -(y.clamp(min=0) + torch.log1p(torch.exp(-y.abs()))) * log2e
+
+    l1, l0 = nsp2(-2 * av), nsp2(2 * av)
+    bits = O._code_bits(d, "cpu").bool()
+    lp = torch.zeros((R, K), dtype=f)
+    for j in range(d):
+        lp = lp + torch.where(bits[:, j], l1[:, j:j + 1], l0[:, j:j + 1])
+    p = torch.exp2(lp)
+    hs = -p * torch.where(lp >= lo2, lp * ln2, lne)
+    pse = hs.double().sum()
+    cr = -(-R // chunks)
+    col = torch.zeros(K, dtype=f)
+    for c in range(chunks):
+        part = torch.zeros(K, dtype=f)
+        for r in range(c * cr, min(R, (c + 1) * cr)):
+            part = part + p[r]
+        col = col + part
+    hp = torch.where(lp >= lo2, -(lp.double() * ln2.double() + 1).float(), -lne)
+    u = (float(np.float32(cp)) * hp.double() + V.double()[None]).float()   # one fma
+    w = p * u
+    sgn = O.codebook_signs(d).float()
+    L = min(K, 16)
+    seg = w.view(R, K // L, L, 1) * sgn.view(1, K // L, L, d)
+    s16 = torch.zeros((R, K // L, d + 1), dtype=f)
+    for i in range(L):   # the 16-code fp32 sums of w sgn_kj and of w
+        s16 = s16 + torch.cat([seg[:, :, i], w.view(R, K // L, L)[:, :, i, None]], -1)
+    parts = s16.double().view(R, ksplit, -1, d + 1).sum(2).float()
+    tot = torch.zeros((R, d + 1), dtype=f)
+    for k in range(ksplit):
+        tot = tot + parts[:, k]
+    grad = tm * (tot[:, :d] - tot[:, d:] * torch.tanh(tm * x))
+    return pse, col.double(), grad.double()
+
+
+@pytest.mark.parametrize("d,R,chunks,ksplit", [(2, 40, 3, 1), (5, 90, 2, 2), (9, 70, 3, 8), (12, 33, 2, 16)])
+@pytest.mark.parametrize("tau", [1e-3, 1.0, 100.0])
+def test_entropy_bounds_hold_for_fp32(d, R, chunks, ksplit, tau):
+    tau = float(np.float32(tau))
+    x = _rows(d, R, d)
+    g = torch.Generator().manual_seed(1)
+    V = (torch.randn(1 << d, generator=g) * 1e-2).float()
+    cp, m = 0.75, 0.8125
+    ref = O.entropy_reference(x, m, tau, cp, V)
+    _, gref = O.loss_and_grad(x, m, tau, cp, V)
+    torch.testing.assert_close(ref.grad, gref, rtol=1e-10, atol=1e-12 * float(gref.abs().max()))   # float64 autograd's gradient
+    hs, cs = O.dense_stats(x, m, tau)
+    torch.testing.assert_close(ref.pse, hs, rtol=1e-12, atol=0)
+    torch.testing.assert_close(ref.colsum, cs, rtol=1e-12, atol=0)
+    pb, cb, gb = ref.bounds(chunks, ksplit)
+    pse, col, grad = _emulate(x, m, tau, cp, V, chunks, ksplit if (1 << d) // ksplit >= 16 else 1)
+    assert abs(float(pse - ref.pse)) <= pb
+    assert ((col - ref.colsum).abs() <= cb).all()
+    assert ((grad - ref.grad).abs() <= gb).all()
+
+
+def test_entropy_bounds_have_teeth():
+    """Each wrong answer below falls outside the bound, on every row of a moderate batch (d = 10, tau = 1)."""
+    d, R, tau, m, cp = 10, 48, 1.0, 0.8125, 0.75
+    K = 1 << d
+    chunks, ksplit = 2, 2
+    g = torch.Generator().manual_seed(3)
+    x = torch.randn(R, d, generator=g, dtype=torch.float64).float().double()
+    V = (torch.randn(K, generator=g) * 1e-2).float()
+    ref = O.entropy_reference(x, m, tau, cp, V)
+    pb, cb, gb = ref.bounds(chunks, ksplit)
+    b = O.entropy_block(x, m, tau, cp, V)
+    p, w = b["p"], b["w"]
+    sgn = O.codebook_signs(d)
+    contrib = ref.tm * (w[:, :, None] * (sgn[None] - ref.t[:, None, :]))   # (R, K, d): code k's part of grad[r, j]
+
+    def outside(err, bound):
+        return bool((err.abs() > bound).any())
+
+    for r in range(R):
+        # one row's contribution missing from its chunk's column sums
+        assert outside(p[r], cb), r
+        assert abs(float(O.h(p[r]).sum())) > pb, r
+        # one 16-code segment (the row's largest) and one K split missing from the row's gradient
+        segs = contrib[r].view(K // 16, 16, d).sum(1)
+        assert outside(segs[segs.abs().amax(1).argmax()], gb[r]), r
+        for half in contrib[r].view(ksplit, K // ksplit, d).sum(1):
+            assert outside(half, gb[r]), r
+        # one code's probability doubled (the row's most likely code)
+        k = int(p[r].argmax())
+        assert outside(p[r, k:k + 1], cb[k:k + 1]), r
+        # the row's gradient replaced by 0
+        assert outside(ref.grad[r], gb[r]), r

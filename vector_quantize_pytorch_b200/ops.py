@@ -699,17 +699,34 @@ def lfq_backward(z: torch.Tensor, grad_out: torch.Tensor, Q: int, n_active: int,
     return gz
 
 
-def lfq_entropy(x: torch.Tensor, rows: torch.Tensor | None, R: int, m: torch.Tensor, tau: float, want_colsum: bool):
+def lfq_entropy_plan(R: int, SG: int, D: int, sms: int, want_colsum: bool) -> tuple[int, int]:
+    """(chunks, ksplit) of the entropy kernels for R rows in each of SG (stage, group) pairs of 2^D codes on `sms` SMs (host
+    only).  chunks (vqb_lfq_entropy): row chunks, enough CTAs for 4 per SM, at most one per 32-row batch, and with the column
+    sums at most 8 Mi floats of per-chunk partials.  ksplit (vqb_lfq_entropy_backward): the K split, doubled while the CTAs
+    are under 4 per SM and each split keeps at least 2048 codes."""
+    K = 1 << D
+    tiles = _queried(lib.vqb_lfq_entropy_tiles(D), "vqb_lfq_entropy_tiles")
+    chunks = -(-4 * sms // (tiles * SG))
+    chunks = max(1, min(chunks, -(-R // 32), 65535))
+    if want_colsum:
+        chunks = max(1, min(chunks, (8 << 20) // (SG * K)))   # partial column sums <= 32 MiB
+    blocks = -(-R // 128) * SG
+    ksplit = 1
+    while blocks * ksplit < 4 * sms and K // (2 * ksplit) >= 2048:
+        ksplit *= 2
+    return chunks, ksplit
+
+
+def lfq_entropy(x: torch.Tensor, rows: torch.Tensor | None, R: int, m: torch.Tensor, tau: float, want_colsum: bool,
+                chunks: int | None = None):
     """vqb_lfq_entropy over x (S, N, G, D) fp32: -> (sum of h(p) per (s, g) (S * G,) fp64, column sums of p (S * G, K) fp32 or
-    None).  rows: int32 (S * G, R) or (R,) row lists, or None for rows 0..R-1."""
+    None).  rows: int32 (S * G, R) or (R,) row lists, or None for rows 0..R-1.  chunks: the plan's by default."""
     _require_cuda(x, rows, m)
     S, N, G, D = x.shape
     SG, K, dev = S * G, 1 << D, x.device
     tiles = _queried(lib.vqb_lfq_entropy_tiles(D), "vqb_lfq_entropy_tiles")
-    chunks = -(-4 * _sms(dev) // (tiles * SG))
-    chunks = max(1, min(chunks, -(-R // 32), 65535))
-    if want_colsum:
-        chunks = max(1, min(chunks, (8 << 20) // (SG * K)))   # partial column sums <= 32 MiB
+    if chunks is None:
+        chunks = lfq_entropy_plan(R, SG, D, _sms(dev), want_colsum)[0]
     rs = 0 if rows is None or rows.dim() == 1 else rows.shape[1]
     pse = torch.empty((SG, chunks, tiles), dtype=torch.float64, device=dev)
     col = torch.empty((chunks, SG, K), dtype=torch.float32, device=dev) if want_colsum else None
@@ -721,15 +738,14 @@ def lfq_entropy(x: torch.Tensor, rows: torch.Tensor | None, R: int, m: torch.Ten
 
 
 def lfq_entropy_backward(x: torch.Tensor, rows: torch.Tensor | None, R: int, m: torch.Tensor, tau: float, cp: torch.Tensor,
-                         V: torch.Tensor | None) -> torch.Tensor:
-    """vqb_lfq_entropy_backward: d/dx (x's layout, zero outside the listed rows) given dL/dp = cp[sg] h'(p) + V[sg, k]."""
+                         V: torch.Tensor | None, ksplit: int | None = None) -> torch.Tensor:
+    """vqb_lfq_entropy_backward: d/dx (x's layout, zero outside the listed rows) given dL/dp = cp[sg] h'(p) + V[sg, k].
+    ksplit: the plan's by default."""
     _require_cuda(x, rows, m, cp, V)
     S, N, G, D = x.shape
-    SG, K, dev = S * G, 1 << D, x.device
-    blocks = -(-R // 128) * SG
-    ksplit = 1
-    while blocks * ksplit < 4 * _sms(dev) and K // (2 * ksplit) >= 2048:
-        ksplit *= 2
+    SG, dev = S * G, x.device
+    if ksplit is None:
+        ksplit = lfq_entropy_plan(R, SG, D, _sms(dev), False)[1]
     rs = 0 if rows is None or rows.dim() == 1 else rows.shape[1]
     work = torch.empty((ksplit, SG, R, D + 1), dtype=torch.float32, device=dev)
     grad = torch.zeros_like(x)
