@@ -473,6 +473,29 @@ int vqb_binmap_backward_plan(int64_t rows, int bits, int sms, int* plan);
 int vqb_binmap_backward(const float* logits, int64_t rows, int bits, const float* g, int64_t g_row_stride,
                         int64_t g_col_stride, int ksplit, double* work, float* dlogits, void* stream);
 
+/* HierarchicalVQ (hierarchical_vq.py "hvq"): the per-scale pool, upsample and residual update around the shared search, fp32,
+ * no atomics (every backward is the gather-form adjoint, so reruns give the same bits).  Images are NCHW (B, D, H, W)
+ * contiguous; rows are the channel-last (B, s, s, D) contiguous map the search reads and writes.  1 <= H, W, s <= 65536.
+ * vqb_hvq_pool: rows = adaptive_avg_pool2d(x, (s, s)) with ATen's windows [floor(i H / s), ceil((i + 1) H / s)) (hvq:134). */
+int vqb_hvq_pool(const float* x, int64_t B, int D, int H, int W, int s, float* rows, void* stream);
+/* g_x (B, D, H, W) = the adjoint of vqb_hvq_pool applied to g_rows (B, s, s, D): each pixel sums g / kh / kw over its windows. */
+int vqb_hvq_pool_backward(const float* g_rows, int64_t B, int D, int H, int W, int s, float* g_x, void* stream);
+/* u = bilinear(rows (B, s, s, D), (H, W), align_corners = False) with ATen's source-index rule, or rows itself when
+ * (s, s) == (H, W) (hvq:105-106).  Writes, each when non-NULL: q = u; recon_out = recon + u (recon NULL: 0 + u);
+ * resid_out = resid - u (needs resid).  At least one output. */
+int vqb_hvq_upsample(const float* rows, int64_t B, int D, int s, int H, int W, float* q, const float* recon,
+                     const float* resid, float* recon_out, float* resid_out, void* stream);
+/* g_rows (B, s, s, D) = the adjoint of vqb_hvq_upsample applied to g_a - g_b (each (B, D, H, W), NULL: zero; not both). */
+int vqb_hvq_upsample_backward(const float* g_a, const float* g_b, int64_t B, int D, int s, int H, int W, float* g_rows,
+                              void* stream);
+/* q = (1 - r) up + r conv over n elements (hvq:25; both factors rounded to fp32, no fma), then recon_out = recon + q (recon
+ * NULL: 0 + q) and resid_out = resid - q, each when non-NULL (at least one; resid_out needs resid). */
+int vqb_hvq_blend_update(const float* up, const float* conv, int64_t n, double r, const float* recon, const float* resid,
+                         float* recon_out, float* resid_out, void* stream);
+/* g_q = g_recon - g_resid (each NULL: zero; not both), g_up = (1 - r) g_q, g_conv = r g_q. */
+int vqb_hvq_blend_backward(const float* g_recon, const float* g_resid, int64_t n, double r, float* g_up, float* g_conv,
+                           void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -127,6 +127,12 @@ SIGNATURES = {
     "vqb_binmap_hot": (_i32, [_vp, _vp, _i64, _i32, _vp, _vp]),
     "vqb_binmap_backward_plan": (_i32, [_i64, _i32, _i32, _vp]),
     "vqb_binmap_backward": (_i32, [_vp, _i64, _i32, _vp, _i64, _i64, _i32, _vp, _vp, _vp]),
+    "vqb_hvq_pool": (_i32, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "vqb_hvq_pool_backward": (_i32, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "vqb_hvq_upsample": (_i32, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "vqb_hvq_upsample_backward": (_i32, [_vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "vqb_hvq_blend_update": (_i32, [_vp, _vp, _i64, _f64, _vp, _vp, _vp, _vp, _vp]),
+    "vqb_hvq_blend_backward": (_i32, [_vp, _vp, _i64, _f64, _vp, _vp, _vp]),
 }
 
 

@@ -897,3 +897,102 @@ def binmap_backward(logits: torch.Tensor, g: torch.Tensor, ksplit: int | None = 
                                       _stream()), "vqb_binmap_backward")
     _count(1 if ksplit == 1 else 2)
     return dl
+
+
+# ---- HierarchicalVQ (csrc/vq_hvq.cu) ----
+# Images are (B, D, H, W) NCHW contiguous fp32; `rows` are the channel-last (B, s, s, D) contiguous maps the search reads and
+# writes, handed around as their (B, D, s, s) views.
+
+def _hvq_image(t: torch.Tensor, what: str) -> torch.Tensor:
+    if t.dtype != torch.float32:
+        raise TypeError(f"vqb200 HierarchicalVQ supports float32 {what}, got {t.dtype}")
+    _require_cuda(t)
+    return t.contiguous()
+
+
+def _hvq_rows(t: torch.Tensor, what: str) -> torch.Tensor:
+    """A (B, D, s, s) map as its channel-last rows (B, s, s, D) contiguous: free for the search's own outputs."""
+    if t.dtype != torch.float32:
+        raise TypeError(f"vqb200 HierarchicalVQ supports float32 {what}, got {t.dtype}")
+    _require_cuda(t)
+    return t.permute(0, 2, 3, 1).contiguous()
+
+
+def hvq_pool(x: torch.Tensor, s: int) -> torch.Tensor:
+    """vqb_hvq_pool: adaptive_avg_pool2d(x, (s, s)) of x (B, D, H, W), returned as the (B, D, s, s) view of channel-last rows."""
+    x = _hvq_image(x, "inputs")
+    B, D, H, W = x.shape
+    rows = torch.empty((B, s, s, D), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.vqb_hvq_pool(_p(x), B, D, H, W, s, _p(rows), _stream()), "vqb_hvq_pool")
+    _count(1)
+    return rows.permute(0, 3, 1, 2)
+
+
+def hvq_pool_backward(g: torch.Tensor, H: int, W: int) -> torch.Tensor:
+    """vqb_hvq_pool_backward: d x (B, D, H, W) from the gradient g (B, D, s, s) of hvq_pool's output."""
+    g = _hvq_rows(g, "gradients")
+    B, s, _, D = g.shape
+    gx = torch.empty((B, D, H, W), dtype=torch.float32, device=g.device)
+    with torch.cuda.device(g.device):
+        check(lib.vqb_hvq_pool_backward(_p(g), B, D, H, W, s, _p(gx), _stream()), "vqb_hvq_pool_backward")
+    _count(1)
+    return gx
+
+
+def hvq_upsample(q: torch.Tensor, H: int, W: int, recon=None, resid=None, want_q=True, want_recon=False, want_resid=False):
+    """vqb_hvq_upsample: u = bilinear(q (B, D, s, s), (H, W)) (q itself when (s, s) == (H, W)).  Returns (u, recon + u,
+    resid - u), each None unless asked for; recon None counts as zero."""
+    rows = _hvq_rows(q, "inputs")
+    B, s, _, D = rows.shape
+    outs = [torch.empty((B, D, H, W), dtype=torch.float32, device=q.device) if want else None
+            for want in (want_q, want_recon, want_resid)]
+    recon = None if recon is None else _hvq_image(recon, "reconstructions")
+    resid = None if resid is None else _hvq_image(resid, "residuals")
+    with torch.cuda.device(q.device):
+        check(lib.vqb_hvq_upsample(_p(rows), B, D, s, H, W, _p(outs[0]), _p(recon), _p(resid), _p(outs[1]), _p(outs[2]),
+                                   _stream()), "vqb_hvq_upsample")
+    _count(1)
+    return tuple(outs)
+
+
+def hvq_upsample_backward(g_a, g_b, s: int) -> torch.Tensor:
+    """vqb_hvq_upsample_backward: d q (B, D, s, s), as the view of channel-last rows, from g_a - g_b (B, D, H, W) (either
+    None: zero, not both)."""
+    g_a = None if g_a is None else _hvq_image(g_a, "gradients")
+    g_b = None if g_b is None else _hvq_image(g_b, "gradients")
+    ref = g_a if g_a is not None else g_b
+    B, D, H, W = ref.shape
+    g_rows = torch.empty((B, s, s, D), dtype=torch.float32, device=ref.device)
+    with torch.cuda.device(ref.device):
+        check(lib.vqb_hvq_upsample_backward(_p(g_a), _p(g_b), B, D, s, H, W, _p(g_rows), _stream()),
+              "vqb_hvq_upsample_backward")
+    _count(1)
+    return g_rows.permute(0, 3, 1, 2)
+
+
+def hvq_blend_update(up: torch.Tensor, conv: torch.Tensor, r: float, recon=None, resid=None, want_resid=True):
+    """vqb_hvq_blend_update: q = (1 - r) up + r conv; returns (recon + q, resid - q or None).  recon None counts as zero."""
+    up, conv = _hvq_image(up, "inputs"), _hvq_image(conv, "inputs")
+    recon = None if recon is None else _hvq_image(recon, "reconstructions")
+    resid = None if resid is None else _hvq_image(resid, "residuals")
+    recon_out = torch.empty_like(up)
+    resid_out = torch.empty_like(up) if want_resid else None
+    with torch.cuda.device(up.device):
+        check(lib.vqb_hvq_blend_update(_p(up), _p(conv), up.numel(), float(r), _p(recon), _p(resid), _p(recon_out),
+                                       _p(resid_out), _stream()), "vqb_hvq_blend_update")
+    _count(1)
+    return recon_out, resid_out
+
+
+def hvq_blend_backward(g_recon, g_resid, r: float):
+    """vqb_hvq_blend_backward: (d up, d conv) from the gradients of recon + q and resid - q (either None: zero, not both)."""
+    g_recon = None if g_recon is None else _hvq_image(g_recon, "gradients")
+    g_resid = None if g_resid is None else _hvq_image(g_resid, "gradients")
+    ref = g_recon if g_recon is not None else g_resid
+    g_up, g_conv = torch.empty_like(ref), torch.empty_like(ref)
+    with torch.cuda.device(ref.device):
+        check(lib.vqb_hvq_blend_backward(_p(g_recon), _p(g_resid), ref.numel(), float(r), _p(g_up), _p(g_conv), _stream()),
+              "vqb_hvq_blend_backward")
+    _count(1)
+    return g_up, g_conv
