@@ -110,6 +110,28 @@ def test_abi_argument_errors():
                                         None) == E_INVALID   # ksplit not a power of two
     assert lib.vqb_lfq_decode(None, 1, 0, 0, 0, 4, 1, 4, 1, None, None, None, None) == E_INVALID
     assert lib.vqb_lfq_entropy_tiles(0) == E_UNSUPPORTED and lib.vqb_lfq_entropy_tiles(18) == 64
+    # the row kernels' shape checks run before the device check: Q, n_active, N * G, and the backward's own pointers
+    P = 1 << 20
+
+    def fwd(N=4, G=1, D=4, Q=2, na=2):
+        return lib.vqb_lfq_forward(P, 0, N, G, D, Q, na, 1, 1, 0, P, P, P, 0, 0, 0, None, None, None, 0, None)
+
+    def bwd(N=4, G=1, D=4, Q=2, na=2, gout=P, gz=P):
+        return lib.vqb_lfq_backward(P, 0, N, G, D, Q, na, 1, 1, 0, P, gout, None, None, None, gz, None)
+
+    for f in (fwd, bwd):
+        assert f(Q=65, na=1) == E_UNSUPPORTED
+        assert f(na=0) == E_INVALID and f(na=3) == E_INVALID and f(Q=0, na=0) == E_INVALID
+        assert f(N=1 << 30, G=2) == E_UNSUPPORTED   # N * G = 2^31
+        assert f(D=0) == E_UNSUPPORTED and f(N=0) == E_INVALID
+    assert lib.vqb_lfq_forward(P, 2, 4, 1, 4, 2, 2, 1, 1, 0, P, P, P, 0, 0, 0, None, None, None, 0, None) == E_INVALID   # fp16
+    assert lib.vqb_lfq_forward(P, 0, 4, 1, 4, 2, 2, 1, 1, 0, P, P, P, 0, 0, 0, None, None, P, 0, None) == E_INVALID   # no blocks
+    assert bwd(gout=None) == E_INVALID and bwd(gz=None) == E_INVALID
+    assert lib.vqb_lfq_decode(P, 1, 0, 0, 0, 4, 1, 4, 65, P, P, None, None) == E_UNSUPPORTED
+    assert lib.vqb_lfq_decode(P, 1, 0, 0, 0, 1 << 30, 2, 4, 1, P, P, None, None) == E_UNSUPPORTED
+    assert lib.vqb_lfq_decode(P, 1, 0, 0, 0, 4, 1, 21, 1, P, P, None, None) == E_UNSUPPORTED
+    assert lib.vqb_lfq_decode(P, 1, 0, 0, 0, 4, 1, 4, 0, P, P, None, None) == E_INVALID
+    assert lib.vqb_lfq_decode(P, 1, 0, 0, 0, 4, 1, 4, 1, P, None, None, None) == E_INVALID   # neither out nor codes
 
 
 # ---- the entropy kernels' error bounds (oracle/lfq_oracle.py::entropy_reference): they hold for fp32 arithmetic and have teeth

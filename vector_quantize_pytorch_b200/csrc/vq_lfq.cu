@@ -55,7 +55,8 @@ __device__ __forceinline__ void load_params(StageParams& p, const float* params,
 }
 
 // One stage's input transform, in the work dtype W (rounded after every op as torch does): the soft clamp tanh(x / c) * c,
-// then the spherical x / max(||x||, 1e-12) * s.  Returns ||x|| (the clamped norm) for the backward; t receives the tanh.
+// then the spherical x / max(||x||, 1e-12) * s.  Returns ||x|| rounded to W, before the clamp, for the backward; t receives
+// the tanh.
 template <bool BF>
 __device__ __forceinline__ float stage_input(float (&x)[LFQ_MAX_D], float (&t)[LFQ_MAX_D], int D, float c, bool sph, float s) {
   if (c != 0.f) {
@@ -66,18 +67,19 @@ __device__ __forceinline__ float stage_input(float (&x)[LFQ_MAX_D], float (&t)[L
         x[j] = rw<BF>(__fmul_rn(t[j], c));
       }
   }
-  float nrm = 1.f;
+  float rn = 1.f;
   if (sph) {
     float ss = 0.f;
 #pragma unroll
     for (int j = 0; j < LFQ_MAX_D; ++j)
       if (j < D) ss = __fmaf_rn(x[j], x[j], ss);
-    nrm = fmaxf(rw<BF>(__fsqrt_rn(ss)), rw<BF>(1e-12f));
+    rn = rw<BF>(__fsqrt_rn(ss));
+    const float nrm = fmaxf(rn, rw<BF>(1e-12f));
 #pragma unroll
     for (int j = 0; j < LFQ_MAX_D; ++j)
       if (j < D) x[j] = rw<BF>(__fmul_rn(rw<BF>(__fdiv_rn(x[j], nrm)), s));
   }
-  return nrm;
+  return rn;
 }
 
 struct FwdArgs {
@@ -384,7 +386,8 @@ __global__ void __launch_bounds__(LFQ_THREADS) lfq_backward_kernel(FwdArgs a, co
       const float s = P.s[q], m = P.m[q], c = P.c[q];
 #pragma unroll
       for (int j = 0; j < LFQ_MAX_D; ++j) x[j] = r[j];
-      const float nrm = stage_input<BF>(x, t, D, c, a.sph, s);
+      const float rn = stage_input<BF>(x, t, D, c, a.sph, s);
+      const float nrm = fmaxf(rn, rw<BF>(1e-12f));
       const float ccq = (cc && live) ? cc[q] : 0.f;
       // d original_input: the straight-through gradient, the entropy gradient, the commitment gradient (2 (x - q) per unit)
       float dot = 0.f;
@@ -401,11 +404,13 @@ __global__ void __launch_bounds__(LFQ_THREADS) lfq_backward_kernel(FwdArgs a, co
             dot += g[j] * (x[j] / s);              // y = x / s is the normalised vector
           }
         }
+      // below the clamp x / eps is linear in x: clamp_min passes the norm's gradient only where ||x|| >= eps, so no projection
+      if (!(rn >= rw<BF>(1e-12f))) dot = 0.f;
 #pragma unroll
       for (int j = 0; j < LFQ_MAX_D; ++j)
         if (j < D) {
           float gx = g[j];
-          if (a.sph) gx = (g[j] - (x[j] / s) * dot) / nrm;   // F.normalize backward (||x|| > 1e-12)
+          if (a.sph) gx = (g[j] - (x[j] / s) * dot) / nrm;   // F.normalize backward
           if (c != 0.f) gx = gx * (1.f - t[j] * t[j]);     // tanh(x / c) * c backward
           acc[j] += rw<BF>(gx);
           const float qv = x[j] > 0.f ? m : -m;
