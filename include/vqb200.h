@@ -496,6 +496,15 @@ int vqb_hvq_blend_update(const float* up, const float* conv, int64_t n, double r
 int vqb_hvq_blend_backward(const float* g_recon, const float* g_resid, int64_t n, double r, float* g_up, float* g_conv,
                            void* stream);
 
+/* RandomProjectionQuantizer (random_projection_quantizer.py "rpq"): the rows its cosine search takes (rpq:49-53), in one fp32
+ * pass over x (N, dim) contiguous:
+ *   rows[r, h E + j] = sum_d LN(x[r])[d] proj[h, d, j]     (N, H E) contiguous; proj (H, dim, E) contiguous, as `rand_projs`
+ * LN(v) = (v - mean) / sqrt(var + 1e-5) with the mean and the biased variance in fp32 (nn.LayerNorm(dim, elementwise_affine =
+ * False)); norm = 0 skips it.  A full fp32 product (no TF32); the normalised x is never written.  1 <= dim <= 65536,
+ * H E <= 1024, N dim and N H E below 2^40 (VQB_E_UNSUPPORTED otherwise); pointers 4-byte aligned (VQB_E_ALIGN). */
+int vqb_rpq_norm_project(const float* x, int64_t N, int dim, const float* proj, int H, int E, int norm, float* rows,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif

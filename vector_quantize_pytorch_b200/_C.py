@@ -133,6 +133,7 @@ SIGNATURES = {
     "vqb_hvq_upsample_backward": (_i32, [_vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
     "vqb_hvq_blend_update": (_i32, [_vp, _vp, _i64, _f64, _vp, _vp, _vp, _vp, _vp]),
     "vqb_hvq_blend_backward": (_i32, [_vp, _vp, _i64, _f64, _vp, _vp, _vp]),
+    "vqb_rpq_norm_project": (_i32, [_vp, _i64, _i32, _vp, _i32, _i32, _i32, _vp, _vp]),
 }
 
 

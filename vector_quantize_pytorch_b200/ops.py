@@ -996,3 +996,25 @@ def hvq_blend_backward(g_recon, g_resid, r: float):
               "vqb_hvq_blend_backward")
     _count(1)
     return g_up, g_conv
+
+
+# ---- RandomProjectionQuantizer (csrc/vq_rpq.cu) ----
+
+def rpq_norm_project(x: torch.Tensor, proj: torch.Tensor, norm: bool) -> torch.Tensor:
+    """vqb_rpq_norm_project: LN(x) @ proj for x (..., dim) and proj (H, dim, E) (`rand_projs`), returned as fp32 rows
+    (prod(x.shape[:-1]), H * E) packed head-major like the reference's 'b n h e -> b n (h e)'; norm False skips the LN."""
+    if x.dtype != torch.float32 or proj.dtype != torch.float32:
+        raise TypeError(f"vqb200 RandomProjectionQuantizer supports float32 inputs, got {x.dtype} (projection {proj.dtype})")
+    _require_cuda(x, proj)
+    if x.device != proj.device:
+        raise RuntimeError(f"vqb200 RandomProjectionQuantizer: inputs on {x.device}, projection on {proj.device}")
+    H, dim, E = proj.shape
+    assert x.shape[-1] == dim, (x.shape, proj.shape)
+    x = x.reshape(-1, dim).contiguous()
+    proj = proj.contiguous()
+    rows = torch.empty((x.shape[0], H * E), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.vqb_rpq_norm_project(_p(x), x.shape[0], dim, _p(proj), H, E, int(bool(norm)), _p(rows), _stream()),
+              "vqb_rpq_norm_project")
+    _count(1)
+    return rows

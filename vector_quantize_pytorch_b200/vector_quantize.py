@@ -395,11 +395,13 @@ class VectorQuantize(nn.Module):
     # Each returns (quantize, embed_ind, commit, glue, learn): the quantized rows and int64 indices in the layout of its input
     # rows, the kernels' commitment loss (None: taken by the glue below), the glue loss's (quantize, target) when that is not
     # (quantize, transform_input(x)), and what _LearnableCodebook needs (idx32, commit_rows) for a learnable codebook.
-    def _quantize_shared(self, x, update, ema_update, loss_weight, fused_loss, commit_grad, ema_update_weight, accum_ema_update):
+    # want_q False: the quantized rows are neither written nor returned (None), for callers that keep only the indices.
+    def _quantize_shared(self, x, update, ema_update, loss_weight, fused_loss, commit_grad, ema_update_weight, accum_ema_update,
+                         want_q=True):
         """One search over all rows; with shared heads every head's sub-vector is a row (vqp:1044-1049)."""
         cbk, shape = self._codebook, x.shape
         flat = x.detach().reshape(-1, shape[-1]).contiguous()
-        q = torch.empty_like(flat)
+        q = torch.empty_like(flat) if want_q else None
         idx64 = torch.empty((flat.shape[0],), dtype=torch.int64, device=flat.device)
         loss_buf = self._loss_scratch(flat.device) if fused_loss else None
         # a learnable codebook (vqp:710) gets the gradient of `quantize` and, in training, of the commitment loss (vqp:1214-1216)
@@ -418,9 +420,9 @@ class VectorQuantize(nn.Module):
         commit = loss_buf.clone().reshape(()) if fused_loss else None
         # the search's index buffer is reused by the next forward
         learn = (idx32.clone(), commit_rows[0] if commit_rows else None) if learns else None
-        return q.reshape(shape), idx64.reshape(shape[:-1]), commit, None, learn
+        return None if q is None else q.reshape(shape), idx64.reshape(shape[:-1]), commit, None, learn
 
-    def _quantize_heads(self, x, update, ema_update, loss_weight, fused_loss):
+    def _quantize_heads(self, x, update, ema_update, loss_weight, fused_loss, want_q=True):
         """separate_codebook_per_head, x (b, n, h, d) (vqp:1044-1049 'b n (h d) -> h b n d', Codebook(num_codebooks=h)): head i
         searches / updates codebook i of the (h, K, d) buffers — h independent chains on the same kernels, in head order (k-means
         init and dead-code expiry draw from the RNG head by head, like the reference's batched_sample_vectors)."""
@@ -439,13 +441,14 @@ class VectorQuantize(nn.Module):
         embed_ind = torch.empty(x.shape[:-1], dtype=torch.int64, device=x.device)   # 'h b n -> b n h' (vqp:1266-1268)
         qs = []
         for i, (v, xi) in enumerate(zip(views, xs)):
-            q = torch.empty_like(xi)
+            q = torch.empty_like(xi) if want_q else None
             v.quantize_rows(xi, update=update, q_out=q, idx64_out=embed_ind[..., i], idx_stride=heads,
                             loss_out=loss_buf[i:i + 1] if fused_loss else None, loss_weight=loss_weight, ema_update=ema_update)
-            qs.append(q.reshape(x.shape[:-2] + (d,)))
+            if want_q:
+                qs.append(q.reshape(x.shape[:-2] + (d,)))
         # one mse over all heads (vqp:1327) == the mean of the heads' (equal-sized) means
         commit = loss_buf.mean() if fused_loss else None
-        return torch.stack(qs, dim=2), embed_ind, commit, None, None
+        return torch.stack(qs, dim=2) if want_q else None, embed_ind, commit, None, None
 
     def _quantize_masked(self, x, mask, update, ema_update, loss_weight, want_loss):
         """mask (B, N) bool (vqp:599-600, :1317-1325, :1378-1396).  Masked positions take no part in the statistics or the loss
@@ -488,6 +491,38 @@ class VectorQuantize(nn.Module):
             commit = loss_buf.clone().reshape(())
         return quantize.reshape(B, N, D), embed_ind.reshape(B, N), commit, glue, None
 
+    def _split_heads(self, x):
+        """(b, n, h d) rows after project_in as the codebook calls take them (vqp:1044-1049); returns (rows, separate)."""
+        heads, batch, n = self.heads, x.shape[0], x.shape[1]
+        separate = heads > 1 and self.separate_codebook_per_head
+        if separate:     # 'b n (h d) -> b n h d': head i is searched in codebook i
+            x = x.reshape(batch, n, heads, -1)
+        elif heads > 1:  # 'b n (h d) -> 1 (b h) n d' — every head's sub-vector is a row for the ONE codebook
+            x = x.reshape(batch, n, heads, -1).transpose(1, 2).reshape(batch * heads, n, -1)
+        return x, separate
+
+    @torch.no_grad()
+    def eval_indices(self, x):
+        """The indices an eval-mode forward(x) returns for channel-last x (b, n, dim) without a mask, computed without
+        writing the quantized rows or running project_out, and with no loss: project_in, the head split and one search per
+        codebook (k-means init included, vqp:703).  For callers that keep only the codes (RandomProjectionQuantizer)."""
+        if x.ndim != 3:
+            raise TypeError(f"eval_indices expects (batch, seq, dim) rows, got shape {tuple(x.shape)}")
+        if not x.is_cuda:
+            raise RuntimeError("vqb200 has no CPU path: inputs must live on a CUDA (H100, sm_90) device")
+        batch, n = x.shape[0], x.shape[1]
+        x, separate = self._split_heads(self.project_in(x))
+        if x.dtype not in (torch.float32, torch.bfloat16):
+            raise TypeError(f"vqb200 supports float32 and bfloat16 inputs, got {x.dtype}")
+        cbk = self._codebook
+        if separate:
+            _, embed_ind, _, _, _ = self._quantize_heads(x, False, cbk.ema_update, 1., False, want_q=False)
+        else:
+            _, embed_ind, _, _, _ = self._quantize_shared(x, False, cbk.ema_update, 1., False, False, None, False, want_q=False)
+            if self.heads > 1:   # '1 (b h) n -> b n h'
+                embed_ind = embed_ind.reshape(batch, self.heads, n).transpose(1, 2)
+        return embed_ind
+
     def forward(self, x, indices=None, mask=None, lens=None, topk=None, sample_codebook_temp=None, freeze_codebook=None,
                 return_loss_breakdown=False, codebook_transform_fn=None, ema_update_weight=None, accum_ema_update=False,
                 ema_update=None):
@@ -526,11 +561,7 @@ class VectorQuantize(nn.Module):
         x, restore = self._to_rows_layout(x)
         x = self.project_in(x)  # vqp:1151
         heads, batch, n = self.heads, x.shape[0], x.shape[1]
-        separate = heads > 1 and self.separate_codebook_per_head
-        if separate:     # 'b n (h d) -> b n h d': head i is searched in codebook i
-            x = x.reshape(batch, n, heads, -1)
-        elif heads > 1:  # vqp:1044-1049: 'b n (h d) -> 1 (b h) n d' — every head's sub-vector is a row for the ONE codebook
-            x = x.reshape(batch, n, heads, -1).transpose(1, 2).reshape(batch * heads, n, -1)
+        x, separate = self._split_heads(x)
         # decided AFTER project_in: with a projection the commitment loss must stay differentiable w.r.t. its weights
         # even when the raw input carries no grad (vqp:1151, :1327)
         input_requires_grad = x.requires_grad and torch.is_grad_enabled()
