@@ -350,6 +350,22 @@ int vqb_rsimvq_backward(const float* x, const float* codes, int Q, int K, const 
  * src, tgt, grad_out, out: [N][D] in `dtype` (arithmetic in fp32, rounded once on store). */
 int vqb_rotate(const void* src, const void* tgt, const void* grad_out, int64_t N, int D, int dtype, void* out, void* stream);
 
+/* The estimator of a masked training step (vector_quantize_pytorch.py:1225-1233, :1317-1325, :1378-1389), one warp per row.
+ * row_mask u8 [N] (0: padding), n_live i64 [1] = the number of live rows, both on the device; src = x, tgt = the codes the
+ * masked search wrote for the live rows (its padding rows are never read).
+ *   grad_out == NULL: forward   live rows tgt, padding rows 0 (pad_zeros != 0) or src
+ *   grad_out != NULL: backward  live rows  E(grad_out) + c (src - tgt),  c = 2 loss_weight grad_loss[0] / (n_live[0] D)
+ *                               padding rows 0 (pad_zeros != 0) or grad_out
+ * E = the rotate_to backward of vqb_rotate (VQB_ESTIMATOR_ROTATE), the identity (VQB_ESTIMATOR_STE) or 0 (VQB_ESTIMATOR_NONE);
+ * grad_loss f32 [1] = d loss / d commitment loss, NULL: no commitment term.  Padding rows never reach the rotation.
+ * src, tgt, grad_out, out: [N][D] in `dtype` (arithmetic in fp32, rounded once on store). */
+#define VQB_ESTIMATOR_NONE 0
+#define VQB_ESTIMATOR_STE 1
+#define VQB_ESTIMATOR_ROTATE 2
+int vqb_rotate_masked(const void* src, const void* tgt, const void* grad_out, const float* grad_loss, const uint8_t* row_mask,
+                      const int64_t* n_live, float loss_weight, int estimator, int pad_zeros, int64_t N, int D, int dtype,
+                      void* out, void* stream);
+
 /* DiVeQ, the directional reparameterization estimator (vector_quantize_pytorch.py:323-330), one warp per row (D <= 1024):
  *   e = q - x,  u = l2norm(e + noise_scale * noise) (detached),  out = x + u * ||e||
  *   grad_out == NULL: forward   out = x + u ||e||                                  (dtype)

@@ -88,6 +88,7 @@ SIGNATURES = {
     "vqb_ema_stats": (_i32, [_vp, _i32, _i64, _i32, _vp, _i32, _vp, _vp, _sz, _vp]),
     "vqb_ema_apply": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _f64, _f64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vqb_rotate": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
+    "vqb_rotate_masked": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _f32, _i32, _i32, _i64, _i32, _i32, _vp, _vp]),
     "vqb_diveq": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _f32, _vp, _vp, _vp]),
     "vqb_peer_barrier": (_i32, [_vp, _i32, _i32, _vp, _vp]),
     "vqb_ema_apply_peers": (_i32, [_vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _f64, _f64, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -486,41 +486,90 @@ rvq_accumulate_smem_kernel(const float* __restrict__ embeds, int64_t embed_strid
 // eps clamp could then scale the row by up to 1e6.  Products of fp32 values are exact in double, so the sums are exact to
 // about D * 2^-53.  nw and the dot products are those of the vectors the second sweep forms with the fp32 ins / int_.
 // ---------------------------------------------------------------------------------------------
+// One row (one warp) of the estimator.  COMMIT (backward only): out += commit * (src - tgt), the commitment-loss gradient that
+// rotate_masked_kernel adds in the same sweep.
+template <int DT, bool BWD, bool COMMIT = false>
+__device__ __forceinline__ void rotate_row(const void* __restrict__ src, const void* __restrict__ tgt,
+                                           const void* __restrict__ grad, int64_t base, int D, int lane, float commit,
+                                           void* out) {
+  using E = Elem<DT>;
+  constexpr float eps = 1e-6f;
+  double ss = 0.0, tt = 0.0, st = 0.0, gs = 0.0, gt = 0.0;
+  for (int i = lane; i < D; i += 32) {
+    const double s = E::load(src, base + i), t = E::load(tgt, base + i);
+    ss = fma(s, s, ss); tt = fma(t, t, tt); st = fma(s, t, st);
+    if (BWD) { const double g = E::load(grad, base + i); gs = fma(g, s, gs); gt = fma(g, t, gt); }
+  }
+  ss = warp_sum(ss); tt = warp_sum(tt); st = warp_sum(st);
+  if (BWD) { gs = warp_sum(gs); gt = warp_sum(gt); }
+  const float ns = static_cast<float>(sqrt(ss)), nt = static_cast<float>(sqrt(tt));
+  const float ins = 1.f / fmaxf(ns, eps), int_ = 1.f / fmaxf(nt, eps);        // safe_div (vqp:52-53)
+  const double dins = ins, dint = int_;
+  // ||u + q||^2 = ||u||^2 + ||q||^2 + 2 u.q
+  const double nw = sqrt(fmax(ss * dins * dins + tt * dint * dint + 2.0 * st * dins * dint, 0.0));
+  const double dinw = 1.0 / fmax(nw, static_cast<double>(eps));                // l2norm eps (vqp:37-38)
+  const float inw = static_cast<float>(dinw);
+  const float lam = nt * ins;
+  // forward: a = e.w, b = e.u ; backward: a = g.w, b = g.q
+  const float a = static_cast<float>(BWD ? (gs * dins + gt * dint) * dinw : (ss * dins + st * dint) * dinw);
+  const float b = static_cast<float>(BWD ? gt * dint : ss * dins);
+  for (int i = lane; i < D; i += 32) {
+    const float s = E::load(src, base + i), t = E::load(tgt, base + i);
+    const float u = s * ins, q = t * int_, w = (u + q) * inw;
+    const float e = BWD ? E::load(grad, base + i) : s;
+    const float r = BWD ? (e - 2.f * a * w + 2.f * b * u) : (e - 2.f * a * w + 2.f * b * q);
+    E::store(out, base + i, COMMIT ? r * lam + commit * (s - t) : r * lam);
+  }
+}
+
 template <int DT, bool BWD>
 __global__ void rotate_kernel(const void* __restrict__ src, const void* __restrict__ tgt, const void* __restrict__ grad,
                               int64_t N, int D, void* out) {
+  const int lane = threadIdx.x & 31;
+  const int wpb = blockDim.x >> 5;
+  for (int64_t row = static_cast<int64_t>(blockIdx.x) * wpb + (threadIdx.x >> 5); row < N;
+       row += static_cast<int64_t>(gridDim.x) * wpb)
+    rotate_row<DT, BWD>(src, tgt, grad, row * D, D, lane, 0.f, out);
+}
+
+// ---------------------------------------------------------------------------------------------
+// The estimator of VectorQuantize's masked training step (vqp:1225-1233, :1317-1325, :1378-1389), one warp per row.  Padding
+// rows (row_mask 0) are written as the padding value and never reach the estimator: the masked search gives them no code, and
+// rotate_to(x, 0) would divide by a zero norm.
+//   forward:  live rows tgt (the value both estimators take), padding rows 0 (pad_zeros) or src
+//   backward: live rows  estimator'(grad) + c (src - tgt),  c = 2 weight grad_loss[0] / (n_live[0] D)  (0 without grad_loss)
+//             padding rows 0 (pad_zeros) or grad
+// n_live and grad_loss are read on the device, so the host never waits for them.
+// ---------------------------------------------------------------------------------------------
+template <int DT, bool BWD>
+__global__ void rotate_masked_kernel(const void* __restrict__ src, const void* __restrict__ tgt, const void* __restrict__ grad,
+                                     const float* __restrict__ grad_loss, const uint8_t* __restrict__ row_mask,
+                                     const int64_t* __restrict__ n_live, float loss_weight, int estimator, int pad_zeros,
+                                     int64_t N, int D, void* out) {
   using E = Elem<DT>;
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
-  constexpr float eps = 1e-6f;
+  float commit = 0.f;
+  if (BWD && grad_loss) {
+    const int64_t nl = *n_live;     // > 0 whenever a live row exists
+    if (nl > 0) commit = static_cast<float>(2.0 * loss_weight * static_cast<double>(*grad_loss) / (static_cast<double>(nl) * D));
+  }
   for (int64_t row = static_cast<int64_t>(blockIdx.x) * wpb + (threadIdx.x >> 5); row < N;
        row += static_cast<int64_t>(gridDim.x) * wpb) {
     const int64_t base = row * D;
-    double ss = 0.0, tt = 0.0, st = 0.0, gs = 0.0, gt = 0.0;
-    for (int i = lane; i < D; i += 32) {
-      const double s = E::load(src, base + i), t = E::load(tgt, base + i);
-      ss = fma(s, s, ss); tt = fma(t, t, tt); st = fma(s, t, st);
-      if (BWD) { const double g = E::load(grad, base + i); gs = fma(g, s, gs); gt = fma(g, t, gt); }
-    }
-    ss = warp_sum(ss); tt = warp_sum(tt); st = warp_sum(st);
-    if (BWD) { gs = warp_sum(gs); gt = warp_sum(gt); }
-    const float ns = static_cast<float>(sqrt(ss)), nt = static_cast<float>(sqrt(tt));
-    const float ins = 1.f / fmaxf(ns, eps), int_ = 1.f / fmaxf(nt, eps);        // safe_div (vqp:52-53)
-    const double dins = ins, dint = int_;
-    // ||u + q||^2 = ||u||^2 + ||q||^2 + 2 u.q
-    const double nw = sqrt(fmax(ss * dins * dins + tt * dint * dint + 2.0 * st * dins * dint, 0.0));
-    const double dinw = 1.0 / fmax(nw, static_cast<double>(eps));                // l2norm eps (vqp:37-38)
-    const float inw = static_cast<float>(dinw);
-    const float lam = nt * ins;
-    // forward: a = e.w, b = e.u ; backward: a = g.w, b = g.q
-    const float a = static_cast<float>(BWD ? (gs * dins + gt * dint) * dinw : (ss * dins + st * dint) * dinw);
-    const float b = static_cast<float>(BWD ? gt * dint : ss * dins);
-    for (int i = lane; i < D; i += 32) {
-      const float s = E::load(src, base + i), t = E::load(tgt, base + i);
-      const float u = s * ins, q = t * int_, w = (u + q) * inw;
-      const float e = BWD ? E::load(grad, base + i) : s;
-      const float r = BWD ? (e - 2.f * a * w + 2.f * b * u) : (e - 2.f * a * w + 2.f * b * q);
-      E::store(out, base + i, r * lam);
+    if (!row_mask[row]) {
+      const void* from = BWD ? grad : src;
+      for (int i = lane; i < D; i += 32) E::store(out, base + i, pad_zeros ? 0.f : E::load(from, base + i));
+    } else if (!BWD) {
+      for (int i = lane; i < D; i += 32) E::store(out, base + i, E::load(tgt, base + i));
+    } else if (estimator == VQB_ESTIMATOR_ROTATE) {
+      rotate_row<DT, true, true>(src, tgt, grad, base, D, lane, commit, out);
+    } else {
+      const bool ste = estimator == VQB_ESTIMATOR_STE;
+      for (int i = lane; i < D; i += 32) {
+        const float d = commit * (E::load(src, base + i) - E::load(tgt, base + i));
+        E::store(out, base + i, ste ? E::load(grad, base + i) + d : d);
+      }
     }
   }
 }
@@ -722,6 +771,35 @@ extern "C" int vqb_rotate(const void* src, const void* tgt, const void* grad_out
   } else {
     if (grad_out) rotate_kernel<VQB_DTYPE_BF16, true><<<g, ROW_THREADS, 0, s>>>(src, tgt, grad_out, N, D, out);
     else rotate_kernel<VQB_DTYPE_BF16, false><<<g, ROW_THREADS, 0, s>>>(src, tgt, nullptr, N, D, out);
+  }
+  return static_cast<int>(cudaGetLastError());
+}
+
+extern "C" int vqb_rotate_masked(const void* src, const void* tgt, const void* grad_out, const float* grad_loss,
+                                 const uint8_t* row_mask, const int64_t* n_live, float loss_weight, int estimator,
+                                 int pad_zeros, int64_t N, int D, int dtype, void* out, void* stream) {
+  if (!src || !tgt || !row_mask || !out || N <= 0 || D <= 0) return VQB_E_INVALID;
+  if (grad_loss && !n_live) return VQB_E_INVALID;
+  if (dtype != VQB_DTYPE_F32 && dtype != VQB_DTYPE_BF16) return VQB_E_INVALID;
+  if (estimator != VQB_ESTIMATOR_NONE && estimator != VQB_ESTIMATOR_STE && estimator != VQB_ESTIMATOR_ROTATE)
+    return VQB_E_INVALID;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int g = capped_grid(N, ROW_THREADS / 32, 16);
+  const int pz = pad_zeros ? 1 : 0;
+  if (dtype == VQB_DTYPE_F32) {
+    if (grad_out)
+      rotate_masked_kernel<VQB_DTYPE_F32, true><<<g, ROW_THREADS, 0, s>>>(src, tgt, grad_out, grad_loss, row_mask, n_live,
+                                                                          loss_weight, estimator, pz, N, D, out);
+    else
+      rotate_masked_kernel<VQB_DTYPE_F32, false><<<g, ROW_THREADS, 0, s>>>(src, tgt, nullptr, nullptr, row_mask, nullptr,
+                                                                           0.f, estimator, pz, N, D, out);
+  } else {
+    if (grad_out)
+      rotate_masked_kernel<VQB_DTYPE_BF16, true><<<g, ROW_THREADS, 0, s>>>(src, tgt, grad_out, grad_loss, row_mask, n_live,
+                                                                           loss_weight, estimator, pz, N, D, out);
+    else
+      rotate_masked_kernel<VQB_DTYPE_BF16, false><<<g, ROW_THREADS, 0, s>>>(src, tgt, nullptr, nullptr, row_mask, nullptr,
+                                                                            0.f, estimator, pz, N, D, out);
   }
   return static_cast<int>(cudaGetLastError());
 }

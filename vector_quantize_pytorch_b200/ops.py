@@ -589,6 +589,34 @@ def rotate(src: torch.Tensor, tgt: torch.Tensor, grad_out: torch.Tensor | None =
     return out.reshape(shape)
 
 
+ESTIMATOR_NONE, ESTIMATOR_STE, ESTIMATOR_ROTATE = 0, 1, 2   # VQB_ESTIMATOR_*
+
+
+def rotate_masked(src: torch.Tensor, tgt: torch.Tensor, row_mask: torch.Tensor, estimator: int, pad_zeros: bool,
+                  grad_out: torch.Tensor | None = None, grad_loss: torch.Tensor | None = None,
+                  n_live: torch.Tensor | None = None, loss_weight: float = 1.) -> torch.Tensor:
+    """Estimator of a masked training step (vqb_rotate_masked).  src, tgt, grad_out (N, D) in one dtype; row_mask (N,) uint8;
+    grad_out None: the forward (live rows tgt, padding rows 0 or src); else d/d src of the estimator on live rows plus
+    2 loss_weight grad_loss (src - tgt) / (n_live D), and on padding rows 0 or grad_out.  grad_loss f32 (1,) and n_live
+    int64 (1,) stay on the device."""
+    _require_cuda(src, tgt, row_mask, grad_out, grad_loss, n_live)
+    N, D = src.shape
+    assert tgt.shape == src.shape and tgt.dtype == src.dtype and (grad_out is None or grad_out.dtype == src.dtype)
+    assert row_mask.dtype == torch.uint8 and row_mask.shape == (N,)
+    assert grad_loss is None or (grad_loss.dtype == torch.float32 and n_live is not None and n_live.dtype == torch.int64)
+    for t in (src, tgt, grad_out, row_mask, grad_loss, n_live):
+        assert t is None or t.is_contiguous()
+    out = torch.empty_like(src)
+    if N == 0:
+        return out
+    with torch.cuda.device(src.device):
+        check(lib.vqb_rotate_masked(_p(src), _p(tgt), _p(grad_out), _p(grad_loss), _p(row_mask), _p(n_live), float(loss_weight),
+                                    int(estimator), int(bool(pad_zeros)), N, D, _dtype_code(src), _p(out), _stream()),
+              "vqb_rotate_masked")
+    _count(1)
+    return out
+
+
 def diveq(x: torch.Tensor, q: torch.Tensor, noise: torch.Tensor, noise_scale: float, grad_out: torch.Tensor | None = None):
     """DiVeQ estimator (vqp:323-330, vqb_diveq): the forward value x + l2norm(q - x + noise_scale * noise) * ||q - x|| when
     grad_out is None, else (dx in x.dtype, dq fp32).  x, q, noise, grad_out: (..., D) in one dtype."""

@@ -400,9 +400,8 @@ class ResidualVQ(nn.Module):
             # in its statistics or loss (vqp:599-600, :1317-1325) and come back as zeros / index -1 (vqp:1378-1396), so their
             # residual is never reduced and their running sum stays zero.  That is exactly the forward over the COMPACTED
             # unmasked rows with zeros / -1 scattered around it (stage-wise: the row count changes from call to call, a
-            # cached program per count would not pay).
-            if x.requires_grad and torch.is_grad_enabled():
-                _unsupported("ResidualVQ.forward(mask=) on inputs / projections that require grad")
+            # cached program per count would not pay).  With gradients the layered path runs on those rows, gathered and
+            # scattered under autograd, so project_in / project_out and the input get the gradients of the reference.
             assert x.ndim == 3 and mask.shape == x.shape[:2]
             rows = mask.reshape(-1).nonzero(as_tuple=True)[0]  # host sync (the reference's masked path syncs as well)
             masked = (rows, torch.zeros((mask.numel(), D), dtype=x.dtype, device=x.device),
@@ -411,8 +410,13 @@ class ResidualVQ(nn.Module):
         if rows is not None and rows.numel() == 0:   # nothing to quantize: no quantizer runs, not even the dropout draw
             quantized = indices = None
             losses = torch.zeros((Q,), dtype=torch.float32, device=x.device)
+            if self._takes_layered(x):   # zero losses and rows that stay in the graph: a zero gradient, as in VectorQuantize
+                quantized = x.reshape(-1, D)[rows]
+                indices = torch.empty((0, Q), dtype=torch.int64, device=x.device)
+                losses = quantized.float().sum().repeat(Q)   # the sum over no rows is an exact zero
         elif self._takes_layered(x):
-            quantized, indices, losses = self._quantize_layered(x, freeze_codebook, self._active_layers(dropout_seed, x.device))
+            xl = x.reshape(-1, D)[rows] if rows is not None else x
+            quantized, indices, losses = self._quantize_layered(xl, freeze_codebook, self._active_layers(dropout_seed, x.device))
         else:
             if x.dtype not in _DTYPES:
                 raise TypeError(f"vqb200 supports float32 and bfloat16 inputs, got {x.dtype}")
@@ -435,7 +439,7 @@ class ResidualVQ(nn.Module):
         shape = x.shape
         if masked is not None:
             rows, quantized_all, indices_all = masked
-            if rows.numel() > 0:
+            if quantized is not None:
                 quantized_all[rows] = quantized
                 indices_all[rows] = indices
             quantized, indices = quantized_all, indices_all

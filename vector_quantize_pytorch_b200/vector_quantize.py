@@ -53,6 +53,35 @@ def rotate_to(src, tgt):
     return _RotateTo.apply(src, tgt)
 
 
+class _MaskedEstimator(torch.autograd.Function):
+    """The estimator and commitment-loss gradient of a masked training step on the in-kernel masked search (vqb_rotate_masked).
+    Forward: the searched codes on live rows, the padding value on padding rows (the values of the no-grad call, bit for bit)
+    and the kernels' commitment loss.  Backward, in one kernel: the estimator's gradient plus
+    2 w dL/dloss (x - q) / (n_live D) on live rows, 0 or the upstream gradient on padding rows.  n_live stays on the device."""
+
+    @staticmethod
+    def forward(ctx, x, q, commit, row_mask, n_live, estimator, pad_zeros, loss_weight):
+        ctx.save_for_backward(x, q, row_mask, n_live)
+        ctx.cfg = (estimator, pad_zeros, loss_weight, commit is not None)
+        out = ops.rotate_masked(x.detach(), q, row_mask, estimator, pad_zeros)
+        return out, (commit.clone() if commit is not None else torch.zeros((), dtype=torch.float32, device=x.device))
+
+    @staticmethod
+    def backward(ctx, grad_out, grad_loss):
+        x, q, row_mask, n_live = ctx.saved_tensors
+        estimator, pad_zeros, loss_weight, has_loss = ctx.cfg
+        gl = grad_loss.float().reshape(1).contiguous() if has_loss else None
+        dx = ops.rotate_masked(x.detach(), q, row_mask, estimator, pad_zeros, grad_out.to(x.dtype).contiguous(), gl, n_live,
+                               loss_weight)
+        return dx, None, None, None, None, None, None, None
+
+
+def _with_grad_of(value, expr):
+    """`value` carrying the gradient of `expr`, which equals it up to rounding (an estimator of it, or the same loss taken by
+    autograd): the forward keeps the bits of the call without gradients."""
+    return value + (expr - expr.detach())
+
+
 def diveq_noise(like):
     """The N(0, 1) draw of DiVeQ (`torch.randn_like(error_dir)`, vqp:327), in `like`'s shape and dtype.  Every DiVeQ forward
     of this package draws through this one function."""
@@ -455,11 +484,25 @@ class VectorQuantize(nn.Module):
         (the reference zeroes their one-hot rows, vqp:599-600, and averages the loss over the unmasked elements against the
         ORIGINAL input, vqp:1317-1325) and come back as zeros / index -1.  Euclidean codebooks: the search kernel takes the mask
         (row_mask of vqb_vq_forward).  Cosine codebooks, pending k-means init, dead-code expiry: the kernels run on the
-        compacted unmasked rows."""
+        compacted unmasked rows.
+
+        When x requires grad, the rows come back with the estimator of vqp:1225-1233 on the live rows (the padding rows pass
+        no gradient, or the upstream gradient when they return the input) and the commitment loss differentiable w.r.t. x;
+        every forward value stays that of the call without gradients.  The in-kernel path takes _MaskedEstimator (no host
+        sync); the compacted path gathers and scatters the rows under autograd."""
         cbk = self._codebook
         B, N, D = x.shape
-        flat = x.detach().reshape(-1, D).contiguous()
-        quantize = torch.zeros_like(flat) if self.return_zeros_for_masked_padding else flat.clone()
+        pad_zeros = self.return_zeros_for_masked_padding
+        grad = x.requires_grad and torch.is_grad_enabled()
+        x_rows = x.reshape(-1, D).contiguous()
+        flat = x_rows.detach()
+        estimator = ops.ESTIMATOR_NONE
+        if self.training and self.route_gradients_to_input:
+            estimator = ops.ESTIMATOR_ROTATE if self.rotation_trick else ops.ESTIMATOR_STE
+        if grad:   # padding rows are written by _MaskedEstimator / the scatter below
+            quantize = torch.empty_like(flat)
+        else:
+            quantize = torch.zeros_like(flat) if pad_zeros else flat.clone()
         embed_ind = torch.full((B * N,), -1, dtype=torch.int64, device=x.device)
         loss_buf = commit = glue = None
         if not self.use_cosine_sim and cbk._initted_host and not (update and cbk.has_dead_code_replacement):
@@ -472,9 +515,19 @@ class VectorQuantize(nn.Module):
             loss_buf = self._loss_scratch(x.device) if want_loss else None
             cbk.quantize_rows(flat, update=update, q_out=quantize, idx64_out=embed_ind, loss_out=loss_buf, loss_weight=loss_weight,
                               ema_update=ema_update, row_mask=row_mask, n_live=n_live)
+            if grad:
+                loss = loss_buf.clone().reshape(()) if loss_buf is not None else None
+                quantize, commit = _MaskedEstimator.apply(x_rows, quantize, loss, row_mask, n_live, estimator, pad_zeros,
+                                                          loss_weight)
+                loss_buf = None
+                if loss is None:
+                    commit = None
         else:
             rows = mask.reshape(-1).nonzero(as_tuple=True)[0]  # host sync (the reference's masked path syncs as well)
+            if grad:   # the padding rows: no gradient, or the input's own (vqp:1378-1389)
+                base = torch.zeros_like(flat) if pad_zeros else x_rows
             if rows.numel() > 0:
+                x_live = x_rows[rows] if grad else None
                 xc = flat[rows].contiguous()
                 qc = torch.empty_like(xc)
                 ic = torch.empty((xc.shape[0],), dtype=torch.int64, device=x.device)
@@ -482,11 +535,27 @@ class VectorQuantize(nn.Module):
                 loss_buf = self._loss_scratch(x.device) if want_loss and not self.use_cosine_sim else None
                 cbk.quantize_rows(xc, update=update, q_out=qc, idx64_out=ic, loss_out=loss_buf, loss_weight=loss_weight,
                                   ema_update=ema_update)
-                quantize[rows] = qc
                 embed_ind[rows] = ic
-                glue = (qc, xc)
-            elif want_loss:   # no unmasked row: no loss term
-                commit = torch.zeros((), dtype=torch.float32, device=x.device)
+                glue = (qc, x_live if grad else xc)
+                if grad:
+                    live = qc
+                    if estimator != ops.ESTIMATOR_NONE:
+                        x_t = cbk.transform_input(x_live)
+                        live = _with_grad_of(qc, rotate_to(x_t, qc) if estimator == ops.ESTIMATOR_ROTATE
+                                             else straight_through(x_t, qc))
+                    quantize = base.index_put((rows,), live)
+                    if loss_buf is not None:   # the kernels' loss with the gradient of the same mse taken by autograd
+                        commit = _with_grad_of(loss_buf.clone().reshape(()), loss_weight * F.mse_loss(qc, x_live))
+                        loss_buf = None
+                else:
+                    quantize[rows] = qc
+            else:   # no unmasked row: no loss term.  With gradients both outputs stay in the graph and pass x a zero gradient,
+                # like the in-kernel path (the sum over no rows is an exact zero)
+                none = x_rows[rows] if grad else None
+                if grad:
+                    quantize = base.index_put((rows,), none)
+                if want_loss:
+                    commit = none.float().sum() if grad else torch.zeros((), dtype=torch.float32, device=x.device)
         if loss_buf is not None:
             commit = loss_buf.clone().reshape(())
         return quantize.reshape(B, N, D), embed_ind.reshape(B, N), commit, glue, None
@@ -538,10 +607,11 @@ class VectorQuantize(nn.Module):
         if mask is not None:
             if self.learnable_codebook:
                 _unsupported("mask / lens with a learnable codebook")
+            if self.directional_reparam and x.requires_grad and torch.is_grad_enabled():
+                # the masked estimators are the rotation trick and straight-through; DiVeQ's is not among them
+                _unsupported("mask / lens with directional_reparam on inputs that require grad")
             if self.has_projections or self.accept_image_fmap or self.accept_3d_fmap or not self.channel_last or self.heads > 1:
                 _unsupported("mask / lens together with projections, feature-map layouts or heads > 1")
-            if x.requires_grad and torch.is_grad_enabled():
-                _unsupported("mask / lens on inputs that require grad")
         elif topk is not None or codebook_transform_fn is not None:
             _unsupported("topk / codebook_transform_fn")
         if not x.is_cuda:
@@ -574,7 +644,8 @@ class VectorQuantize(nn.Module):
         fused_loss = want_loss and not input_requires_grad
         # the kernels return weight * mse already rounded like F.mse_loss in x.dtype (vqp:1327-1329); LossBreakdown.commitment
         # is the UNweighted mse: ask them for weight 1 then
-        split_weight = fused_loss and return_loss_breakdown and self.commitment_weight != 1.
+        # (a masked call always takes the kernels' loss, with or without gradients)
+        split_weight = (fused_loss or (want_loss and mask is not None)) and return_loss_breakdown and self.commitment_weight != 1.
         update = cbk.updates(training, freeze_codebook, ema_update)
         loss_weight = 1. if split_weight else self.commitment_weight
         if mask is not None:
@@ -613,8 +684,8 @@ class VectorQuantize(nn.Module):
         if training:
             if want_loss and not fused:
                 loss = loss + commit * self.commitment_weight
-            # ---- gradient estimator (vqp:1225-1237)
-            if input_requires_grad and self.route_gradients_to_input:
+            # ---- gradient estimator (vqp:1225-1237); a masked call ran it on its live rows already
+            if input_requires_grad and self.route_gradients_to_input and mask is None:
                 x_t = cbk.transform_input(x)
                 if self.rotation_trick:
                     quantize = rotate_to(x_t, quantize)
