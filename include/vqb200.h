@@ -521,6 +521,30 @@ int vqb_hvq_blend_backward(const float* g_recon, const float* g_resid, int64_t n
 int vqb_rpq_norm_project(const float* x, int64_t N, int dim, const float* proj, int H, int E, int norm, float* rows,
                          void* stream);
 
+/* LatentQuantize (latent_quantization.py "lq").  Tables: at most VQB_LQ_MAX_DIM latents and VQB_LQ_MAX_VALUES values in all,
+ * staged in shared memory (VQB_E_UNSUPPORTED beyond). */
+#define VQB_LQ_MAX_DIM 256
+#define VQB_LQ_MAX_VALUES 8192
+#define VQB_LQ_MAX_LOSS_BLOCKS 1024
+/* z [N][C][D] contiguous in dtype (f32 or bf16), C codebooks sharing the D per-latent tables.  vals f32 [total]: the D tables
+ * concatenated (any order, duplicates allowed); meta i32 [3][D] on the device: table lengths (summing to total), half widths
+ * levels // 2, basis.  Per latent the first j minimising |z - vals_i[j]| in fp32 (a NaN distance is the minimum, as
+ * torch.argmin), codes f32 [N][C][D] = z + (v - z), idx i32 [N][C] = int32(sum_i ((codes_i * 2) * hw_i + hw_i) * basis_i) in
+ * fp32, each operation rounded separately, the sum left to right, truncated by cvt.rzi (NaN -> 0, saturating). */
+int vqb_lq_quantize(const void* z, int dtype, int64_t N, int C, int D, const float* vals, int total, const int32_t* meta,
+                    float* codes, int32_t* idx, void* stream);
+/* The CTA count of vqb_lq_loss over n elements (the length of its partial array), or a VQB_E_* code.  Host-only. */
+int vqb_lq_loss_blocks(int64_t n);
+/* loss f32 [1] = w_c m_c + w_q m_q, m = mean over n of (x - out)^2 (x f32 or bf16, out f32, the same element order), a term's
+ * m replaced by 0 unless its flag use_c / use_q (0 / 1) is set.  w_c, w_q: f32 [1] on the device.  partial f64 [blocks],
+ * blocks = vqb_lq_loss_blocks(n).  Two launches, fp64 partials added in a fixed order, no atomics. */
+int vqb_lq_loss(const void* x, int dtype, const float* out, int64_t n, const float* wc, const float* wq, int use_c, int use_q,
+                double* partial, int blocks, float* loss, void* stream);
+/* The loss's gradients for g_loss f32 [1] on the device: gx [n] in x's dtype = (2/n) (x - out) (w_q g) (0 without use_q) and
+ * gout f32 [n] = (2/n) (out - x) (w_c g) (0 without use_c); either output may be NULL, not both.  One launch. */
+int vqb_lq_loss_backward(const void* x, int dtype, const float* out, int64_t n, const float* g_loss, const float* wc,
+                         const float* wq, int use_c, int use_q, void* gx, float* gout, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -13,6 +13,7 @@ _i32, _i64, _f32, _f64, _vp, _sz = _c.c_int, _c.c_int64, _c.c_float, _c.c_double
 
 DTYPE_F32, DTYPE_BF16 = 0, 1
 METRIC_EUCLID, METRIC_COSINE = 0, 1
+VQB_LQ_MAX_DIM, VQB_LQ_MAX_VALUES = 256, 8192   # LatentQuantize's table cap (include/vqb200.h)
 
 class FusedOutputs(ctypes.Structure):
     """Mirror of `vqb_fused_outputs` (include/vqb200.h)."""
@@ -135,6 +136,10 @@ SIGNATURES = {
     "vqb_hvq_blend_update": (_i32, [_vp, _vp, _i64, _f64, _vp, _vp, _vp, _vp, _vp]),
     "vqb_hvq_blend_backward": (_i32, [_vp, _vp, _i64, _f64, _vp, _vp, _vp]),
     "vqb_rpq_norm_project": (_i32, [_vp, _i64, _i32, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "vqb_lq_quantize": (_i32, [_vp, _i32, _i64, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "vqb_lq_loss_blocks": (_i32, [_i64]),
+    "vqb_lq_loss": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _i32, _i32, _vp, _i32, _vp, _vp]),
+    "vqb_lq_loss_backward": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
 }
 
 

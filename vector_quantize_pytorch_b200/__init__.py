@@ -5,7 +5,8 @@ Drop-in for ONE path of lucidrains/vector-quantize-pytorch: `VectorQuantize`, `R
 `ResidualSimVQ`, finite scalar quantization (`FSQ`, `ResidualFSQ`, `GroupedResidualFSQ`),
 lookup-free quantization (`LFQ`, `ResidualLFQ`, `GroupedResidualLFQ`), finite scalar perturbation (`FSP`)
 the binary mapper (`BinaryMapper`), multi-scale residual VQ over feature maps (`HierarchicalVQ`), the BEST-RQ random-projection
-quantizer (`RandomProjectionQuantizer`) and the one-quantizer container `Sequential`.
+quantizer (`RandomProjectionQuantizer`), latent quantization (`LatentQuantize`) and the one-quantizer container
+`Sequential`.
 The hot path is hand-written CUDA (wgmma / TMA / mbarrier) in `csrc/`, bound through the C ABI in
 `include/vqb200.h`.  No Triton, no CPU fallback.
 """
@@ -22,9 +23,10 @@ from .fsp import FSP  # noqa: E402
 from .binary_mapper import BinaryMapper  # noqa: E402
 from .hierarchical_vq import HierarchicalVQ  # noqa: E402
 from .random_projection_quantizer import RandomProjectionQuantizer  # noqa: E402
+from .latent_quantize import LatentQuantize  # noqa: E402
 from .utils import Sequential  # noqa: E402
 
 __all__ = ["Codebook", "EuclideanCodebook", "CosineSimCodebook", "VectorQuantize", "ResidualVQ", "GroupedResidualVQ", "SimVQ",
            "ResidualSimVQ", "FSQ", "ResidualFSQ", "GroupedResidualFSQ",
            "LFQ", "ResidualLFQ", "GroupedResidualLFQ", "FSP", "BinaryMapper", "HierarchicalVQ",
-           "RandomProjectionQuantizer", "Sequential"]
+           "RandomProjectionQuantizer", "LatentQuantize", "Sequential"]

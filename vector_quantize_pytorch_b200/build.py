@@ -11,7 +11,7 @@ import sys
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libvqb200.so")
-SOURCES = ["vq_assign.cu", "vq_aux.cu", "vq_ema.cu", "vq_forward.cu", "vq_peer.cu", "vq_rsimvq.cu", "vq_diveq.cu", "vq_fsq.cu", "vq_lfq.cu", "vq_fsp.cu", "vq_binmap.cu", "vq_hvq.cu", "vq_rpq.cu"]
+SOURCES = ["vq_assign.cu", "vq_aux.cu", "vq_ema.cu", "vq_forward.cu", "vq_peer.cu", "vq_rsimvq.cu", "vq_diveq.cu", "vq_fsq.cu", "vq_lfq.cu", "vq_fsp.cu", "vq_binmap.cu", "vq_hvq.cu", "vq_rpq.cu", "vq_lq.cu"]
 HEADERS = ["ptx.cuh", "vqb_common.cuh", "code_operands.cuh", "gather_row.cuh", "epilogue.cuh", "row_io.cuh", os.path.join("..", "..", "include", "vqb200.h")]
 
 NVCC_FLAGS = [

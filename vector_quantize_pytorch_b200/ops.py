@@ -1046,3 +1046,67 @@ def rpq_norm_project(x: torch.Tensor, proj: torch.Tensor, norm: bool) -> torch.T
               "vqb_rpq_norm_project")
     _count(1)
     return rows
+
+
+# ---- LatentQuantize (csrc/vq_lq.cu) ----
+
+def lq_quantize(z: torch.Tensor, C: int, vals: torch.Tensor, meta: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """vqb_lq_quantize: z (N, C * D) fp32 / bf16 -> (codes (N, C * D) fp32, indices (N, C) int32).  vals: the D value tables
+    concatenated, fp32; meta (3, D) int32: table lengths, half widths, basis; both on z's device."""
+    z = float_input(z, "LatentQuantize")
+    _require_cuda(vals, meta)
+    N, CD = z.shape
+    D = CD // C
+    codes = torch.empty((N, CD), dtype=torch.float32, device=z.device)
+    idx = torch.empty((N, C), dtype=torch.int32, device=z.device)
+    if N == 0:
+        return codes, idx
+    with torch.cuda.device(z.device):
+        check(lib.vqb_lq_quantize(_p(z), _dtype_code(z), N, C, D, _p(vals), vals.numel(), _p(meta), _p(codes), _p(idx),
+                                  _stream()), "vqb_lq_quantize")
+    _count(1)
+    return codes, idx
+
+
+def _lq_loss_operands(x, out, wc, wq):
+    """The loss kernels' operands: x fp32 / bf16 and out fp32, contiguous, of one size; wc, wq one-element fp32 tensors; all on
+    one CUDA device (TypeError / ValueError / RuntimeError otherwise)."""
+    if x.dtype not in FLOAT_DTYPES or out.dtype != torch.float32 or wc.dtype != torch.float32 or wq.dtype != torch.float32:
+        raise TypeError(f"vqb200 LatentQuantize loss takes fp32 / bf16 x and fp32 out and weights, got {x.dtype}, {out.dtype}, "
+                        f"{wc.dtype}, {wq.dtype}")
+    if x.numel() != out.numel() or wc.numel() != 1 or wq.numel() != 1 or not (x.is_contiguous() and out.is_contiguous()):
+        raise ValueError("vqb200 LatentQuantize loss: x and out contiguous of one size, one-element weights")
+    _require_cuda(x, out, wc, wq)
+    if len({t.device for t in (x, out, wc, wq)}) != 1:
+        raise RuntimeError("vqb200 LatentQuantize loss: operands on different devices")
+
+
+def lq_loss(x: torch.Tensor, out: torch.Tensor, wc: torch.Tensor, wq: torch.Tensor, use_c: bool, use_q: bool) -> torch.Tensor:
+    """vqb_lq_loss: w_c mse + w_q mse of x (fp32 / bf16) and out (fp32), contiguous and of the same shape, as an fp32 scalar; a
+    term counts only when its host flag is set.  wc, wq: fp32 scalars on the device."""
+    _lq_loss_operands(x, out, wc, wq)
+    n = x.numel()
+    loss = torch.empty((), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        blocks = _queried(lib.vqb_lq_loss_blocks(n), "vqb_lq_loss_blocks")
+        partial = torch.empty(blocks, dtype=torch.float64, device=x.device)
+        check(lib.vqb_lq_loss(_p(x), _dtype_code(x), _p(out), n, _p(wc), _p(wq), int(use_c), int(use_q), _p(partial), blocks,
+                              _p(loss), _stream()), "vqb_lq_loss")
+    _count(2)
+    return loss
+
+
+def lq_loss_backward(x: torch.Tensor, out: torch.Tensor, g_loss: torch.Tensor, wc: torch.Tensor, wq: torch.Tensor, use_c: bool,
+                     use_q: bool, want_gx: bool = True, want_gout: bool = True):
+    """vqb_lq_loss_backward: (d x in x's dtype or None, d out fp32 or None) of lq_loss for dL/dloss g_loss (fp32 scalar on the
+    device)."""
+    _lq_loss_operands(x, out, wc, wq)
+    _require_cuda(g_loss)
+    gx = torch.empty_like(x) if want_gx else None
+    gout = torch.empty_like(out) if want_gout else None
+    g_loss = g_loss.float().contiguous()
+    with torch.cuda.device(x.device):
+        check(lib.vqb_lq_loss_backward(_p(x), _dtype_code(x), _p(out), x.numel(), _p(g_loss), _p(wc), _p(wq), int(use_c),
+                                       int(use_q), _p(gx), _p(gout), _stream()), "vqb_lq_loss_backward")
+    _count(1)
+    return gx, gout

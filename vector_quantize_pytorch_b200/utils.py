@@ -1,7 +1,7 @@
 """`Sequential`: plain modules around exactly one quantizer of this package, called in order, with the quantizer's extra
 outputs returned after the last module's output (the reference's utils.Sequential).  `QUANTIZE_KLASSES` is what counts as
-a quantizer: every quantizer of the reference that this package has (not `LatentQuantize`); `BinaryMapper` is not one, as
-in the reference."""
+a quantizer: every quantizer of the reference that this package has except `LatentQuantize`, which it does not accept (yet);
+`BinaryMapper` is not one, as in the reference."""
 from torch import nn
 
 from .fsp import FSP
